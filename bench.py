@@ -8,7 +8,9 @@ One "step" = everything a reference session.run(train_tensor) computes (16 netwo
 generator-set and discriminator-set gradients) plus BOTH Adam applies (SURVEY 8d, "mode B").
 `value` = (source,target) pairs per second over all ranks with inputs resident in HBM; `e2e` = the same through
 the public API (GanModel.train_step) with pinned-host inputs copied H2D and the losses read back D2H every step.
-Prints ONE JSON line on rank 0.
+Prints ONE JSON line on rank 0.  `--dump-outputs DIR` also writes what the last timed step computed (the losses, and a
+fixed sample of the gradient and of the updated variables) as DIR/<name>.npy, so that two builds can be compared output
+for output on identical seeded inputs.
 """
 from __future__ import annotations
 
@@ -43,11 +45,41 @@ def _peaks():
               'which': 'measured'}
     except (OSError, ValueError, KeyError, TypeError):
       pass
-  return {'hbm_gbs': 6650.0, 'tf': 1400.0, 'which': 'fallback'}
+  # NVIDIA H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense BF16 989 TFLOP/s -- not reached figures
+  return {'hbm_gbs': 3350.0, 'tf': 989.0, 'which': 'H100 SXM data sheet'}
+
+
+def gpu_info(index=0):
+  """Card name and power limit, reported beside every number measured on it."""
+  info = {'name': torch.cuda.get_device_name(index), 'power_limit_w': None, 'sm_count':
+          torch.cuda.get_device_properties(index).multi_processor_count}
+  try:
+    out = subprocess.run(['nvidia-smi', '-i', str(index), '--query-gpu=power.limit', '--format=csv,noheader,nounits'],
+                         capture_output=True, text=True, timeout=10).stdout.strip()
+    info['power_limit_w'] = float(out)
+  except (OSError, ValueError, subprocess.SubprocessError):
+    pass
+  return info
+
+
+DUMP_SAMPLE = 1 << 22     # elements kept of a larger output (16 MB of float32): four outputs stay well under 64 MB
+
+
+def dump_outputs(out_dir, arrays):
+  """Writes each named tensor as out_dir/<name>.npy in float32; a tensor larger than DUMP_SAMPLE elements is replaced by
+  a fixed, seeded sample of its flattened elements (the same indices on every run)."""
+  import numpy as np
+  os.makedirs(out_dir, exist_ok=True)
+  for name, t in arrays.items():
+    a = t.detach().float().cpu().reshape(-1).numpy()
+    if a.size > DUMP_SAMPLE:
+      idx = np.sort(np.random.default_rng(0).choice(a.size, DUMP_SAMPLE, replace=False))
+      a = a[idx]
+    np.save(os.path.join(out_dir, name + '.npy'), a)
 
 
 class ClockSampler(threading.Thread):
-  """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+  """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
   def __init__(self, index=0):
     super().__init__(daemon=True)
@@ -114,10 +146,6 @@ def bench_cuda(args):
       dist.barrier()
     torch.cuda.synchronize()
 
-  for kv in args.set_option:
-    from twingan_b200._lib import lib as _twg_lib
-    key, value = kv.split('=')
-    _twg_lib().call('twg_set_option', int(key), int(value))
   ddp_check = None
   if world > 1 and not args.no_ddp_check:
     # pre-flight: N NCCL ranks == N sequential micro-batches through the product, parameters identical across ranks
@@ -160,12 +188,16 @@ def bench_cuda(args):
   launches0 = L.launch_count()
   e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
   e0.record()
+  last = None
   for i in range(args.steps):
-    step_resident(i)
+    last = step_resident(i)
   e1.record()
   barrier()
   launches = (L.launch_count() - launches0) if not use_graph else model.launches_per_step * args.steps
   ms = e0.elapsed_time(e1)
+  if args.dump_outputs and rank == 0 and last is not None:
+    dump_outputs(args.dump_outputs, {'g_loss': last[0], 'd_loss': last[1], 'gradient': model.flat_grad,
+                                     'variables': model.variables.flat})
   # e2e leg
   step_e2e(0)
   barrier()
@@ -201,42 +233,31 @@ def bench_cuda(args):
                                          max_num_channels=args.max_channels)
     # Per-family detail comes from one eager pass with CUDA events around every conv launch; events serialise the launches
     # and add their own latency, so the family times sum to MORE than the graph-replayed step -- use them as shares.
-    KERNELS = {'tc_tap': 'k_conv_htap_tc<BN> (persistent wide-layer halo kernel) + k_conv_fwd_tc<CC,BN> (tap-per-TMA, hw < 16): '
-                         'fwd+dgrad of the wide layers',
-               'tc_halo': 'k_conv_halo_tc<CIN,BN,SUB> (halo-tile persistent implicit GEMM, fwd+dgrad of the 16-64-channel layers)',
-               'tc_wgrad': 'k_conv_wgrad_rows<CN,BNW> (row-shift, narrow layers) + k_conv_wgrad_halo<CN,BNW> (W >= 16) + '
-                           'k_conv_wgrad_tc2<CN,BNW> (4x4 / 8x8): weight gradients',
+    KERNELS = {'tc_fwd': 'k_conv_fwd_wgmma<CC,BN> (implicit GEMM, wgmma + TMA): fwd+dgrad of the 3x3 / 1x1 layers',
+               'tc_wgrad': 'k_conv_wgrad_wgmma<CN,BNW> (tap-stacked implicit GEMM, wgmma + TMA): weight gradients',
                'fp32_cuda_core': 'k_conv_*_simt (exact fp32 CUDA-core convs: 4x4 VALID head, FC, non-tensor-core shapes)',
                'tc_ws': 'k_pw_* (fromRGB / toRGB 1x1 convs, exact fp32)'}
     families = {}
-    for k in ('tc_tap', 'tc_wgrad', 'tc_halo', 'tc_ws', 'fp32_cuda_core'):
+    for k in ('tc_fwd', 'tc_wgrad', 'tc_ws', 'fp32_cuda_core'):
       v = conv_stats.get(k)
       if v:
         families[k] = {'kernel': KERNELS[k], 'launches_per_step': v['launches'], 'ms_eager_events': v['ms'],
                        'algorithmic_tflops': v['tflops'], 'frac_of_bf16_peak': round(v['tflops'] / peaks['tf'], 5),
                        'algorithmic_gbs': v.get('algorithmic_gbs'),
-                       'frac_of_measured_hbm': round(v.get('algorithmic_gbs', 0.0) / peaks['hbm_gbs'], 4)}
+                       'frac_of_hbm_peak': round(v.get('algorithmic_gbs', 0.0) / peaks['hbm_gbs'], 4)}
     conv_ms = sum(v['ms'] for v in conv_stats.values())
     conv_fl = sum(v['flops'] for v in conv_stats.values())
     step_tf = step_flop / (per_step * 1e-3) / 1e12
-    traffic, traffic_src = None, None
-    tpath = os.path.join(ROOT, 'profiles', 'r02_ncu_traffic.json')
-    if os.path.exists(tpath):
-      try:
-        tj = json.load(open(tpath))
-        traffic, traffic_src = tj.get('dominant_kernel_dram_bytes_per_launch'), tj
-      except (OSError, ValueError):
-        pass
     out = {
         'metric': METRIC, 'value': round(value, 3), 'unit': UNIT, 'n_gpus': world, 'steps': args.steps,
         'warmup': args.warmup, 'ms_per_step': round(per_step, 3), 'higher_is_better': True, 'scaling': 'weak',
-        'vs_baseline': None, 'dtype': 'f32 (conv MACs as split-bf16 x3 on tcgen05, fp32 accumulate)',
-        'data': 'synthetic',
+        'vs_baseline': None, 'dtype': 'f32 (conv MACs as split-bf16 x3 on wgmma, fp32 accumulate)',
+        'data': 'synthetic', 'gpu': gpu_info(local),
         'config': {'workload': 'configs[3]: %dx%d full TwinGAN G+D step (mode B: 16 passes + 2 DRAGAN, both gradient '
                                'sets, both Adam applies), batch %d/GPU, %s, pixel-norm, UNet, DRAGAN' % (hw, hw, batch, args.norm),
                    'global_batch': batch * world, 'parallelism': 'dp%d' % world,
                    'l2': 'activation working set >> L2 (GBs per step); two alternating input sets',
-                   'conv_precision': 'tcgen05 split-bf16' if ops.get_precision() else 'fp32 CUDA cores',
+                   'conv_precision': 'wgmma split-bf16' if ops.get_precision() else 'fp32 CUDA cores',
                    'pass_structure': 'pass-by-pass (16 separate passes)' if args.pass_by_pass else
                                      'weight-sharing passes batched: E 2x16, G 4x16, E 2x16, D 3x16 per domain, DRAGAN 16+16',
                    'images_per_pair': 2, 'cuda_graph': use_graph},
@@ -247,19 +268,18 @@ def bench_cuda(args):
         # whole G+D step over the step time, against the measured dense bf16 peak.
         'roofline': {
             'bound': 'tensor', 'achieved': round(step_tf, 3), 'peak': peaks['tf'], 'unit': 'TFLOP/s',
-            'frac': round(step_tf / peaks['tf'], 5), 'traffic': traffic,
+            'frac': round(step_tf / peaks['tf'], 5),
             'kernel': 'whole G+D step: %.3f TFLOP of algorithmic conv MACs (12 F_E + 12 F_G + 34 F_D per pair) in %.2f ms, %d '
                       'launches' % (step_flop / 1e12, per_step, int(launches) // max(args.steps, 1)),
             'ceiling': 'split-bf16 forms 3 partial products per MAC, so a tensor-bound layer caps at 0.333 of the bf16 peak; '
                        'every hw >= 64 layer is HBM-bound (SURVEY 8a.1), hence step_mixed_frac',
-            'peak_source': peaks['which'] + ' bf16 sustained (MEASURED_PEAKS.json)',
+            'peak_source': peaks['which'],
             'step_tc_frac': round(step_tf / peaks['tf'], 5),
             'step_mixed_frac': round(mixed['step'] / (per_step * 1e-3), 5),
             'step_mixed_bound_ms': round(mixed['step'] * 1e3, 3),
             'step_algorithmic_tflop': round(step_flop / 1e12, 4),
             'conv_family_tflops': round(conv_fl / max(conv_ms, 1e-9) / 1e9, 3), 'conv_family_ms_eager_events': round(conv_ms, 3),
             'families': families,
-            'traffic_source': traffic_src,
         },
     }
     if ddp_check is not None:
@@ -357,7 +377,7 @@ def infer_measure(args, dev, steps=None):
          'frac_of_bf16_peak': round(gflop * 1e9 * batch / (ms * 1e-3) / 1e12 / peaks['tf'], 5)}
   if alg_bytes:
     out['algorithmic_gbs'] = round(alg_bytes / (ms * 1e-3) / 1e9, 1)
-    out['frac_of_measured_hbm'] = round(alg_bytes / (ms * 1e-3) / 1e9 / peaks['hbm_gbs'], 4)
+    out['frac_of_hbm_peak'] = round(alg_bytes / (ms * 1e-3) / 1e9 / peaks['hbm_gbs'], 4)
     out['algorithmic_bytes'] = alg_bytes
   return out
 
@@ -371,8 +391,8 @@ def bench_infer(args):
   m = infer_measure(args, dev)
   sampler.stop_flag = True
   m.update({'n_gpus': 1, 'warmup': args.warmup, 'ms_per_step': m['latency_ms'], 'higher_is_better': True, 'scaling': 'weak',
-            'vs_baseline': None, 'dtype': 'f32 (conv MACs as split-bf16 x3 on tcgen05, fp32 accumulate)', 'data': 'synthetic',
-            'clocks': sampler.summary()})
+            'vs_baseline': None, 'dtype': 'f32 (conv MACs as split-bf16 x3 on wgmma, fp32 accumulate)', 'data': 'synthetic',
+            'gpu': gpu_info(dev.index or 0), 'clocks': sampler.summary()})
   print(json.dumps(m), flush=True)
 
 
@@ -503,9 +523,9 @@ def main():
   ap.add_argument('--no-graph', action='store_true', help='eager launches instead of CUDA-graph replay')
   ap.add_argument('--pass-by-pass', action='store_true',
                   help="A/B: run the reference's 16 separate network passes instead of batching the weight-sharing ones")
-  ap.add_argument('--set-option', action='append', default=[], metavar='KEY=VALUE',
-                  help='twg_set_option A/B switch applied before the run (e.g. 2=1: one sub-tile per halo tile)')
-  ap.add_argument('--profile-one-step', action='store_true', help='1 warm-up + 1 step only (for ncu launch lists)')
+  ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                  help='after the timed steps, write what the last one computed as DIR/<name>.npy (float32)')
+  ap.add_argument('--profile-one-step', action='store_true', help='1 warm-up + 1 step only (for a profiler launch list)')
   ap.add_argument('--no-secondary', action='store_true', help='skip the configs[4] inference measurement (secondary.infer)')
   ap.add_argument('--no-ddp-check', action='store_true', help='skip the data-parallel pre-flight at N > 1')
   args = ap.parse_args()

@@ -1,4 +1,4 @@
-/* twg.h -- C ABI of libtwg.so, the sm_100a kernel library behind twingan_b200.
+/* twg.h -- C ABI of libtwg.so, the sm_90a (H100) kernel library behind twingan_b200.
  *
  * Drop-in boundary (SURVEY.md 8b).  The reference (jerryli27/TwinGAN) has NO FFI: every FLOP of its
  * hot path runs inside TensorFlow-1.8 library kernels reached through the Python plug-in points
@@ -7,16 +7,18 @@
  *
  * Conventions
  *  - every pointer is a CUDA device pointer owned by the caller (twg_sum_scalars takes a HOST array of device
- *    pointers); the library never allocates or frees device memory.  Mutable global state: the thread-local
- *    last-error string, the launch counter, one-time kernel attribute set-up, and the process-wide tuning switches of
- *    twg_set_option (plain ints read at launch time -- set them before the first call from any thread);
- *  - every call takes a cudaStream_t (passed as void*), is asynchronous and graph-capturable; calls from several host
- *    threads are safe as long as twg_set_option is not called concurrently;
+ *    pointers); the library never allocates or frees device memory at run time.  Mutable global state: the thread-local
+ *    last-error string, the launch counter, one-time kernel attribute set-up, and one 32 MB device buffer per device
+ *    (allocated when the library loads) for the partial sums of cross-block reductions;
+ *  - results are bit-identical from run to run: reductions add their partial sums in a fixed order, never with fp32
+ *    atomics;
+ *  - every call takes a cudaStream_t (passed as void*), is asynchronous and graph-capturable.  Calls for one device must
+ *    be ordered on one stream (the partial-sum buffer is shared); calls from several host threads are safe when they are;
  *  - returns 0 on success, <0 on invalid argument / unsupported shape / CUDA error (see twg_last_error);
  *  - activations are NHWC fp32, conv weights HWIO fp32 ([kh][kw][Cin][Cout]), like the reference
  *    (libs/batch_norm.py:409; tf.contrib.layers.conv2d);
  *  - "rows" = N*H*W pixels, "C" = channels.
- *  - sm_100a only.  There is no CPU path.
+ *  - sm_90a only.  There is no CPU path.
  */
 #ifndef TWG_H_
 #define TWG_H_
@@ -53,7 +55,7 @@ int64_t twg_launch_count(void);
  *      tf.gradients-generated Conv2DBackpropInput / Conv2DBackpropFilter -------------------------------
  * Stride 1.  x:[N,H,W,Cin]  w:[k,k,Cin,Cout]  y:[N,Ho,Wo,Cout], Ho = H + 2*pad - k + 1.
  * SAME for k=3 is pad=1, k=1 pad=0; VALID is pad=0.
- * `prec`: 0 = fp32 CUDA-core path (always available), 1 = tcgen05 tensor-core path with split-bf16
+ * `prec`: 0 = fp32 CUDA-core path (always available), 1 = wgmma tensor-core path with split-bf16
  * (3 MMAs per product, ~fp32 accuracy); the tensor-core path returns TWG_ERR_UNSUPPORTED for shapes it
  * does not cover and the caller picks prec=0 for those.                                              */
 int twg_conv_fwd(const float* x, const float* w, float* y, int N, int H, int W, int Cin, int Cout, int k, int pad,
@@ -70,7 +72,7 @@ int64_t twg_conv_workspace_bytes(int N, int H, int W, int Cin, int Cout, int k, 
 /* ---- tensor-core convolution on pre-split operands ("split-bf16 planes": hi plane then lo plane, bf16, same
  *      NHWC element order as the fp32 tensor; x = hi + lo).  Lets the caller split an activation once and reuse
  *      it for forward + wgrad, a gradient once for dgrad + wgrad, and a weight once per optimiser step.        */
-/* 1 if the tcgen05 path covers this stride-1 conv shape (3x3 SAME / 1x1, channels multiple of 16), else 0 */
+/* 1 if the tensor-core path covers this stride-1 conv shape (3x3 SAME / 1x1, channels multiple of 16), else 0 */
 int twg_conv_tc_supported(int N, int H, int W, int Cin, int Cout, int k, int pad);
 /* planes: 2*n bf16 */
 int twg_split_act(const float* x, void* planes, int64_t n, twg_stream_t stream);
@@ -90,7 +92,7 @@ int twg_conv_bias_act_fwd_planes_mask(const void* x_planes, const void* w_planes
  * libs/batch_norm.py:266-278 turns the normaliser into the per-channel affine a = gamma / sqrt(moving_var + eps),
  * b = beta - moving_mean * a, twg_norm_eval_affine):  z = pixel_norm?(lrelu?(a[c] * conv(x, w) + b[c])), flags =
  * TWG_FLAG_LRELU | TWG_FLAG_PIXNORM, written as fp32 z and / or split planes (either may be NULL, not both).  Covered
- * shapes: twg_conv_has_act_mask(...) == 1 (the halo kernel: a thread holds all Cout channels of its pixel). */
+ * shapes: twg_conv_has_act_mask(...) == 1 (one output-channel block: a pixel's Cout channels sit in one CTA). */
 int twg_conv_affine_act_fwd_planes(const void* x_planes, const void* w_planes, const float* a, const float* b, int flags,
                                    float* z, void* z_planes, int N, int H, int W, int Cin, int Cout, int k, int pad,
                                    twg_stream_t stream);
@@ -112,23 +114,9 @@ int twg_conv_dgrad_planes(const void* gy_planes, const void* w_planes, float* gx
 int twg_conv_wgrad_planes(const void* x_planes, const void* gy_planes, float* gw, int N, int H, int W, int Cin,
                           int Cout, int k, int pad, int accumulate, twg_stream_t stream);
 
-/* tuning / A-B switches (process-wide, not part of the reference-facing surface):
- *   key 1 = use the halo-tile persistent kernel for small-channel 3x3 layers (default 1)
- *   key 2 = sub-tiles per halo tile: 0 = per-shape default, 1 / 2 / 4 force it (profiles/r01_halo_subtiles.txt)
- *   key 3 = stage the A operand in TMEM (TS-mode MMA) in the tap-per-TMA kernel (default 0; measured slower)
- *   key 4 = 2-CTA clusters with TMA-multicast weight tiles in the tap-per-TMA kernel (wide layers)
- *   key 6 = persistent halo-tile kernel for the wide 3x3 layers (Cin % 64 == 0, Cout >= 64, H, W >= 16; default 1)
- *   key 7 = halo weight-gradient kernel (x halo loaded once per pixel tile, taps as descriptor views; 3x3, W >= 16;
- *           default 1; 0 = tap-stacked kernel everywhere)
- *   key 8 = CTA-pair (tcgen05 cta_group::2) variant of the wide-layer halo kernel for Cout % 128 == 0 (default 0:
- *           measured slower than the single-CTA halo kernel, profiles/r02_conv_ab_cta_pair.txt)
- *   key 9 = row-shift weight-gradient kernel for the narrow 3x3 layers (Cin chunk 16/32, or 64 with Cout <= 32): the
- *           kh taps are rows of an interleaved gy box, so one MMA covers all nine taps (default 1; 0 = key 7's kernel) */
 /* host utility (no GPU): CRC-32C (Castagnoli) of `n` bytes continuing from `crc` (0 to start) -- the checksum of
  * TensorFlow's checkpoint format (twingan_b200/tf_checkpoint.py) */
 int64_t twg_crc32c(const void* data, int64_t n, int64_t crc);
-
-int twg_set_option(int key, int value);
 
 /* ---- normaliser + activation + pixel-norm: replaces tf.nn.moments/tf.nn.batch_normalization
  *      (libs/batch_norm.py:430,470; libs/instance_norm.py:131-135), tf.maximum(0.2x,x) (util_misc.py:86)

@@ -6,11 +6,11 @@ the CUDA path: only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s
 ``cpu_baseline`` / ``--impl reference`` legs may import it.  The product package
 ``twingan_b200`` never imports anything under ``oracle/``.
 
-PINNING (what this restatement has been held to, and what it has not).  The reference (/root/reference,
+PINNING (what this restatement has been held to, and what it has not).  The reference (
 jerryli27/TwinGAN @4e55934) is Python-2 + tensorflow==1.8, cannot be run as shipped in this container, and ships no
 test or golden vector for nets/pggan.py, nets/pggan_utils.py, libs/*, twingan.py or image_generation.py
 (SURVEY.md section 4, 8c).  What is pinned, by tests/test_cpu_reference_golden.py against
-tests/golden/reference_pggan.npz: the reference's OWN code -- nets/pggan.py, nets/pggan_utils.py, libs/batch_norm.py,
+tests/golden/reference_pggan_*.npz: the reference's OWN code -- nets/pggan.py, nets/pggan_utils.py, libs/batch_norm.py,
 libs/instance_norm.py, util_misc.fp16_friendly_leaky_relu, and the method sources of twingan.GanModel._clone_fn /
 add_loss, image_generation.GanModel.add_gan_loss / _add_dragan_loss / get_perturbed_batch / get_growing_image and
 deployment/model_deploy.py (two clones) --
@@ -727,7 +727,7 @@ def apply_stat_updates(cfg: Config, norm_state: Dict[str, Tensor], nets: Nets) -
   the 2-3 passes that share one `_s`/`_t` variable undefined; SURVEY 8a.4-7)."""
   for base, d, upd in nets.stat_updates:
     # batch_renorm passes decay=0.99 (nets/pggan_utils.py:165); plain batch_norm passes none and gets
-    # conditional_batch_norm's default 0.999 (libs/batch_norm.py:44) -- pinned by tests/golden/reference_pggan.npz
+    # conditional_batch_norm's default 0.999 (libs/batch_norm.py:44) -- pinned by tests/golden/reference_pggan_*.npz
     decay = 0.99 if 'stddev' in upd else 0.999
     if 'stddev' in upd:
       for var, wname, val in (('renorm_mean', 'renorm_mean_weight', upd['mean']),

@@ -1,17 +1,17 @@
 """Golden vectors produced by THE REFERENCE'S OWN network code.
 
-Runs /root/reference/nets/pggan.py (+ nets/pggan_utils.py, libs/batch_norm.py, libs/instance_norm.py and the leaky-ReLU
+Runs the reference's nets/pggan.py (+ nets/pggan_utils.py, libs/batch_norm.py, libs/instance_norm.py and the leaky-ReLU
 of util_misc.py:68-86) under tests/golden/tf18_shim.py -- a torch-backed stand-in for the few dozen TensorFlow-1.8 API
 entry points those files use -- with the wiring of twingan.py:196-270,370-373 (scopes `encoder_content`, `generator`,
 `discriminator_s`; per-domain `_s` / `_t` normaliser postfixes; UNet end points), and stores inputs, every variable the
 reference created (under the name the reference gave it), outputs, end points, gradients and the normaliser state after
-the pass in tests/golden/reference_pggan.npz.
+the pass in tests/golden/reference_pggan_*.npz.
 
-Only runnable where /root/reference exists (this authoring container); the .npz travels.  tests/test_cpu_reference_golden.py
-then holds oracle/twingan_oracle.py to these vectors.  What this does and does not pin is stated at the top of
+Needs a checkout of the reference (--reference DIR); the stored vectors are all the tests need.
+tests/test_cpu_reference_golden.py then holds oracle/twingan_oracle.py to these vectors.  What this does and does not pin is stated at the top of
 tf18_shim.py.
 
-  python tests/golden/make_reference_golden.py [--reference /root/reference]
+  python tests/golden/make_reference_golden.py --reference DIR
 """
 from __future__ import annotations
 
@@ -30,6 +30,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 import tf18_shim as tfs  # noqa: E402
 from golden_provider import stable_hash_provider  # noqa: E402
+import npz_parts  # noqa: E402
 
 CASES = [
     # name, hw, is_growing, alpha, max channels, norm type, batch, global_step, store values?
@@ -229,7 +230,7 @@ def build_reference_ganmodel(ref_root, tf, pggan):
 
 
 # SURVEY 8f-4: optional flags on the same wiring -- loss architectures (image_generation.py:330-389, 414-439) and the
-# equalized learning rate (nets/pggan_utils.py:236-254); written to reference_f4.npz by `--f4`
+# equalized learning rate (nets/pggan_utils.py:236-254); written to reference_f4_*.npz by `--f4`
 F4_CLONE_CASES = [
     ('f4_wgan_gp8', 8, False, 0, 1000, 16, 'instance_norm', 3,
      dict(loss_architecture='wgan_gp', gradient_penalty_lambda=10.0, wgan_drift_loss_weight=0.1)),
@@ -466,9 +467,9 @@ def reference_stage_loop(ref_root, tf, flag_values):
 
 def main():
   ap = argparse.ArgumentParser()
-  ap.add_argument('--reference', default='/root/reference')
-  ap.add_argument('--out', default=os.path.join(HERE, 'reference_pggan.npz'))
-  ap.add_argument('--f4', action='store_true', help='only the SURVEY 8f-4 optional-flag cases -> reference_f4.npz')
+  ap.add_argument('--reference', required=True, help='checkout of the reference project')
+  ap.add_argument('--out', default=os.path.join(HERE, 'reference_pggan'), help='path stem of the parts')
+  ap.add_argument('--f4', action='store_true', help='only the SURVEY 8f-4 optional-flag cases -> reference_f4_*.npz')
   args = ap.parse_args()
   tf, pggan, pggan_utils = load_reference(args.reference)
   out = {}
@@ -476,9 +477,9 @@ def main():
     GanModel, ns = build_reference_ganmodel(args.reference, tf, pggan)
     for case in F4_CLONE_CASES:
       run_clone_case(tf, pggan, GanModel, ns, case, out)
-    path = os.path.join(os.path.dirname(args.out), 'reference_f4.npz')
-    np.savez_compressed(path, **out)
-    print('wrote %s (%.1f MB, %d arrays)' % (path, os.path.getsize(path) / 1e6, len(out)))
+    stem = os.path.join(os.path.dirname(args.out), 'reference_f4')
+    npz_parts.save(stem, out)
+    print('wrote %s_*.npz (%d arrays)' % (stem, len(out)))
     return
   for case in CASES:
     run_case(tf, pggan, pggan_utils, case, out)
@@ -486,7 +487,7 @@ def main():
   for case in CLONE_CASES:
     run_clone_case(tf, pggan, GanModel, ns, case, out)
   run_deploy_case(tf, pggan, GanModel, ns, out)
-  np.savez_compressed(args.out, **out)
+  npz_parts.save(args.out, out)
   import json
   meta = {'flag_defaults': reference_flag_defaults(args.reference)}
   for tag, fl in (('default', dict(train_dir='/ckpt', is_training=True, do_export=False, program_name='twingan',
@@ -501,7 +502,7 @@ def main():
   json.dump(meta, open(jpath, 'w'), indent=1, sort_keys=True, default=str)
   print('wrote %s (%d flag defaults, %d + %d stages)' % (jpath, len(meta['flag_defaults']), len(meta['stages_default']),
                                                         len(meta['stages_small'])))
-  print('wrote %s (%.1f MB, %d arrays)' % (args.out, os.path.getsize(args.out) / 1e6, len(out)))
+  print('wrote %s_*.npz (%d arrays)' % (args.out, len(out)))
 
 
 if __name__ == '__main__':

@@ -1,6 +1,6 @@
 """The oracle against golden vectors produced by THE REFERENCE'S OWN CODE.
 
-tests/golden/reference_pggan.npz was written by tests/golden/make_reference_golden.py, which executes the reference's
+tests/golden/reference_pggan_*.npz were written by tests/golden/make_reference_golden.py, which executes the reference's
 nets/pggan.py, nets/pggan_utils.py, libs/batch_norm.py, libs/instance_norm.py and its leaky-ReLU (util_misc.py:68-86)
 under a torch-backed stand-in for the TensorFlow-1.8 API (tests/golden/tf18_shim.py), wired like twingan.py:196-270.
 That pins, against reference code rather than against a second reading of it: variable names and shapes (at the training
@@ -20,16 +20,17 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, 'golden'))
 from golden_provider import stable_hash_provider  # noqa: E402
+import npz_parts  # noqa: E402
 from oracle import twingan_oracle as O  # noqa: E402
 
-GOLDEN = os.path.join(HERE, 'golden', 'reference_pggan.npz')
+GOLDEN = os.path.join(HERE, 'golden', 'reference_pggan')
 VALUE_CASES = ['in16', 'in16grow', 'renorm8grow', 'bn8', 'in4']
 NAME_CASES = ['full256', 'full128grow']
 
 
 @pytest.fixture(scope='module')
 def golden():
-  return np.load(GOLDEN)
+  return npz_parts.load(GOLDEN)
 
 
 def _cfg(z, case):
@@ -165,7 +166,7 @@ F4_CASES = ['f4_wgan_gp8', 'f4_wgan8', 'f4_hinge16grow', 'f4_gan8', 'f4_eqlr_dra
 
 @pytest.fixture(scope='module')
 def golden_f4():
-  return np.load(os.path.join(HERE, 'golden', 'reference_f4.npz'))
+  return npz_parts.load(os.path.join(HERE, 'golden', 'reference_f4'))
 
 
 @pytest.mark.parametrize('case', F4_CASES)

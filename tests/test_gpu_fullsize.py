@@ -18,7 +18,7 @@ from tests.parity import _log_result
 pytestmark = pytest.mark.gpu
 
 DEV = 'cuda:0'
-# the full-resolution layers of the 256^2 stage at 16 images (SURVEY 8a.1): halo kernel, tap kernel, both wgrad variants
+# the full-resolution layers of the 256^2 stage at 16 images (SURVEY 8a.1): narrow, wide and mixed channel counts
 FULL_SHAPES = [
     (16, 256, 256, 16, 16),    # E/D block256 conv1
     (16, 256, 256, 16, 32),    # E/D block256 conv2
@@ -157,7 +157,7 @@ def test_batched_passes_equal_the_reference_pass_structure_at_full_size(built_li
   Gradients of this network are only reproducible to ~1e-2 (L2) from one run to the next of the SAME code: split-K
   convolutions and wgrad use fp32 atomics (summation order varies), instance norm with eps 1e-6 amplifies that to ~3e-5
   in the forward tensors, and a few of the 1.6e9 leaky-ReLU pre-activations land on the other side of their kink
-  (measured: gpurun_out/r2_noise.log; the oracle tests transfer the active set, two 16 GB device runs cannot).  So the
+  (measured; the oracle tests transfer the active set, two 16 GB device runs cannot).  So the
   pass-by-pass step is run twice: its distance to itself is the noise floor the batched step is held to."""
   from twingan_b200 import ops, twingan
   ops.set_precision(1)

@@ -34,7 +34,7 @@ CONV_SHAPES = [
     (4, 1, 1, 256, 1, 1, 0),      # FC as 1x1
     (1, 32, 32, 128, 128, 3, 1),
     (2, 16, 16, 512, 256, 3, 1),  # UNet-concat width
-    (12, 32, 32, 64, 128, 3, 1),  # wide-layer halo kernel (>= 96 tile items), BN = 128
+    (12, 32, 32, 64, 128, 3, 1),  # wide layer, BN = 128
     (4, 40, 36, 128, 256, 3, 1),  # same, ragged tiles, two Cout blocks, two Cin chunks
     (3, 64, 64, 64, 64, 3, 1),    # same, BN = 64
     (2, 32, 32, 32, 64, 3, 1),    # row-box weight gradient (16/32-channel layers, W >= 16)
@@ -235,8 +235,8 @@ def test_baseline_config2_fused_layer_family(built_lib, cout, prec):
   step 0) with leaky-ReLU and pixel-norm, forward + backward with upstream gradient ~ N(0,1), seeds 0/1/2, against the
   fp64 oracle cast to fp32: 1e-3 relative (inf-norm over inf-norm) on every tensor, and per element on the forward
   output with rtol 1e-3 / atol 1e-5 -- met by every element on the exact-fp32 path (prec 0).  The split-bf16 tensor-core
-  path (prec 1) carries ~5e-6 relative error per product, i.e. absolute errors up to ~5e-5 on O(1) outputs: measured on
-  a B200, 1.0e-4 of the elements exceed atol 1e-5 and the worst is 5.4e-5 (6e-6 of max|z|); the test bounds that tail
+  path (prec 1) carries ~5e-6 relative error per product, i.e. absolute errors up to ~5e-5 on O(1) outputs: a small
+  fraction of the elements exceeds atol 1e-5 (worst ~5e-5, ~6e-6 of max|z|); the test bounds that tail
   (fraction <= 1e-3, worst <= 2e-4) instead of pretending it is not there.  The leaky-ReLU active set is
   transferred like in the whole-step tests (DESIGN.md 4, kinks)."""
   from twingan_b200 import ops
@@ -529,42 +529,38 @@ def test_batched_wiring_ops(built_lib):
   assert rel_err(r, torch.cat([e, e]).detach()) == 0 and rel_err(ge, gr[:3] + gr[3:]) < 1e-6
 
 
-def test_wide_halo_kernel_matches_the_tap_kernel_and_fuses_the_discriminator_epilogue(built_lib):
-  """twg_set_option(6, .) A/B: the persistent wide-layer halo kernel against the tap-per-TMA kernel on the same operands
-  (forward, dgrad, and the fused bias + leaky-ReLU + split-plane epilogue of the discriminator layers)."""
+def test_wide_conv_and_fused_discriminator_epilogue(built_lib):
+  """A wide layer (128 -> 128 channels) on the tensor-core path: forward, dgrad, and the fused bias + leaky-ReLU +
+  split-plane epilogue of the discriminator layers, against the fp64 convolution."""
   from twingan_b200 import ops
-  L = built_lib
   ops.set_precision(1)
   N, H, W, Ci, Co = 16, 32, 32, 128, 128          # >= 16384 pixels: the fused discriminator epilogue is used
   x = _dev(_rand((N, H, W, Ci), 101))
   w = _dev(_rand((3, 3, Ci, Co), 102, 0.05))
   b = _dev(_rand((Co,), 103, 0.1))
   gy = _dev(_rand((N, H, W, Co), 104))
-  res = {}
-  for opt in (1, 0):
-    L.call('twg_set_option', 6, opt)
-    y = ops.conv_fwd_raw(x, w, 3, 1)
-    gx = ops.conv_dgrad_raw(gy, w, (N, H, W, Ci), 3, 1)
-    z = ops.conv_bias_act(x, w, b, 1, True, 'D', emit_planes=True)
-    zp = ops._take_planes(z)
-    res[opt] = (y, gx, z.detach(), zp.float().sum(0))
-  L.call('twg_set_option', 6, 1)
+  y = ops.conv_fwd_raw(x, w, 3, 1)
+  gx = ops.conv_dgrad_raw(gy, w, (N, H, W, Ci), 3, 1)
+  z = ops.conv_bias_act(x, w, b, 1, True, 'D', emit_planes=True)
+  zp = ops._take_planes(z)
   torch.cuda.synchronize()
-  for a, c in zip(res[1], res[0]):
-    assert rel_err(a, c) < 2e-5        # same products, other accumulation order (chunk-major vs tap-major)
-  ref = O.leaky_relu(O.conv2d_nhwc(x.double().cpu(), w.double().cpu(), 'SAME') + b.double().cpu())
-  assert rel_err(res[1][2], ref) < 1e-4
-  assert rel_err(res[1][3], res[1][2]) < 1e-5          # planes: hi + lo == z
+  x64, w64 = x.double().cpu().requires_grad_(True), w.double().cpu()
+  y64 = O.conv2d_nhwc(x64, w64, 'SAME')
+  (gx64,) = torch.autograd.grad(y64, x64, gy.double().cpu())
+  assert rel_err(y, y64) < 1e-4
+  assert rel_err(gx, gx64) < 1e-4
+  ref = O.leaky_relu(y64.detach() + b.double().cpu())
+  assert rel_err(z.detach(), ref) < 1e-4
+  assert rel_err(zp.float().sum(0), z.detach()) < 1e-5          # planes: hi + lo == z
 
 
 @pytest.mark.parametrize('shape', [(16, 128, 128, 16, 16), (8, 72, 80, 16, 32), (16, 64, 64, 32, 64), (16, 64, 64, 64, 16),
                                    (6, 64, 64, 32, 32), (5, 40, 48, 16, 64), (5, 40, 48, 32, 16), (9, 64, 64, 64, 32)])
 def test_row_shift_wgrad_matches_the_halo_wgrad(built_lib, shape):
-  """twg_set_option(9, .) A/B on shapes with several tiles per CTA (the stage ring wraps): the row-shift weight-gradient
-  kernel against the halo kernel on the same planes, and both against the fp64 convolution."""
+  """Two weight-gradient kernels on the same operands, on shapes with several pixel tiles per CTA (the stage rings wrap):
+  the tensor-core kernel (split-bf16 wgmma, taps stacked along M) against the exact-fp32 CUDA-core kernel, and both
+  against the fp64 convolution.  (The id is kept from the kernels this A/B was first written for.)"""
   from twingan_b200 import ops
-  L = built_lib
-  ops.set_precision(1)
   N, H, W, Ci, Co = shape
   x = _rand((N, H, W, Ci), 111).requires_grad_(False)
   gy = _rand((N, H, W, Co), 112)
@@ -572,16 +568,16 @@ def test_row_shift_wgrad_matches_the_halo_wgrad(built_lib, shape):
   (ref,) = torch.autograd.grad(O.conv2d_nhwc(x, w, 'SAME'), w, gy)
   xd, gd = _dev(x), _dev(gy)
   res = {}
-  for opt in (1, 0):
-    L.call('twg_set_option', 9, opt)
-    res[opt] = ops.conv_wgrad_raw(xd, gd, 3, 1)
-  L.call('twg_set_option', 9, 1)
+  for prec in (1, 0):
+    ops.set_precision(prec)
+    res[prec] = ops.conv_wgrad_raw(xd, gd, 3, 1)
+  ops.set_precision(1)
   torch.cuda.synchronize()
   assert rel_err(res[1], res[0]) < 2e-5
   assert rel_err(res[1], ref) < 1e-4 and rel_err(res[0], ref) < 1e-4
 
 
-# N, H, W, Cin, Cout: halo-kernel shapes incl. ragged tiles in both directions and every sub-tile count
+# N, H, W, Cin, Cout: shapes with epilogue statistics, incl. ragged tiles in both directions
 STATS_SHAPES = [(3, 64, 64, 16, 16), (2, 24, 40, 16, 32), (2, 128, 128, 32, 32), (2, 20, 36, 64, 16), (4, 16, 16, 32, 64),
                 (2, 72, 80, 16, 16)]
 
@@ -605,7 +601,7 @@ def test_conv_epilogue_statistics(built_lib, shape, offset):
   xd, wd = _dev(x), _dev(w)
   xp, wp = ops.split_act(xd), ops.weight_planes(wd, False)
   y, stats, slots = ops.conv_fwd_planes_stats(xp, wp, N, H, W, Cin, Cout, 3, 1)
-  assert stats is not None and slots > 0, 'halo-kernel shape must offer epilogue statistics'
+  assert stats is not None and slots > 0, 'this shape must offer epilogue statistics'
   y_plain = ops.conv_fwd_planes(xp, wp, N, H, W, Cin, Cout, 3, 1)
   assert torch.equal(y, y_plain)                       # the statistics epilogue does not change y
   buf = torch.empty((4, N, Cout), device='cuda:0')

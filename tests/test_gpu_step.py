@@ -60,7 +60,7 @@ def test_step_parity_config4_256(built_lib, prec, batch):
   network amplifies a relative conv error by ~500x on its way through ~100 layer applications with instance norm
   (eps 1e-6): split-bf16's ~2e-6 per product (residues x - hi - lo and the dropped lo.lo term) lands at ~1e-3, fp32's
   6e-8 at ~1e-4.  For scale: the SAME code run twice on the 16-pair batch differs from itself by 1e-2 in this gradient
-  (fp32 atomics order + leaky-ReLU kinks, gpurun_out/r2_noise.log).  The bound asserted for prec 1 is the measured one,
+  (fp32 atomics order + leaky-ReLU kinks).  The bound asserted for prec 1 is the measured one,
   not the north-star's; DESIGN.md section 4 says what closing the gap would cost."""
   res = run_step_parity(hw=256, batch=batch, max_num_channels=256, norm='instance_norm', is_growing=False, prec=prec,
                         verbose=True, tol=REL_TOL if prec == 0 else TOL_256_TENSOR_CORE)
@@ -108,7 +108,7 @@ def test_step_parity_optional_flags(built_lib, hw, batch, mc, growing, extra, ws
   """SURVEY 8f-4 rows built on the same kernels: --loss_architecture wgan / wgan_gp (+ drift) / hinge / gan
   (image_generation.py:330-439), --equalized_learning_rate (nets/pggan_utils.py:236-254) and --use_res_block (:257-264),
   whole step against the fp64
-  oracle (itself held to the reference's own method sources on these flags: tests/golden/reference_f4.npz).  Exact-fp32
+  oracle (itself held to the reference's own method sources on these flags: tests/golden/reference_f4_*.npz).  Exact-fp32
   convs: these rows are about wiring; the tensor-core precision is covered by the default-flag cases."""
   extra = dict(extra)
   norm = extra.pop('_norm', 'instance_norm')
@@ -204,7 +204,7 @@ def test_graph_replay_matches_eager(built_lib):
                                   'f4_hinge16grow', 'f4_gan8', 'f4_eqlr_dragan8', 'f4_eqlr_hinge64', 'f4_res16grow',
                                   'f4_res_eqlr_renorm8'])
 def test_product_matches_vectors_from_the_reference_code(built_lib, case):
-  """The CUDA path against tests/golden/reference_pggan.npz directly: losses and forward tensors that the reference's own
+  """The CUDA path against tests/golden/reference_pggan_*.npz directly: losses and forward tensors that the reference's own
   _clone_fn / add_loss produced under the TF stand-in (tests/golden/make_reference_golden.py).  Forward quantities
   only -- gradient parity needs the kink-aware comparison of test_step_parity."""
   import ast
@@ -218,7 +218,8 @@ def test_product_matches_vectors_from_the_reference_code(built_lib, case):
   from twingan_b200 import ops, twingan
   from tests.parity import rel_err
   import json
-  z = np.load(os.path.join(here, 'golden', 'reference_f4.npz' if case.startswith('f4_') else 'reference_pggan.npz'))
+  import npz_parts
+  z = npz_parts.load(os.path.join(here, 'golden', 'reference_f4' if case.startswith('f4_') else 'reference_pggan'))
   hw, growing, mc, batch, gs, max_steps = [int(v) for v in z[case + '/meta']]
   norm = str(z[case + '/norm'])
   alpha = (gs / max_steps) if growing else 0.0

@@ -1,4 +1,4 @@
-"""twingan_b200 -- B200-native (sm_100a) engine for the TwinGAN G+D training step and the
+"""twingan_b200 -- H100-native (sm_90a) engine for the TwinGAN G+D training step and the
 inference-only generator of jerryli27/TwinGAN.  See DESIGN.md.
 
 Layout: csrc/ (CUDA kernels + the C-ABI of include/twg.h, built into libtwg.so), `ops` (operator

@@ -1,4 +1,4 @@
-// Shared helpers for libtwg.so (sm_100a only).
+// Shared helpers for libtwg.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -15,12 +15,20 @@ extern std::atomic<int64_t> g_launches;
 int fail(int code, const char* fmt, ...);
 int check_launch(const char* what);
 
+// Deterministic cross-block sums.  A kernel whose blocks would each add a partial sum into the same outputs instead stores
+// block b's partial of output i at parts[b * n + i] (parts = partials(nb * n), zeroed when `zero`), and add_partials then
+// adds them to out[i] in block order -- fp32 atomics would add them in whatever order the blocks finish, and the training
+// step amplifies that last-bit noise into visibly different results from run to run.  The buffer is owned by the library
+// (one per device), so kernels of this library must not run concurrently on two streams of one device.
+float* partials(int64_t n, bool zero, cudaStream_t st);
+int add_partials(float* out, const float* parts, int nb, int64_t n, cudaStream_t st);
+
 inline cudaStream_t S(twg_stream_t s) { return reinterpret_cast<cudaStream_t>(s); }
 inline int64_t cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
 constexpr float kLeak = 0.2f;        // util_misc.py:68
 constexpr float kPixEps = 1e-6f;     // nets/pggan_utils.py:330
-constexpr int kNumSMs = 148;         // B200
+constexpr int kNumSMs = 132;         // H100 SXM: grid sizing (waves, split-K) only, never results
 
 __device__ __forceinline__ float lrelu(float x) { return fmaxf(kLeak * x, x); }
 __device__ __forceinline__ float lrelu_slope(float ref) { return ref > 0.f ? 1.f : kLeak; }

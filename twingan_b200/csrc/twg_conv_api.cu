@@ -1,5 +1,5 @@
 // C-ABI entry points of the convolution family: dispatch between the exact-fp32 CUDA-core path
-// (prec=0, twg_conv_simt.cu) and the tcgen05 tensor-core path (prec=1, twg_conv_tc.cu).
+// (prec=0, twg_conv_simt.cu) and the wgmma tensor-core path (prec=1, twg_conv_tc.cu).
 #include <string.h>
 #include "twg_common.cuh"
 
@@ -12,14 +12,6 @@ int conv_fwd_tc(const float*, const float*, float*, int, int, int, int, int, int
 int conv_wgrad_tc(const float*, const float*, float*, int, int, int, int, int, int, int, int, void*, int64_t, cudaStream_t);
 int64_t conv_tc_workspace(int, int, int, int, int, int, int);
 bool conv_tc_supported(int, int, int, int, int, int, int);
-void set_use_halo(bool);
-void set_halo_mode(int);
-void set_fwd_cluster(int);
-void set_fwd_ts(int);
-void set_use_htap(int);
-void set_use_wgrad_row(int);
-void set_use_wgrad_rows(int);
-void set_use_htap2(int);
 int split_act_planes(const float*, void*, int64_t, cudaStream_t);
 int split_weight_planes(const float*, void*, int, int, int, int, cudaStream_t);
 int conv_fwd_tc_planes(const void*, const void*, float*, int, int, int, int, int, int, int, bool, cudaStream_t,
@@ -191,18 +183,6 @@ int64_t twg_crc32c(const void* data, int64_t n, int64_t crc) {
   }
   while (n-- > 0) c = table[0][(c ^ *p++) & 0xFF] ^ (c >> 8);
   return (int64_t)(c ^ 0xFFFFFFFFu);
-}
-
-int twg_set_option(int key, int value) {
-  if (key == 1) { set_use_halo(value != 0); return TWG_OK; }
-  if (key == 2) { set_halo_mode(value); return TWG_OK; }
-  if (key == 4) { set_fwd_cluster(value); return TWG_OK; }
-  if (key == 3) { set_fwd_ts(value); return TWG_OK; }
-  if (key == 6) { set_use_htap(value); return TWG_OK; }
-  if (key == 7) { set_use_wgrad_row(value); return TWG_OK; }
-  if (key == 8) { set_use_htap2(value); return TWG_OK; }
-  if (key == 9) { set_use_wgrad_rows(value); return TWG_OK; }
-  return fail(TWG_ERR_INVALID, "twg_set_option: unknown key %d", key);
 }
 
 }  // extern "C"

@@ -168,7 +168,7 @@ __global__ void __launch_bounds__(256) k_pw_wgrad(const float* __restrict__ smal
       }
       if (threadIdx.x < G) {
         const int l = (lg + (j / 4) * 32) * 4 + (j & 3);
-        atomicAdd(&gw[s * ws_s + l * ws_l], sm[threadIdx.x]);
+        gw[(int64_t)blockIdx.x * S * L + s * ws_s + l * ws_l] = sm[threadIdx.x];   // this block's partial (add_partials)
       }
     }
   }
@@ -248,10 +248,13 @@ int pw_wgrad(const float* x, const float* gy, float* gw, int64_t P, int Cin, int
   if (blocks > 4 * kNumSMs) blocks = 4 * kNumSMs;
   const int64_t chunk = cdiv(P, blocks);
   blocks = cdiv(P, chunk);
-  if (V == 1) k_pw_wgrad<1><<<(unsigned)blocks, 256, 0, st>>>(small, big, gw, P, S, L, G, ws_s, ws_l, chunk);
-  else if (V == 2) k_pw_wgrad<2><<<(unsigned)blocks, 256, 0, st>>>(small, big, gw, P, S, L, G, ws_s, ws_l, chunk);
-  else k_pw_wgrad<4><<<(unsigned)blocks, 256, 0, st>>>(small, big, gw, P, S, L, G, ws_s, ws_l, chunk);
-  return check_launch("twg_conv pointwise wgrad");
+  float* parts = partials(blocks * S * L, true, st);
+  if (!parts) return fail(TWG_ERR_UNSUPPORTED, "twg_conv pointwise wgrad: %d x %d too wide", Cin, Cout);
+  if (V == 1) k_pw_wgrad<1><<<(unsigned)blocks, 256, 0, st>>>(small, big, parts, P, S, L, G, ws_s, ws_l, chunk);
+  else if (V == 2) k_pw_wgrad<2><<<(unsigned)blocks, 256, 0, st>>>(small, big, parts, P, S, L, G, ws_s, ws_l, chunk);
+  else k_pw_wgrad<4><<<(unsigned)blocks, 256, 0, st>>>(small, big, parts, P, S, L, G, ws_s, ws_l, chunk);
+  if (int rc = check_launch("twg_conv pointwise wgrad")) return rc;
+  return add_partials(gw, parts, (int)blocks, (int64_t)S * L, st);
 }
 
 }  // namespace twg

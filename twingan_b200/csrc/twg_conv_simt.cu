@@ -124,8 +124,8 @@ __global__ void __launch_bounds__(256) k_conv_fwd_simt(const float* __restrict__
     for (int j = 0; j < TN; ++j) {
       const int co = n0 + tx * TN + j;
       if (co < g.Cout) {
-        if (gridDim.z == 1) y[m * g.Cout + co] = acc[i][j];
-        else atomicAdd(&y[m * g.Cout + co], acc[i][j]);
+        // split-K: y is the partial buffer, slice blockIdx.z (add_partials sums the slices in order)
+        y[(int64_t)blockIdx.z * M * g.Cout + m * g.Cout + co] = acc[i][j];
       }
     }
   }
@@ -201,7 +201,8 @@ __global__ void __launch_bounds__(256) k_conv_wgrad_simt(const float* __restrict
 #pragma unroll
     for (int j = 0; j < TN; ++j) {
       const int co = co0 + tx * TN + j;
-      if (co < g.Cout) atomicAdd(&gw[((int64_t)tap * g.Cin + ci) * g.Cout + co], acc[i][j]);
+      if (co < g.Cout)   // this pixel split's partial (add_partials sums the splits in order)
+        gw[(int64_t)blockIdx.y * g.k * g.k * g.Cin * g.Cout + ((int64_t)tap * g.Cin + ci) * g.Cout + co] = acc[i][j];
     }
   }
 }
@@ -211,22 +212,29 @@ static int launch_fwd(const float* x, const float* w, float* y, ConvGeom g, bool
   const int bn = g.Cout <= 16 ? 16 : 64;
   const int64_t ctas = cdiv(M, 128) * cdiv(g.Cout, bn);
   const int num_kb = g.k * g.k * (int)cdiv(g.Cin, 8);
-  // split-K when the output tile grid cannot fill the GPU (4x4-resolution layers, the 4x4 VALID head, the FC)
+  // split-K when the output tile grid cannot fill the GPU (4x4-resolution layers, the 4x4 VALID head, the FC); the
+  // splits store partial tiles that add_partials sums in split order, so the result is the same on every run
   int64_t splits = 1;
   if (ctas < kNumSMs) splits = cdiv(2 * kNumSMs, ctas);
   if (splits > num_kb / 4) splits = num_kb / 4 > 0 ? num_kb / 4 : 1;
   const int kbps = (int)cdiv(num_kb, splits);
   splits = cdiv(num_kb, kbps);
-  if (splits > 1) cudaMemsetAsync(y, 0, sizeof(float) * M * g.Cout, st);
+  float* out = y;
+  if (splits > 1) {
+    out = partials(splits * M * g.Cout, false, st);
+    if (!out) return fail(TWG_ERR_UNSUPPORTED, "twg_conv simt: output too large for the split buffer");
+    cudaMemsetAsync(y, 0, sizeof(float) * M * g.Cout, st);
+  }
   dim3 grid((unsigned)cdiv(M, 128), (unsigned)cdiv(g.Cout, bn), (unsigned)splits);
   if (bn == 16) {
-    if (transposed) k_conv_fwd_simt<16, 2, true><<<grid, 256, 0, st>>>(x, w, y, g, kbps);
-    else k_conv_fwd_simt<16, 2, false><<<grid, 256, 0, st>>>(x, w, y, g, kbps);
+    if (transposed) k_conv_fwd_simt<16, 2, true><<<grid, 256, 0, st>>>(x, w, out, g, kbps);
+    else k_conv_fwd_simt<16, 2, false><<<grid, 256, 0, st>>>(x, w, out, g, kbps);
   } else {
-    if (transposed) k_conv_fwd_simt<64, 4, true><<<grid, 256, 0, st>>>(x, w, y, g, kbps);
-    else k_conv_fwd_simt<64, 4, false><<<grid, 256, 0, st>>>(x, w, y, g, kbps);
+    if (transposed) k_conv_fwd_simt<64, 4, true><<<grid, 256, 0, st>>>(x, w, out, g, kbps);
+    else k_conv_fwd_simt<64, 4, false><<<grid, 256, 0, st>>>(x, w, out, g, kbps);
   }
-  return check_launch("twg_conv simt");
+  if (int rc = check_launch("twg_conv simt")) return rc;
+  return splits > 1 ? add_partials(y, out, (int)splits, M * g.Cout, st) : TWG_OK;
 }
 
 int conv_fwd_simt(const float* x, const float* w, float* y, int N, int H, int W, int Cin, int Cout, int k, int pad,
@@ -258,11 +266,15 @@ int conv_wgrad_simt(const float* x, const float* gy, float* gw, int N, int H, in
   int64_t mps = cdiv(cdiv(M, splits), 16) * 16;
   splits = cdiv(M, mps);
   dim3 grid((unsigned)tiles, (unsigned)splits);
-  if (bmc == 16 && bnc == 16) k_conv_wgrad_simt<16, 16><<<grid, 256, 0, st>>>(x, gy, gw, g, mps);
-  else if (bmc == 16) k_conv_wgrad_simt<16, 64><<<grid, 256, 0, st>>>(x, gy, gw, g, mps);
-  else if (bnc == 16) k_conv_wgrad_simt<64, 16><<<grid, 256, 0, st>>>(x, gy, gw, g, mps);
-  else k_conv_wgrad_simt<64, 64><<<grid, 256, 0, st>>>(x, gy, gw, g, mps);
-  return check_launch("twg_conv_wgrad simt");
+  const int64_t gw_elems = (int64_t)k * k * Cin * Cout;
+  float* parts = partials(splits * gw_elems, true, st);
+  if (!parts) return fail(TWG_ERR_UNSUPPORTED, "twg_conv_wgrad simt: weight too large for the split buffer");
+  if (bmc == 16 && bnc == 16) k_conv_wgrad_simt<16, 16><<<grid, 256, 0, st>>>(x, gy, parts, g, mps);
+  else if (bmc == 16) k_conv_wgrad_simt<16, 64><<<grid, 256, 0, st>>>(x, gy, parts, g, mps);
+  else if (bnc == 16) k_conv_wgrad_simt<64, 16><<<grid, 256, 0, st>>>(x, gy, parts, g, mps);
+  else k_conv_wgrad_simt<64, 64><<<grid, 256, 0, st>>>(x, gy, parts, g, mps);
+  if (int rc = check_launch("twg_conv_wgrad simt")) return rc;
+  return add_partials(gw, parts, (int)splits, gw_elems, st);
 }
 
 }  // namespace twg

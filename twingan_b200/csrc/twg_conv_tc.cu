@@ -1,17 +1,15 @@
-// tcgen05 tensor-core convolution for sm_100a: implicit-GEMM forward / data-gradient and weight-gradient
-// with split-bf16 operands ("bf16x3": x = hi + lo, three MMAs per product, fp32 TMEM accumulation), so
-// results match an fp32 convolution to ~1e-5 relative while running on the 5th-gen tensor cores.
+// wgmma tensor-core convolution for sm_90a: implicit-GEMM forward / data-gradient and weight-gradient with
+// split-bf16 operands ("bf16x3": x = hi + lo, three MMAs per product -- lo.hi, hi.lo, hi.hi -- fp32 register
+// accumulation), so results match an fp32 convolution to ~1e-5 relative while running on the tensor cores.
 //
-// Data path (per CTA, warp-specialised, mbarrier pipeline):
-//   warp 0   : TMA producer   -- cp.async.bulk.tensor 4D boxes {Cc, TW, TH, TN} of the NHWC bf16 hi/lo planes
-//                                (signed start coordinates + hardware zero fill == SAME padding), 2D boxes of
-//                                the K-major weight planes, landing in 128B/64B/32B-swizzled shared memory
-//   warp 1   : MMA issuer     -- one elected lane issues tcgen05.mma.cta_group::1.kind::f16 (M=128, N=BN, K=16)
-//                                straight from the swizzled tiles; tcgen05.commit frees the smem stage
-//   warps 2-5: epilogue       -- tcgen05.ld 32x32b (thread = output pixel, registers = channels), fp32 NHWC
-//                                vector stores
-// The same TMA tiles serve the forward (pixel rows are the K-major A operand) and the weight gradient
-// (pixel rows are the GEMM K dimension, channels MN-major for both operands).
+// Both kernels are warp-specialised around an mbarrier ring (288 threads per CTA):
+//   warps 0-7 : two consumer warpgroups; each issues wgmma.mma_async m64nNk16 on its 64-row half of the M = 128 tile
+//               straight from the swizzled shared-memory tiles and runs the epilogue from its accumulator registers
+//   warp 8    : TMA producer -- cp.async.bulk.tensor 4D boxes {C, TW, TH, TN} of the NHWC bf16 hi/lo planes (signed
+//               start coordinates + hardware zero fill == SAME padding) and 2D boxes of the K-major weight planes,
+//               landing in 128B/64B/32B-swizzled shared memory (the swizzle width is the channel chunk's row length)
+// The forward reads pixels as the K-major A operand; the weight gradient reads the same NHWC tiles as MN-major operands
+// (pixels are its GEMM K dimension), so no operand is ever transposed in memory.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -32,7 +30,10 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int dbg_id = 0) {
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   // try_wait suspends for a bounded time per attempt; a pipeline bug must surface as a trap, never as a hung GPU
   uint32_t done = 0;
   uint64_t t0 = 0;
@@ -50,16 +51,12 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int db
       uint64_t now;
       asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
       if (t0 == 0) t0 = now;
-      else if (now - t0 > 2000000000ull) {             // 2 s without progress: report and abort the kernel
-        printf("twg: mbarrier wait timed out: block (%d,%d,%d) thread %d barrier-id %d parity %u\n", blockIdx.x, blockIdx.y,
-               blockIdx.z, threadIdx.x, dbg_id, parity);
-        __trap();
-      }
+      else if (now - t0 > 2000000000ull) __trap();    // 2 s without progress: abort the kernel (no printf here: a call
+                                                      // in the kernel would serialise the wgmma pipeline)
     }
   }
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_4d(const CUtensorMap* tm, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3) {
   asm volatile(
@@ -73,129 +70,93 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* tm, uint64_t* bar
       ::"r"(smem_u32(dst)), "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-// one CTA of a cluster loads the box and the hardware writes it to the same shared-memory offset of every CTA in `mask`,
-// completing the transaction bytes on the mbarrier at the same offset in each of them
-__device__ __forceinline__ void tma_load_2d_mc(const CUtensorMap* tm, uint64_t* bar, void* dst, int c0, int c1, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, %5}], [%2], %3;"
-      ::"r"(smem_u32(dst)), "l"(tm), "r"(smem_u32(bar)), "h"(mask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.aligned;\nbarrier.cluster.wait.aligned;" ::: "memory");
-}
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* tm) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(tm) : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]   (A operand staged in tensor memory: no shared-memory fetch of A per MMA)
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// smem (matrix descriptor) -> TMEM: 128 lanes x 256 bits = one K=16 bf16 slice of a 128-row A operand
-__device__ __forceinline__ void tmem_cp_128x256b(uint32_t tmem_dst, uint64_t sdesc) {
-  asm volatile("tcgen05.cp.cta_group::1.128x256b [%0], %1;" ::"r"(tmem_dst), "l"(sdesc) : "memory");
-}
-// mbarrier arrives once all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// same, arriving on the barrier at this offset in every CTA of `mask` (a stage shared through TMA multicast is free
-// only when ALL the CTAs that received it have consumed it)
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(mask) : "memory");
-}
-// issue only: the caller batches several loads and waits once (tmem_ld_wait)
-__device__ __forceinline__ void tmem_ld16_issue(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// warpgroup MMA: D[64 x N] (+)= A[64 x 16] * B[16 x N], A and B described by shared-memory matrix descriptors.
+// TA / TB = 1: the operand is MN-major (M or N contiguous in shared memory) instead of K-major.
+template <int N>
+struct Wgmma;
+template <>
+struct Wgmma<16> {
+  template <int TA, int TB>
+  __device__ __forceinline__ static void mma(float (&d)[8], uint64_t a, uint64_t b) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %10, %11;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a), "l"(b), "n"(TA), "n"(TB));
+  }
+};
+template <>
+struct Wgmma<32> {
+  template <int TA, int TB>
+  __device__ __forceinline__ static void mma(float (&d)[16], uint64_t a, uint64_t b) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %18, %19;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a), "l"(b), "n"(TA), "n"(TB));
+  }
+};
+template <>
+struct Wgmma<64> {
+  template <int TA, int TB>
+  __device__ __forceinline__ static void mma(float (&d)[32], uint64_t a, uint64_t b) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %34, %35;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a), "l"(b), "n"(TA), "n"(TB));
+  }
+};
+template <>
+struct Wgmma<128> {
+  template <int TA, int TB>
+  __device__ __forceinline__ static void mma(float (&d)[64], uint64_t a, uint64_t b) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %66, %67;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a), "l"(b), "n"(TA), "n"(TB));
+  }
+};
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void fence_acc(float (&d)[R]) {
 #pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ---- descriptors (cute/arch/mma_sm100_desc.hpp bit layout) ------------------------------------------------
-// shared-memory matrix descriptor: start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | version=1 [46,48) |
-// layout [61,64) (2 = 128B swizzle, 4 = 64B, 6 = 32B)
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout,
-                                             uint32_t base_offset = 0) {
-  uint64_t d = (uint64_t)(base_offset & 7) << 49;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
+// ---- sm_90 shared-memory matrix descriptor ------------------------------------------------------------
+// start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | base offset [49,52) = 0 | layout [62,64): 1 = 128B, 2 = 64B, 3 = 32B swizzle.
+// K-major swizzled operand: SBO = stride between 8-row groups, LBO unused; a K step of 16 bf16 inside the swizzle atom
+// advances the start address by 32 bytes.  MN-major swizzled operand: LBO = stride between MN atoms (one atom = one
+// swizzle row of channels), SBO = stride between groups of 8 K rows.
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
+  uint64_t d = (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)layout << 61;
+  d |= (uint64_t)layout << 62;
   return d;
 }
-// advance a descriptor's start address by a byte offset (multiple of 16): one 64-bit add on the issue path
+// advance a descriptor's start address by a byte offset (multiple of 16)
 __device__ __forceinline__ uint64_t desc_add(uint64_t d, uint32_t byte_off) { return d + (uint64_t)(byte_off >> 4); }
+__host__ __device__ constexpr uint32_t swizzle_layout_for(int cc) { return cc == 64 ? 1u : (cc == 32 ? 2u : 3u); }
 
-// instruction descriptor: c=f32 [4,6)=1, a=bf16 [7,10)=1, b=bf16 [10,13)=1, a_major bit15, b_major bit16,
-// N>>3 [17,23), M>>4 [24,29)
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__host__ __device__ constexpr uint32_t swizzle_layout_for(int cc) { return cc == 64 ? 2u : (cc == 32 ? 4u : 6u); }
-
-// write 4 consecutive fp32 values as split-bf16 planes (hi plane [n], lo plane [n]); e4 = element index / 4
-__device__ __forceinline__ void st_planes4(void* planes, int64_t n_total, int64_t e4, float4 v) {
-  // hi = bf16(x), lo = bf16(x - hi), two values per conversion instruction (cvt.rn.bf16x2.f32); same rounding as the scalar form
-  const __nv_bfloat162 h01 = __floats2bfloat162_rn(v.x, v.y), h23 = __floats2bfloat162_rn(v.z, v.w);
-  const float2 f01 = __bfloat1622float2(h01), f23 = __bfloat1622float2(h23);
-  const __nv_bfloat162 l01 = __floats2bfloat162_rn(v.x - f01.x, v.y - f01.y), l23 = __floats2bfloat162_rn(v.z - f23.x, v.w - f23.y);
-  uint2 hv, lv;
-  hv.x = *reinterpret_cast<const uint32_t*>(&h01); hv.y = *reinterpret_cast<const uint32_t*>(&h23);
-  lv.x = *reinterpret_cast<const uint32_t*>(&l01); lv.y = *reinterpret_cast<const uint32_t*>(&l23);
+// write 2 consecutive fp32 values as split-bf16 planes (hi plane [n], lo plane [n]); e = even element index
+__device__ __forceinline__ void st_planes2(void* planes, int64_t n_total, int64_t e, float a, float b) {
+  const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+  const float2 f = __bfloat1622float2(h);
+  const __nv_bfloat162 l = __floats2bfloat162_rn(a - f.x, b - f.y);
   __nv_bfloat16* hi = reinterpret_cast<__nv_bfloat16*>(planes);
-  reinterpret_cast<uint2*>(hi)[e4] = hv;
-  reinterpret_cast<uint2*>(hi + n_total)[e4] = lv;
+  *reinterpret_cast<__nv_bfloat162*>(hi + e) = h;
+  *reinterpret_cast<__nv_bfloat162*>(hi + n_total + e) = l;
 }
 
 // ----------------------------------------------------------------------------------------------------
@@ -255,12 +216,10 @@ struct TcGeom {
   int tiles_w, tiles_h, tiles_n;
 };
 
-#ifndef TWG_TAP_EPI_CH
-#define TWG_TAP_EPI_CH 16
-#endif
-#ifndef TWG_TAP_CAT
-#define TWG_TAP_CAT 1    // A/B: 0 builds the three-MMA variant
-#endif
+constexpr int kConsumerWarps = 8;                       // two warpgroups
+constexpr int kThreads = (kConsumerWarps + 1) * 32;     // + the TMA producer warp
+// Registers are allocated in units of four warps, so a CTA of kThreads gets at most 168 a thread: every tile's
+// accumulators (BN / 2, or groups * BNW / 2 for the weight gradient) must fit well below that.
 
 template <int CC, int BN>
 struct FwdSmem {
@@ -268,46 +227,40 @@ struct FwdSmem {
   static constexpr int kBTileRaw = BN * CC * 2;
   static constexpr int kBTile = (kBTileRaw + 1023) / 1024 * 1024;
   static constexpr int kStage = 2 * kATile + 2 * kBTile;
-  // big stages: as many as fit in ~200 KB (1 CTA/SM); small stages: up to 8 within ~96 KB so that two CTAs fit
-  // per SM and enough TMA bytes are in flight to cover the ~1.5 us load latency (Little's law, ~64 KB per SM)
-  static constexpr int kStages = (kStage >= 40 * 1024)
-                                     ? ((kStage * 4 <= 200 * 1024) ? 4 : (kStage * 3 <= 200 * 1024 ? 3 : 2))
-                                     : ((96 * 1024 / kStage) > 8 ? 8 : (96 * 1024 / kStage));
-  static constexpr int kBytes = kStages * kStage + 1024 /*align*/ + 512 /*barriers*/;
+  // enough stages to keep ~100+ KB of TMA traffic in flight per CTA, within the 227 KB an H100 block may use
+  static constexpr int kStagesRaw = (200 * 1024) / kStage;
+  static constexpr int kStages = kStagesRaw > 8 ? 8 : (kStagesRaw < 2 ? 2 : kStagesRaw);
+  static constexpr int kBytes = kStages * kStage + 1024 /*align*/ + 256 /*barriers*/;
+  static_assert(kBytes <= 227 * 1024, "forward conv exceeds shared memory");
 };
 
-// CL = 2: the two CTAs of a cluster own neighbouring pixel tiles and the SAME weight tile; each loads half of it and
-// TMA multicasts it to both (the kernel is bound by the L2 -> shared-memory feed, 64 KB per 768 tensor-pipe cycles, not
-// by the tensor pipe: profiles/r01_mma_issue_rate_probe.txt), which cuts the weight traffic per CTA in half.
-template <int CC, int BN, bool TS, int CL = 1>
-__global__ void __launch_bounds__(192, 1) k_conv_fwd_tc(const __grid_constant__ CUtensorMap tm_a_hi,
-                                                        const __grid_constant__ CUtensorMap tm_a_lo,
-                                                        const __grid_constant__ CUtensorMap tm_b_hi,
-                                                        const __grid_constant__ CUtensorMap tm_b_lo,
-                                                        float* __restrict__ y, TcGeom g,
-                                                        const float* __restrict__ bias, int act, int kb_per_split,
-                                                        void* __restrict__ z_planes) {
+// Epilogue options (all null / 0 = plain fp32 store):
+//   bias, act & 1      : + bias[c], leaky-ReLU                       (discriminator layers)
+//   z_planes           : also store the result as split-bf16 planes  (input of the next conv)
+//   act_mask           : sign of the (activated) result, 4 bits per 4 channels (the activation backward reads these)
+//   stats              : {count, pivot, S1, S2} per (image, tile, consumer warp, channel) for the instance-norm statistics
+//   aff_a              : z = pixel_norm?(lrelu?(aff_a[c] * conv + bias[c])), act bit 1 = pixel norm (Cout == BN: a row of
+//                        the accumulator fragment is spread over 4 lanes, so the pixel's mean square is a 4-lane sum)
+template <int CC, int BN>
+__global__ void __launch_bounds__(kThreads, 1) k_conv_fwd_wgmma(const __grid_constant__ CUtensorMap tm_a_hi,
+                                                                const __grid_constant__ CUtensorMap tm_a_lo,
+                                                                const __grid_constant__ CUtensorMap tm_b_hi,
+                                                                const __grid_constant__ CUtensorMap tm_b_lo,
+                                                                float* __restrict__ y, TcGeom g,
+                                                                const float* __restrict__ bias, int act,
+                                                                void* __restrict__ z_planes, float4* __restrict__ stats,
+                                                                uint8_t* __restrict__ act_mask, const float* __restrict__ aff_a) {
   using SM = FwdSmem<CC, BN>;
   constexpr int kStages = SM::kStages;
-  // TS: the A operand (hi and lo, CC/16 K-slices of 8 TMEM columns each) is staged in tensor memory behind the accumulator
-  constexpr uint32_t kACols = TS ? 2 * (CC / 16) * 8 : 0;
-  // kCat: [B_hi | B_lo] (adjacent in shared memory) is fed as ONE N = 2*BN operand: two MMAs per K-step instead of three
-  // and 20 KB instead of 24 KB of operand reads per K-step at BN = 128 -- the kernel is bound by shared-memory bandwidth
-  // (MMA operand reads + TMA fill > 128 B/clk/SM), see DESIGN.md 3.2.  The hi.lo partial sums land in columns
-  // [BN, 2BN) and the epilogue adds them.
-  constexpr bool kCat = !TS && (SM::kBTileRaw % 1024 == 0) && (2 * BN <= 256) && (TWG_TAP_CAT != 0);
-  constexpr uint32_t kNeed = (kCat ? 2 * BN : BN) + kACols;
-  constexpr uint32_t kTmemCols = kNeed <= 32 ? 32 : (kNeed <= 64 ? 64 : (kNeed <= 128 ? 128 : (kNeed <= 256 ? 256 : 512)));
+  // the statistics, sign-mask and pixel-norm epilogues exist for the single-block shapes only (Cout <= 64; the host
+  // never asks for them otherwise), which keeps the BN = 128 instantiation within its registers
+  constexpr bool kFused = BN <= 64;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * SM::kStage);
-  uint64_t* full = bars;                 // [kStages]
-  uint64_t* empty = bars + kStages;      // [kStages]
-  uint64_t* tmem_full = bars + 2 * kStages;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * kStages + 1);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + kStages * SM::kStage);   // [kStages]
+  uint64_t* empty = full + kStages;                                           // [kStages]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // tile coordinates
   int mt = blockIdx.x;
   const int tw_i = mt % g.tiles_w; mt /= g.tiles_w;
   const int th_i = mt % g.tiles_h;
@@ -315,28 +268,17 @@ __global__ void __launch_bounds__(192, 1) k_conv_fwd_tc(const __grid_constant__ 
   const int w0 = tw_i * g.TW, h0 = th_i * g.TH, n0 = tn_i * g.TN;
   const int co0 = blockIdx.y * BN;
   const int cchunks = g.Cin / CC;
-  // split-K: blockIdx.z owns a contiguous range of (tap, cin-chunk) blocks; partial tiles are combined with fp32
-  // atomics (low-resolution wide layers have too few output tiles to fill 148 SMs otherwise)
-  const int kb_begin = blockIdx.z * kb_per_split;
-  const int kb_end = min(g.k * g.k * cchunks, kb_begin + kb_per_split);
+  const int kb_begin = 0, kb_end = g.k * g.k * cchunks;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kConsumerWarps && lane == 0) {
     prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_a_lo); prefetch_tmap(&tm_b_hi); prefetch_tmap(&tm_b_lo);
-    for (int s = 0; s < kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], CL); }
-    mbar_init(tmem_full, 1);
+    for (int s = 0; s < kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kConsumerWarps); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  if constexpr (CL > 1) cluster_sync_all();     // the peer's TMA / commits must find these barriers initialised
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  constexpr uint16_t kMask = (uint16_t)((1u << CL) - 1);
 
-  if (warp == 0) {
+  if (warp == kConsumerWarps) {
     if (lane == 0) {
-      const uint32_t crank = (CL > 1) ? cluster_ctarank() : 0;
       int stage = 0; uint32_t phase = 0;
       for (int kb = kb_begin; kb < kb_end; ++kb) {
         mbar_wait(&empty[stage], phase ^ 1);
@@ -346,178 +288,190 @@ __global__ void __launch_bounds__(192, 1) k_conv_fwd_tc(const __grid_constant__ 
         mbar_expect_tx(&full[stage], 2 * SM::kATile + 2 * SM::kBTileRaw);
         tma_load_4d(&tm_a_hi, &full[stage], sa, cc * CC, w0 + kw - g.pad, h0 + kh - g.pad, n0);
         tma_load_4d(&tm_a_lo, &full[stage], sa + SM::kATile, cc * CC, w0 + kw - g.pad, h0 + kh - g.pad, n0);
-        if constexpr (CL == 1) {
-          tma_load_2d(&tm_b_hi, &full[stage], sa + 2 * SM::kATile, cc * CC, tap * g.Cout + co0);
-          tma_load_2d(&tm_b_lo, &full[stage], sa + 2 * SM::kATile + SM::kBTile, cc * CC, tap * g.Cout + co0);
-        } else {
-          // this CTA's 1/CL of the weight rows, delivered to every CTA of the cluster (box = BN/CL rows)
-          constexpr int kRows = BN / CL;
-          const uint32_t off = crank * (kRows * CC * 2);
-          tma_load_2d_mc(&tm_b_hi, &full[stage], sa + 2 * SM::kATile + off, cc * CC, tap * g.Cout + co0 + crank * kRows, kMask);
-          tma_load_2d_mc(&tm_b_lo, &full[stage], sa + 2 * SM::kATile + SM::kBTile + off, cc * CC,
-                         tap * g.Cout + co0 + crank * kRows, kMask);
-        }
+        tma_load_2d(&tm_b_hi, &full[stage], sa + 2 * SM::kATile, cc * CC, tap * g.Cout + co0);
+        tma_load_2d(&tm_b_lo, &full[stage], sa + 2 * SM::kATile + SM::kBTile, cc * CC, tap * g.Cout + co0);
         if (++stage == kStages) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(128, BN, 0, 0);
-      constexpr uint32_t layout = swizzle_layout_for(CC);
-      constexpr uint32_t sbo = 8 * CC * 2;   // 8 rows of CC bf16
-      int stage = 0; uint32_t phase = 0;
-      for (int kb = kb_begin; kb < kb_end; ++kb) {
-        mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + stage * SM::kStage);
-        const uint32_t a_hi = sa, a_lo = sa + SM::kATile, b_hi = sa + 2 * SM::kATile, b_lo = b_hi + SM::kBTile;
-        const uint64_t dah0 = make_desc(a_hi, 16, sbo, layout), dal0 = make_desc(a_lo, 16, sbo, layout);
-        const uint64_t dbh0 = make_desc(b_hi, 16, sbo, layout), dbl0 = make_desc(b_lo, 16, sbo, layout);
-        if (TS) {
-          // stage A_hi / A_lo of this smem stage in TMEM once (tcgen05.cp runs in the MMA pipe, in issue order), then
-          // feed the three products from there: A is fetched from shared memory once instead of 3x (hi twice, lo once)
-          const uint32_t ta_hi = tmem_base + BN, ta_lo = ta_hi + (CC / 16) * 8;
+    return;
+  }
+
+  // ---- consumers: warpgroup wg owns accumulator rows [64 wg, 64 wg + 64) of the 128-pixel tile ----
+  const int wg = warp >> 2;
+  // The MMAs of kFlush consecutive stages accumulate into a fresh fragment `part`, which is then added to `acc` with fp32
+  // adds: one tensor-core accumulation chain over the whole K = 9 * Cin (up to ~14 k products) loses ~1e-5 relative.
+  constexpr int kFlush = 4;
+  float acc[BN / 2], part[BN / 2];
 #pragma unroll
-          for (int ks = 0; ks < CC / 16; ++ks) {
-            tmem_cp_128x256b(ta_hi + ks * 8, desc_add(dah0, ks * 32));
-            tmem_cp_128x256b(ta_lo + ks * 8, desc_add(dal0, ks * 32));
-          }
+  for (int i = 0; i < BN / 2; ++i) { acc[i] = 0.f; part[i] = 0.f; }
+  {
+    constexpr uint32_t layout = swizzle_layout_for(CC);
+    constexpr uint32_t sbo = 8 * CC * 2;   // 8 rows of CC bf16
+    int stage = 0, prev = -1, chained = 0; uint32_t phase = 0;
+    for (int kb = kb_begin; kb < kb_end; ++kb) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * SM::kStage);
+      const uint32_t a_hi = sa + wg * (64 * CC * 2), a_lo = a_hi + SM::kATile;
+      const uint32_t b_hi = sa + 2 * SM::kATile, b_lo = b_hi + SM::kBTile;
+      const uint64_t dah = make_desc(a_hi, 16, sbo, layout), dal = make_desc(a_lo, 16, sbo, layout);
+      const uint64_t dbh = make_desc(b_hi, 16, sbo, layout), dbl = make_desc(b_lo, 16, sbo, layout);
+      wgmma_fence();
 #pragma unroll
-          for (int ks = 0; ks < CC / 16; ++ks) {
-            const uint32_t off = ks * 32;
-            umma_bf16_ts(tmem_base, ta_lo + ks * 8, desc_add(dbh0, off), idesc, (kb != kb_begin) || (ks != 0));
-            umma_bf16_ts(tmem_base, ta_hi + ks * 8, desc_add(dbl0, off), idesc, 1);
-            umma_bf16_ts(tmem_base, ta_hi + ks * 8, desc_add(dbh0, off), idesc, 1);
-          }
-        } else {
-#pragma unroll
-          for (int ks = 0; ks < CC / 16; ++ks) {
-            const uint32_t off = ks * 32;   // 16 bf16 along K inside the swizzle atom
-            if constexpr (kCat) {
-              constexpr uint32_t idesc2 = make_idesc(128, 2 * BN, 0, 0);
-              umma_bf16(tmem_base, desc_add(dah0, off), desc_add(dbh0, off), idesc2, (kb != kb_begin) || (ks != 0));
-              umma_bf16(tmem_base, desc_add(dal0, off), desc_add(dbh0, off), (2 * BN <= 64) ? idesc2 : idesc, 1);   // + lo.lo where free
-            } else {
-              umma_bf16(tmem_base, desc_add(dal0, off), desc_add(dbh0, off), idesc, (kb != kb_begin) || (ks != 0));
-              umma_bf16(tmem_base, desc_add(dah0, off), desc_add(dbl0, off), idesc, 1);
-              umma_bf16(tmem_base, desc_add(dah0, off), desc_add(dbh0, off), idesc, 1);
-            }
-          }
-        }
-        if constexpr (CL == 1) umma_commit(&empty[stage]);
-        else umma_commit_mc(&empty[stage], kMask);      // the stage is shared: free it in every CTA of the cluster
-        if (++stage == kStages) { stage = 0; phase ^= 1; }
+      for (int ks = 0; ks < CC / 16; ++ks) {
+        const uint32_t off = ks * 32;   // 16 bf16 along K inside the swizzle atom
+        Wgmma<BN>::template mma<0, 0>(part, desc_add(dal, off), desc_add(dbh, off));
+        Wgmma<BN>::template mma<0, 0>(part, desc_add(dah, off), desc_add(dbl, off));
+        Wgmma<BN>::template mma<0, 0>(part, desc_add(dah, off), desc_add(dbh, off));
       }
-      umma_commit(tmem_full);
+      wgmma_commit();
+      wgmma_wait<1>();                  // the previous stage's MMAs have read their operands: hand that stage back
+      if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev]); }
+      prev = stage;
+      if (++stage == kStages) { stage = 0; phase ^= 1; }
+      if (++chained == kFlush || kb + 1 == kb_end) {
+        wgmma_wait<0>();
+        fence_acc(part);
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) { acc[i] += part[i]; part[i] = 0.f; }
+        fence_acc(part);
+        chained = 0;
+      }
     }
-  } else {
-    // epilogue warps 2..5 -> TMEM lane quarter (warp % 4)
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
-    int t = m;
+  }
+
+  // ---- epilogue: thread holds rows r0 = 16 (warp % 4) + lane / 4 (+ 8) and columns 8 j + 2 (lane % 4) (+ 1) ----
+  const int quad = lane & 3;
+  int64_t e_row[2];
+  bool ok[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    int t = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
     const int tw = t % g.TW; t /= g.TW;
     const int th = t % g.TH;
     const int tn = t / g.TH;
     const int n = n0 + tn, h = h0 + th, w = w0 + tw;
-    const bool ok = n < g.N && h < g.H && w < g.W;
-    mbar_wait(tmem_full, 0);
-    tc_fence_after();
-    float* dst = y + ((((int64_t)n * g.H + h) * g.W + w) * g.Cout + co0);
-    constexpr int CH = (BN >= TWG_TAP_EPI_CH) ? TWG_TAP_EPI_CH : 16;   // columns per TMEM round trip (loads issued back to back, one wait)
-#pragma unroll 1
-    for (int c = 0; c < BN; c += CH) {
-      uint32_t r[CH];
+    ok[i] = n < g.N && h < g.H && w < g.W;
+    e_row[i] = (((int64_t)n * g.H + h) * g.W + w) * g.Cout + co0;
+  }
+  if (bias) {
 #pragma unroll
-      for (int cc = 0; cc < CH; cc += 16) tmem_ld16_issue(tmem_base + ((uint32_t)(q * 32) << 16) + c + cc, r + cc);
-      uint32_t r2[kCat ? CH : 1];
-      if constexpr (kCat) {
+    for (int j = 0; j < BN / 8; ++j) {
+      const int c = co0 + 8 * j + 2 * quad;
+      const float b0 = __ldg(bias + c), b1 = __ldg(bias + c + 1);
+      float a0 = 1.f, a1 = 1.f;
+      if (aff_a) { a0 = __ldg(aff_a + c); a1 = __ldg(aff_a + c + 1); }
 #pragma unroll
-        for (int cc = 0; cc < CH; cc += 16) tmem_ld16_issue(tmem_base + ((uint32_t)(q * 32) << 16) + BN + c + cc, r2 + cc);
+      for (int i = 0; i < 2; ++i) {
+        float v0 = fmaf(a0, acc[4 * j + 2 * i], b0), v1 = fmaf(a1, acc[4 * j + 2 * i + 1], b1);
+        if (act & 1) { v0 = lrelu(v0); v1 = lrelu(v1); }
+        acc[4 * j + 2 * i] = v0; acc[4 * j + 2 * i + 1] = v1;
       }
-      tmem_ld_wait();
-      float v[CH];
+    }
+  }
+  if (kFused && aff_a && (act & 2)) {
 #pragma unroll
-      for (int j = 0; j < CH; ++j) {
-        v[j] = __uint_as_float(r[j]);
-        if constexpr (kCat) v[j] += __uint_as_float(r2[j]);
-        if (bias) {   // fused discriminator epilogue: + bias, leaky-ReLU
-          v[j] += __ldg(bias + co0 + c + j);
-          if (act) v[j] = lrelu(v[j]);
-        }
+    for (int i = 0; i < 2; ++i) {
+      float ss = 0.f;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) ss = fmaf(acc[4 * j + 2 * i], acc[4 * j + 2 * i], fmaf(acc[4 * j + 2 * i + 1], acc[4 * j + 2 * i + 1], ss));
+      ss += __shfl_xor_sync(0xffffffffu, ss, 1);
+      ss += __shfl_xor_sync(0xffffffffu, ss, 2);
+      const float rinv = rsqrtf(ss * (1.f / (float)BN) + kPixEps);
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) { acc[4 * j + 2 * i] *= rinv; acc[4 * j + 2 * i + 1] *= rinv; }
+    }
+  }
+  const int64_t n_total = (int64_t)g.N * g.H * g.W * g.Cout;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int c = 8 * j + 2 * quad;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
+      uint32_t m = 0;
+      if (kFused && act_mask) {   // lanes 2q and 2q+1 hold channels 4q' .. 4q'+3 of the row: one mask byte per float4 of z
+        m = (v0 > 0.f ? 1u : 0u) | (v1 > 0.f ? 2u : 0u);
+        m |= __shfl_xor_sync(0xffffffffu, m, 1) << 2;
       }
-      if (ok) {
-        if (gridDim.z == 1) {
+      if (!ok[i]) continue;
+      const int64_t e = e_row[i] + c;
+      if (y) *reinterpret_cast<float2*>(y + e) = make_float2(v0, v1);
+      if (z_planes) st_planes2(z_planes, n_total, e, v0, v1);
+      if (kFused && act_mask && (quad & 1) == 0) act_mask[e >> 2] = (uint8_t)m;
+    }
+  }
+  if (kFused && stats) {
+    // One record per (consumer warp, channel) over the warp's 16 pixel rows, around the pivot p = the value of the warp's
+    // first row (lanes 0..3); twg_norm_finalize_partials merges the records.  Tiles never span images (TN == 1 here).
+    float cnt = (ok[0] ? 1.f : 0.f) + (ok[1] ? 1.f : 0.f);
 #pragma unroll
-          for (int j = 0; j < CH; j += 4) {
-            const float4 o = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-            *reinterpret_cast<float4*>(dst + c + j) = o;
-            if (z_planes) st_planes4(z_planes, (int64_t)g.N * g.H * g.W * g.Cout, ((dst - y) + c + j) >> 2, o);
+    for (int off = 4; off < 32; off <<= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, off);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const float p = __shfl_sync(0xffffffffu, acc[4 * j + e], quad);
+        float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          if (ok[i]) {
+            const float d = acc[4 * j + 2 * i + e] - p;
+            s1 += d;
+            s2 = fmaf(d, d, s2);
           }
-        } else {
+        }
 #pragma unroll
-          for (int j = 0; j < CH; j += 4)
-            atomicAdd(reinterpret_cast<float4*>(dst + c + j), make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]));
+        for (int off = 4; off < 32; off <<= 1) {
+          s1 += __shfl_xor_sync(0xffffffffu, s1, off);
+          s2 += __shfl_xor_sync(0xffffffffu, s2, off);
+        }
+        if (lane < 4) {
+          const int slots = g.tiles_h * g.tiles_w * kConsumerWarps;
+          const int slot = (th_i * g.tiles_w + tw_i) * kConsumerWarps + warp;
+          stats[((int64_t)n0 * slots + slot) * g.Cout + co0 + 8 * j + 2 * quad + e] = make_float4(cnt, p, s1, s2);
         }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (CL > 1) cluster_sync_all();   // no CTA leaves while its peer may still multicast into it / arrive on its barriers
-  if (warp == 1) tmem_dealloc(tmem_base, kTmemCols);
 }
 
 // ----------------------------------------------------------------------------------------------------
 // weight-gradient kernel ("tap-stacked"):  gw[tap][ci][co] += sum_pix x[pix + tap][ci] * gy[pix][co]
 //   D[M = (tap, ci) stacked: TG = 128/CN taps x CN channels][N = BNW output channels], K = pixels.
-//   A = TG shifted x tap tiles that sit back to back in shared memory (MN-major, LBO = one tap tile), so ONE
-//   M=128 MMA covers TG taps and every A byte streamed from shared memory is useful (a first version with M = Cout padded to
-//   128 spent 128-row operand reads on 16..32 useful rows); B = the gy tile (MN-major).  ceil(9/TG) accumulators live in TMEM.
+//   A = TG shifted x tap tiles back to back in shared memory, read MN-major with LBO = one tap tile, so one M = 128 tile
+//   covers TG taps (warpgroup wg takes taps [TG/2 wg, TG/2 wg + TG/2)); B = the gy tile, MN-major.  The ceil(9/TG)
+//   accumulators of all tap groups stay in registers over the CTA's pixel tiles and are added to gw once.
 //   Pipeline unit = one tap group (TG*2 tiles = 64 KB), two stages; gy tiles have their own 2-stage ring.
 // ----------------------------------------------------------------------------------------------------
 template <int CN, int BNW>
-struct Wg2Cfg {
-  static constexpr int TG = 128 / CN;                       // taps per M=128 group
+struct WgCfg {
+  static constexpr int TG = 128 / CN;                       // taps per M = 128 group
   static constexpr int kXTile = 128 * CN * 2;               // one tap tile, one plane
   static constexpr int kAStage = 2 * TG * kXTile;           // hi group + lo group = 64 KB
   static constexpr int kGTile = 128 * BNW * 2;              // gy tile, one plane
   static constexpr int kGStage = 2 * kGTile;
   static constexpr int kAStages = 2, kGStages = 2;
-  static constexpr int kEpiPitch = 16 * 4 + 16;               // 16 fp32 columns of one accumulator row + pad
-  static constexpr int kEpiBytes = 4 * 32 * kEpiPitch;        // 4 epilogue warps x 32 rows
-  static constexpr int kBytes = kAStages * kAStage + kGStages * kGStage + kEpiBytes + 1024 + 512;
+  static constexpr int kBytes = kAStages * kAStage + kGStages * kGStage + 1024 + 256;
   static constexpr int kMaxGroups = (9 + TG - 1) / TG;
-  // CN <= 32: [gy_hi | gy_lo] is fed as ONE N = 2*BNW operand (two MMAs per k-step instead of three; the hi.lo
-  // partial sums land in a second column block that the epilogue adds).  CN = 64 would need 640 TMEM columns.
-  static constexpr bool kCat = (CN <= 32);
-  static constexpr int kAccCols = kCat ? 2 * BNW : BNW;
-  // consecutive k-steps into one accumulator serialise on the MMA latency: alternate between kKAcc independent
-  // accumulators per tap group when TMEM has room (the epilogue adds them)
-  static constexpr int kKAcc = (kMaxGroups * 2 * kAccCols <= 512) ? 2 : 1;
-  static constexpr uint32_t kColsNeeded = kMaxGroups * kKAcc * kAccCols;
-  static constexpr uint32_t kTmemCols = kColsNeeded <= 32 ? 32 : kColsNeeded <= 64 ? 64 : kColsNeeded <= 128 ? 128 : kColsNeeded <= 256 ? 256 : 512;
+  static_assert(kBytes <= 227 * 1024, "weight-gradient conv exceeds shared memory");
 };
 
 template <int CN, int BNW>
-__global__ void __launch_bounds__(192, 1) k_conv_wgrad_tc2(const __grid_constant__ CUtensorMap tm_g_hi,
-                                                           const __grid_constant__ CUtensorMap tm_g_lo,
-                                                           const __grid_constant__ CUtensorMap tm_x_hi,
-                                                           const __grid_constant__ CUtensorMap tm_x_lo,
-                                                           float* __restrict__ gw, TcGeom g, int tiles_per_cta) {
-  using C = Wg2Cfg<CN, BNW>;
+__global__ void __launch_bounds__(kThreads, 1) k_conv_wgrad_wgmma(const __grid_constant__ CUtensorMap tm_g_hi,
+                                                                  const __grid_constant__ CUtensorMap tm_g_lo,
+                                                                  const __grid_constant__ CUtensorMap tm_x_hi,
+                                                                  const __grid_constant__ CUtensorMap tm_x_lo,
+                                                                  float* __restrict__ gw, TcGeom g, int tiles_per_cta) {
+  using C = WgCfg<CN, BNW>;
   constexpr int TG = C::TG;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sa = smem;                                     // [kAStages][hi: TG tiles][lo: TG tiles]
   uint8_t* sg = smem + C::kAStages * C::kAStage;          // [kGStages][hi][lo]
-  uint8_t* se = sg + C::kGStages * C::kGStage;            // epilogue staging
-  uint64_t* bars = reinterpret_cast<uint64_t*>(se + C::kEpiBytes);
-  uint64_t* afull = bars;
+  uint64_t* afull = reinterpret_cast<uint64_t*>(sg + C::kGStages * C::kGStage);
   uint64_t* aempty = afull + C::kAStages;
   uint64_t* gfull = aempty + C::kAStages;
   uint64_t* gempty = gfull + C::kGStages;
-  uint64_t* tmem_full = gempty + C::kGStages;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int taps = g.k * g.k;
@@ -528,20 +482,15 @@ __global__ void __launch_bounds__(192, 1) k_conv_wgrad_tc2(const __grid_constant
   const int t_begin = blockIdx.x * tiles_per_cta;
   const int t_end = min(total_tiles, t_begin + tiles_per_cta);
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kConsumerWarps && lane == 0) {
     prefetch_tmap(&tm_g_hi); prefetch_tmap(&tm_g_lo); prefetch_tmap(&tm_x_hi); prefetch_tmap(&tm_x_lo);
-    for (int s = 0; s < C::kAStages; ++s) { mbar_init(&afull[s], 1); mbar_init(&aempty[s], 1); }
-    for (int s = 0; s < C::kGStages; ++s) { mbar_init(&gfull[s], 1); mbar_init(&gempty[s], 1); }
-    mbar_init(tmem_full, 1);
+    for (int s = 0; s < C::kAStages; ++s) { mbar_init(&afull[s], 1); mbar_init(&aempty[s], kConsumerWarps); }
+    for (int s = 0; s < C::kGStages; ++s) { mbar_init(&gfull[s], 1); mbar_init(&gempty[s], kConsumerWarps); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr, C::kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp == kConsumerWarps) {
     if (lane == 0) {
       int as = 0, gs = 0; uint32_t aph = 0, gph = 0;
       for (int t = t_begin; t < t_end; ++t) {
@@ -550,14 +499,14 @@ __global__ void __launch_bounds__(192, 1) k_conv_wgrad_tc2(const __grid_constant
         const int th_i = mt % g.tiles_h;
         const int tn_i = mt / g.tiles_h;
         const int w0 = tw_i * g.TW, h0 = th_i * g.TH, n0 = tn_i * g.TN;
-        mbar_wait(&gempty[gs], gph ^ 1, 10 + gs);
+        mbar_wait(&gempty[gs], gph ^ 1);
         mbar_expect_tx(&gfull[gs], C::kGStage);
         tma_load_4d(&tm_g_hi, &gfull[gs], sg + gs * C::kGStage, co0, w0, h0, n0);
         tma_load_4d(&tm_g_lo, &gfull[gs], sg + gs * C::kGStage + C::kGTile, co0, w0, h0, n0);
         if (++gs == C::kGStages) { gs = 0; gph ^= 1; }
         for (int grp = 0; grp < groups; ++grp) {
           const int tap0 = grp * TG, ntap = min(TG, taps - tap0);
-          mbar_wait(&aempty[as], aph ^ 1, 20 + as);
+          mbar_wait(&aempty[as], aph ^ 1);
           mbar_expect_tx(&afull[as], 2 * ntap * C::kXTile);
           uint8_t* base = sa + as * C::kAStage;
           for (int j = 0; j < ntap; ++j) {
@@ -570,1207 +519,77 @@ __global__ void __launch_bounds__(192, 1) k_conv_wgrad_tc2(const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(128, BNW, 1, 1);
-      constexpr uint32_t idesc2 = make_idesc(128, 2 * BNW, 1, 1);
-      constexpr uint32_t la = swizzle_layout_for(CN), lb = swizzle_layout_for(BNW >= 64 ? 64 : BNW);
-      constexpr uint32_t sbo_a = 8 * CN * 2, sbo_b = 8 * BNW * 2;        // stride between 8-pixel groups
-      int as = 0, gs = 0; uint32_t aph = 0, gph = 0;
-      for (int t = t_begin; t < t_end; ++t) {
-        mbar_wait(&gfull[gs], gph, 30 + gs);
-        tc_fence_after();
-        const uint32_t gb_hi = smem_u32(sg + gs * C::kGStage), gb_lo = gb_hi + C::kGTile;
-        for (int grp = 0; grp < groups; ++grp) {
-          mbar_wait(&afull[as], aph, 40 + as);
-          tc_fence_after();
-          const uint32_t xa_hi = smem_u32(sa + as * C::kAStage), xa_lo = xa_hi + TG * C::kXTile;
-          const uint32_t dbase = tmem_base + grp * C::kKAcc * C::kAccCols;
-          const uint64_t dah0 = make_desc(xa_hi, C::kXTile, sbo_a, la), dal0 = make_desc(xa_lo, C::kXTile, sbo_a, la);
-          const uint64_t dbh0 = make_desc(gb_hi, C::kGTile, sbo_b, lb), dbl0 = make_desc(gb_lo, C::kGTile, sbo_b, lb);
+    return;
+  }
+
+  const int wg = warp >> 2;
+  float acc[C::kMaxGroups][BNW / 2];
+#pragma unroll
+  for (int a = 0; a < C::kMaxGroups; ++a)
+#pragma unroll
+    for (int i = 0; i < BNW / 2; ++i) acc[a][i] = 0.f;
+  {
+    constexpr uint32_t la = swizzle_layout_for(CN), lb = swizzle_layout_for(BNW);
+    constexpr uint32_t sbo_a = 8 * CN * 2, sbo_b = 8 * BNW * 2;        // stride between 8-pixel groups (K)
+    int as = 0, gs = 0; uint32_t aph = 0, gph = 0;
+    for (int t = t_begin; t < t_end; ++t) {
+      mbar_wait(&gfull[gs], gph);
+      const uint32_t gb_hi = smem_u32(sg + gs * C::kGStage), gb_lo = gb_hi + C::kGTile;
+      const uint64_t dbh = make_desc(gb_hi, C::kGTile, sbo_b, lb), dbl = make_desc(gb_lo, C::kGTile, sbo_b, lb);
+#pragma unroll
+      for (int grp = 0; grp < C::kMaxGroups; ++grp) {
+        if (grp >= groups) break;
+        mbar_wait(&afull[as], aph);
+        if (grp * TG + wg * (TG / 2) < taps) {         // warpgroup-uniform: skip a half tile that holds no tap
+          const uint32_t xa_hi = smem_u32(sa + as * C::kAStage) + wg * (TG / 2) * C::kXTile, xa_lo = xa_hi + TG * C::kXTile;
+          const uint64_t dah = make_desc(xa_hi, C::kXTile, sbo_a, la), dal = make_desc(xa_lo, C::kXTile, sbo_a, la);
+          // one tile's 128 pixels go to a fresh fragment that is then added to the running sum with fp32 adds: a CTA
+          // covers up to ~10^4 pixels, and one tensor-core accumulation chain that long loses ~1e-4 relative
+          float part[BNW / 2];
+#pragma unroll
+          for (int i = 0; i < BNW / 2; ++i) part[i] = 0.f;
+          fence_acc(part);
+          wgmma_fence();
 #pragma unroll
           for (int ks = 0; ks < 128 / 16; ++ks) {          // 16 pixels per MMA
             const uint32_t offa = ks * 2 * sbo_a, offb = ks * 2 * sbo_b;
-            const uint32_t d = dbase + (ks % C::kKAcc) * C::kAccCols;
-            const uint32_t accum = (t != t_begin) || (ks >= C::kKAcc);
-            if (C::kCat) {
-              // B = [gy_hi | gy_lo]: the lo tile follows the hi tile at LBO = kGTile, i.e. it is the next N atom
-              umma_bf16(d, desc_add(dah0, offa), desc_add(dbh0, offb), idesc2, accum);
-              // x_lo . [gy_hi | gy_lo]: at N = 2*BNW <= 64 the lo.lo term costs nothing (an MMA takes the 54.5-cycle issue
-              // floor whatever its width below N = 128), so it is kept; wider, only x_lo . gy_hi is formed
-              umma_bf16(d, desc_add(dal0, offa), desc_add(dbh0, offb), (2 * BNW <= 64) ? idesc2 : idesc, 1);
-            } else {
-              umma_bf16(d, desc_add(dal0, offa), desc_add(dbh0, offb), idesc, accum);
-              umma_bf16(d, desc_add(dah0, offa), desc_add(dbl0, offb), idesc, 1);
-              umma_bf16(d, desc_add(dah0, offa), desc_add(dbh0, offb), idesc, 1);
-            }
+            Wgmma<BNW>::template mma<1, 1>(part, desc_add(dal, offa), desc_add(dbh, offb));
+            Wgmma<BNW>::template mma<1, 1>(part, desc_add(dah, offa), desc_add(dbl, offb));
+            Wgmma<BNW>::template mma<1, 1>(part, desc_add(dah, offa), desc_add(dbh, offb));
           }
-          umma_commit(&aempty[as]);
-          if (++as == C::kAStages) { as = 0; aph ^= 1; }
-        }
-        umma_commit(&gempty[gs]);
-        if (++gs == C::kGStages) { gs = 0; gph ^= 1; }
-      }
-      umma_commit(tmem_full);
-    }
-  } else if (t_begin < t_end) {
-    // TMEM lane m = (tap within group) * CN + ci holds gw[tap][ci][co0 .. co0+BNW).  Each 16-column chunk is staged
-    // through shared memory so that 4 consecutive lanes add one row's 64 contiguous bytes with float4 atomics
-    // (8 L2 transactions per warp instruction instead of 32 scalar ones).
-    const int q = warp & 3;
-    uint8_t* stg = se + q * (32 * C::kEpiPitch);
-    mbar_wait(tmem_full, 0, 50);
-    tc_fence_after();
-    for (int grp = 0; grp < groups; ++grp) {
-#pragma unroll 1
-      for (int c = 0; c < BNW; c += 16) {
-        float v[16];
-        const uint32_t t0 = tmem_base + ((uint32_t)(q * 32) << 16) + grp * C::kKAcc * C::kAccCols + c;
-        tmem_ld16(t0, v);
+          wgmma_commit();
+          wgmma_wait<0>();
+          fence_acc(part);
 #pragma unroll
-        for (int a = 0; a < C::kKAcc; ++a) {
-#pragma unroll
-          for (int hf = 0; hf < (C::kCat ? 2 : 1); ++hf) {
-            if (a == 0 && hf == 0) continue;
-            float u[16];
-            tmem_ld16(t0 + a * C::kAccCols + hf * BNW, u);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] += u[j];
-          }
-        }
-#pragma unroll
-        for (int j = 0; j < 16; j += 4)
-          *reinterpret_cast<float4*>(stg + lane * C::kEpiPitch + j * 4) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-        __syncwarp();
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int idx = i * 32 + lane;
-          const int row = idx >> 2, quad = idx & 3;          // row within this warp's 32 TMEM lanes
-          const int m = q * 32 + row;
-          const int tap = grp * TG + m / CN, ci = ci0 + (m % CN);
-          if (tap < taps && ci < g.Cin) {
-            const float4 val = *reinterpret_cast<const float4*>(stg + row * C::kEpiPitch + quad * 16);
-            atomicAdd(reinterpret_cast<float4*>(gw + ((int64_t)tap * g.Cin + ci) * g.Cout + co0 + c + quad * 4), val);
-          }
+          for (int i = 0; i < BNW / 2; ++i) acc[grp][i] += part[i];
         }
         __syncwarp();
+        if (lane == 0) mbar_arrive(&aempty[as]);
+        if (++as == C::kAStages) { as = 0; aph ^= 1; }
       }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&gempty[gs]);
+      if (++gs == C::kGStages) { gs = 0; gph ^= 1; }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, C::kTmemCols);
-}
-
-// ----------------------------------------------------------------------------------------------------
-// Halo weight gradient (3x3 SAME, W >= 16).  The tap-stacked kernel above fetches the x tile nine times (once per tap):
-// on the 16/32-channel high-resolution layers that is 640 B per pixel through L2 and the kernel is L2-bound (ncu,
-// [64,256,256,16]x[..16]: 530 us, L2 hit 77 %, tensor pipe 9 %); on the 64-channel-chunk layers the nine 32 KB fills per
-// tile compete with the MMAs' operand reads for shared-memory bandwidth (tensor pipe 38 %).  Here a pixel tile of
-// 8 rows x 16 pixels loads its x HALO once -- ONE box of 10 x 18 pixels per plane -- and every tap is the same bytes
-// seen through an MN-major descriptor: K-step = one tile row (16 pixels, contiguous in the halo row), tap (kh, kw) =
-// start address advanced by (kh*18 + kw) pixels.  Several taps share one M = 128 MMA because the M-atom stride (LBO) of
-// the descriptor is free: any set of taps whose offsets form an arithmetic progression is one operand --
-//   CN <= 32: per kernel row kh, atoms kw = 0, 1, 2, ... at LBO = ONE PIXEL (128/CN atoms, three of them real taps; the
-//             others read the pixels further right, and an accumulator row depends on its own operand row only, so
-//             those rows are simply never stored);
-//   CN = 64 : two atoms per MMA -- (kh,0)+(kh,1) at LBO = one pixel for kh = 0..2, (0,2)+(1,2) at LBO = one halo row,
-//             and (2,2)+unused: five accumulators, the same MMA count as tap stacking.
-// Fill per tile: 46-ish KB instead of nine tap tiles.  The accumulators are visited round-robin inside a K-step, so
-// consecutive MMAs never serialise on one accumulator.
-// ----------------------------------------------------------------------------------------------------
-template <int CN, int BNW>
-struct WgHaloCfg {
-  static constexpr int TH = 8, TW = 16, BW = TW + 2, BH = TH + 2;
-  static constexpr int kPx = CN * 2;                                      // bytes of one pixel of the x box
-  static constexpr int kBoxRaw = BH * BW * kPx;                           // one plane of the halo box
-  static constexpr int kBox = (kBoxRaw + 8 * kPx + 1023) / 1024 * 1024;   // + room for the unused atoms' reads
-  static constexpr int kGTile = 128 * BNW * 2;                            // gy tile, one plane
-  static constexpr int kStage = 2 * kBox + 2 * kGTile;
-  static constexpr int kStagesRaw = (196 * 1024) / kStage;
-  static constexpr int kStages = kStagesRaw > 4 ? 4 : (kStagesRaw < 2 ? 2 : kStagesRaw);
-  static constexpr int kEpiPitch = 16 * 4 + 16;
-  static constexpr int kEpiBytes = 4 * 32 * kEpiPitch;
-  static constexpr int kBytes = kStages * kStage + kEpiBytes + 1024 + 512;
-  static_assert(kBytes <= 227 * 1024, "halo wgrad exceeds shared memory");
-  // [gy_hi | gy_lo] is ONE N = 2*BNW operand for every shape: two MMAs per K-step (x_hi.[gy_hi|gy_lo], x_lo.gy_hi) instead
-  // of three.  64-channel chunks with BNW = 64 would need 5 x 128 = 640 TMEM columns, so their five tap groups are split
-  // into two SETS -- {0,1,2} and {3,4} -- handled by different CTAs (both load the same small halo; the MMA work, which
-  // is what bounds the kernel, is divided 3 : 2 and the launcher sizes the two CTA populations accordingly).
-  static constexpr bool kCat = true;
-  static constexpr int kGroups = (CN <= 32) ? 3 : 5;
-  static constexpr int kAccCols = 2 * BNW;
-  static constexpr bool kSplitSets = (kGroups * kAccCols > 512);
-  static constexpr int kGroupsPerCta = kSplitSets ? 3 : kGroups;
-  static constexpr uint32_t kNeed = kGroupsPerCta * kAccCols;
-  static constexpr uint32_t kTmemCols = kNeed <= 128 ? 128 : (kNeed <= 256 ? 256 : 512);
-  static_assert(kNeed <= 512, "halo wgrad exceeds TMEM");
-};
-
-// group -> (pixel offset of its first atom inside the halo, atom stride in pixels, taps of its atoms 0 and 1 [CN = 64])
-__device__ __forceinline__ void wg_halo_group(int cn, int grp, int bw, int& off_px, int& lbo_px, int& tap0, int& tap1) {
-  if (cn <= 32) { off_px = grp * bw; lbo_px = 1; tap0 = grp * 3; tap1 = grp * 3 + 1; return; }     // atoms kw = 0, 1, 2, ..
-  if (grp < 3) { off_px = grp * bw; lbo_px = 1; tap0 = grp * 3; tap1 = grp * 3 + 1; }
-  else if (grp == 3) { off_px = 2; lbo_px = bw; tap0 = 2; tap1 = 5; }
-  else { off_px = 2 * bw + 2; lbo_px = 1; tap0 = 8; tap1 = -1; }
-}
-
-template <int CN, int BNW>
-__global__ void __launch_bounds__(192, 1) k_conv_wgrad_halo(const __grid_constant__ CUtensorMap tm_g_hi,
-                                                            const __grid_constant__ CUtensorMap tm_g_lo,
-                                                            const __grid_constant__ CUtensorMap tm_x_hi,
-                                                            const __grid_constant__ CUtensorMap tm_x_lo,
-                                                            float* __restrict__ gw, int N, int H, int W, int Cin, int Cout,
-                                                            int tiles_w, int tiles_h, int tiles_per_cta, int ctas_set_a,
-                                                            int tiles_per_cta_b) {
-  // kSplitSets: blockIdx.x < ctas_set_a -> tap groups {0,1,2} over tiles_per_cta tiles each; the other CTAs -> groups
-  // {3,4} over tiles_per_cta_b tiles each.  Otherwise ctas_set_a = gridDim.x and every CTA handles all groups.
-  using C = WgHaloCfg<CN, BNW>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* se = smem + C::kStages * C::kStage;            // epilogue staging
-  uint64_t* bars = reinterpret_cast<uint64_t*>(se + C::kEpiBytes);
-  uint64_t* full = bars;
-  uint64_t* empty = full + C::kStages;
-  uint64_t* tmem_full = empty + C::kStages;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full + 1);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int co0 = blockIdx.y * BNW;
-  const int ci0 = blockIdx.z * CN;
-  const int total_tiles = N * tiles_h * tiles_w;
-  const bool set_b = C::kSplitSets && (int)blockIdx.x >= ctas_set_a;
-  const int g_first = set_b ? 3 : 0;
-  const int g_count = C::kSplitSets ? (set_b ? 2 : 3) : C::kGroups;
-  const int t_begin = set_b ? ((int)blockIdx.x - ctas_set_a) * tiles_per_cta_b : (int)blockIdx.x * tiles_per_cta;
-  const int t_end = min(total_tiles, t_begin + (set_b ? tiles_per_cta_b : tiles_per_cta));
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tm_g_hi); prefetch_tmap(&tm_g_lo); prefetch_tmap(&tm_x_hi); prefetch_tmap(&tm_x_lo);
-    for (int s = 0; s < C::kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(tmem_full, 1);
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc(tmem_ptr, C::kTmemCols);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int st = 0; uint32_t ph = 0;
-      for (int t = t_begin; t < t_end; ++t) {
-        int mt = t;
-        const int tw_i = mt % tiles_w; mt /= tiles_w;
-        const int th_i = mt % tiles_h;
-        const int n = mt / tiles_h;
-        const int w0 = tw_i * C::TW, h0 = th_i * C::TH;
-        mbar_wait(&empty[st], ph ^ 1, 300 + st);
-        uint8_t* base = smem + st * C::kStage;
-        mbar_expect_tx(&full[st], 2 * C::kBoxRaw + 2 * C::kGTile);
-        tma_load_4d(&tm_x_hi, &full[st], base, ci0, w0 - 1, h0 - 1, n);
-        tma_load_4d(&tm_x_lo, &full[st], base + C::kBox, ci0, w0 - 1, h0 - 1, n);
-        tma_load_4d(&tm_g_hi, &full[st], base + 2 * C::kBox, co0, w0, h0, n);
-        tma_load_4d(&tm_g_lo, &full[st], base + 2 * C::kBox + C::kGTile, co0, w0, h0, n);
-        if (++st == C::kStages) { st = 0; ph ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc1 = make_idesc(128, BNW, 1, 1);
-      constexpr uint32_t idesc2 = make_idesc(128, 2 * BNW, 1, 1);
-      constexpr uint32_t la = swizzle_layout_for(CN), lb = swizzle_layout_for(BNW >= 64 ? 64 : BNW);
-      constexpr uint32_t px = C::kPx;
-      constexpr uint32_t sbo_a = 8 * px, sbo_b = 8 * BNW * 2; // stride between 8-pixel groups along K
-      int st = 0; uint32_t ph = 0;
-      for (int t = t_begin; t < t_end; ++t) {
-        mbar_wait(&full[st], ph, 310 + st);
-        tc_fence_after();
-        const uint32_t base = smem_u32(smem + st * C::kStage);
-        const uint32_t gb_hi = base + 2 * C::kBox;
-        const uint64_t dbh0 = make_desc(gb_hi, C::kGTile, sbo_b, lb);     // N atoms: gy_hi then gy_lo (LBO = one plane)
+  if (t_begin >= t_end) return;
+  // accumulator row m = (tap within group) * CN + ci, column = output channel
+  const int quad = lane & 3;
 #pragma unroll
-        for (int r = 0; r < C::TH; ++r) {                     // K-step = tile row r (16 pixels)
-          const uint64_t dbh = desc_add(dbh0, r * 2 * sbo_b);
+  for (int grp = 0; grp < C::kMaxGroups; ++grp) {
+    if (grp >= groups) break;
 #pragma unroll
-          for (int gi = 0; gi < C::kGroupsPerCta; ++gi) {
-            if (gi >= g_count) break;
-            int off_px, lbo_px, tap0, tap1;
-            if constexpr (C::kSplitSets) {                     // group index is a run-time value only in this case
-              const int grp = g_first + gi;
-              off_px = grp < 3 ? grp * C::BW : (grp == 3 ? 2 : 2 * C::BW + 2);
-              lbo_px = grp == 3 ? C::BW : 1;
-            } else {
-              wg_halo_group(CN, gi, C::BW, off_px, lbo_px, tap0, tap1);
-            }
-            const uint32_t xa_hi = base + (r * C::BW + off_px) * px;
-            const uint64_t dah = make_desc(xa_hi, lbo_px * px, sbo_a, la), dal = make_desc(xa_hi + C::kBox, lbo_px * px, sbo_a, la);
-            const uint32_t d = tmem_base + gi * C::kAccCols;
-            const uint32_t accum = (t != t_begin) || (r != 0);
-            umma_bf16(d, dah, dbh, idesc2, accum);
-            umma_bf16(d, dal, dbh, (2 * BNW <= 64) ? idesc2 : idesc1, 1);   // + x_lo.gy_lo where the issue floor hides it
-          }
-        }
-        umma_commit(&empty[st]);
-        if (++st == C::kStages) { st = 0; ph ^= 1; }
-      }
-      umma_commit(tmem_full);
-    }
-  } else if (t_begin < t_end) {
-    // TMEM lane m = (atom = m / CN, ci = m % CN) of accumulator `grp`; atoms that are not taps are skipped.  Staged through
-    // shared memory for float4 atomics like the tap-stacked kernel.
-    const int q = warp & 3;
-    uint8_t* stg = se + q * (32 * C::kEpiPitch);
-    mbar_wait(tmem_full, 0, 320);
-    tc_fence_after();
-    for (int gi = 0; gi < g_count; ++gi) {
-      const int grp = g_first + gi;
-      int off_px, lbo_px, tap0, tap1;
-      wg_halo_group(CN, grp, C::BW, off_px, lbo_px, tap0, tap1);
-#pragma unroll 1
-      for (int c = 0; c < BNW; c += 16) {
-        float v[16], u[16];
-        const uint32_t t0 = tmem_base + ((uint32_t)(q * 32) << 16) + gi * C::kAccCols + c;
-        tmem_ld16(t0, v);
-        tmem_ld16(t0 + BNW, u);
+    for (int i = 0; i < 2; ++i) {
+      const int m = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
+      const int tap = grp * TG + m / CN, ci = ci0 + (m % CN);
+      if (tap >= taps || ci >= g.Cin) continue;
+      // gw here is the pixel-split partial buffer: slice blockIdx.x, summed over the splits in order by add_partials
+      float* dst = gw + (int64_t)blockIdx.x * taps * g.Cin * g.Cout + ((int64_t)tap * g.Cin + ci) * g.Cout + co0 + 2 * quad;
 #pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] += u[j];
-#pragma unroll
-        for (int j = 0; j < 16; j += 4)
-          *reinterpret_cast<float4*>(stg + lane * C::kEpiPitch + j * 4) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-        __syncwarp();
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int idx = i * 32 + lane;
-          const int row = idx >> 2, quad = idx & 3;
-          const int m = q * 32 + row;
-          const int atom = m / CN, ci = ci0 + (m % CN);
-          int tap;
-          if (CN <= 32) tap = (atom < 3) ? tap0 + atom : -1;
-          else tap = atom == 0 ? tap0 : tap1;
-          if (tap >= 0 && ci < Cin) {
-            const float4 val = *reinterpret_cast<const float4*>(stg + row * C::kEpiPitch + quad * 16);
-            atomicAdd(reinterpret_cast<float4*>(gw + ((int64_t)tap * Cin + ci) * Cout + co0 + c + quad * 4), val);
-          }
-        }
-        __syncwarp();
-      }
+      for (int j = 0; j < BNW / 8; ++j)
+        *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(acc[grp][4 * j + 2 * i], acc[grp][4 * j + 2 * i + 1]);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, C::kTmemCols);
-}
-
-// ----------------------------------------------------------------------------------------------------
-// Row-shift weight gradient (3x3 SAME, W >= 16, Cin chunk <= 64, Cout block <= 32 or Cin chunk <= 32).
-//
-// The halo kernel above issues one MMA pair per kernel ROW kh (three accumulators; the three kw taps of a row are the M
-// atoms), i.e. 6 MMAs per 16-pixel K-step, and every one of them costs the 54.5-cycle issue floor at N = 2*BNW <= 64:
-// the 16/32-channel layers run at ~10 % of the tensor pipe and 30 % of HBM.  The kh shift does not have to be applied
-// to x:   gw[kh][kw] = sum_p x[p_r+kh-1][p_c+kw-1] gy[p_r][p_c]  =  sum over x rows xr of  x[xr][.+kw-1] gy[xr-kh+1][.]
-// so for ONE x row the three kh taps are three gy ROWS -- and rows of a gy box are an arithmetic progression of shared
-// memory addresses, i.e. N atoms of one MN-major B operand (the atom stride LBO is free, like the kw atoms of A).  One
-// MMA then covers all nine taps:  D[(kw, ci)][(row j = 2-kh, plane, co)] += x_row[16 px] . gy_rows[16 px].
-//   * x box: TH rows x 18 pixels per plane (no row halo), atoms kw = 0,1,2,.. at LBO = one pixel as above.
-//   * gy box: (TH+2) rows x 16 pixels with the hi and lo planes INTERLEAVED BY ROW -- one 5-D TMA box over
-//     {C, W, plane, H, N} -- so (row j, plane) -> slot 2j+plane is one progression: for BNW = 16 all six are ONE N = 96
-//     operand and a K-step is 2 MMAs (x_hi.[..], x_lo.[..]; the lo.lo product is free under the issue floor) instead
-//     of 6; for BNW >= 32 the planes are separate N = 3*BNW operands (slot stride 2) and a K-step is 3 MMAs, all into
-//     the same accumulator (the epilogue only needs the sum of the partial products).
-//   * 64-channel chunks: two M groups -- atoms (kw0, kw1) and (kw2, unused).
-// Rows of gy outside the image are zero-filled by TMA, which is exactly the missing (x row, kh) pairs at the border.
-// ----------------------------------------------------------------------------------------------------
-template <int CN, int BNW>
-struct WgRowsCfg {
-  static constexpr int TH = 8, TW = 16, BW = TW + 2, GH = TH + 2;
-  static constexpr int kPx = CN * 2;                                      // bytes of one pixel of the x box
-  static constexpr int kXRaw = TH * BW * kPx;                             // one plane of the x box
-  static constexpr int kX = (kXRaw + 8 * kPx + 1023) / 1024 * 1024;       // + room for the unused atoms' reads
-  static constexpr int kGRow = TW * BNW * 2;                              // one gy row of one plane
-  static constexpr int kGRaw = GH * 2 * kGRow;                            // rows x planes, interleaved
-  static constexpr int kG = (kGRaw + 1023) / 1024 * 1024;
-  static constexpr int kStage = 2 * kX + kG;
-  static constexpr int kStagesRaw = (196 * 1024) / kStage;
-  static constexpr int kStages = kStagesRaw > 6 ? 6 : (kStagesRaw < 2 ? 2 : kStagesRaw);
-  static constexpr int kEpiPitch = 16 * 4 + 16;
-  static constexpr int kEpiBytes = 4 * 32 * kEpiPitch;
-  static constexpr int kBytes = kStages * kStage + kEpiBytes + 1024 + 512;
-  static_assert(kBytes <= 227 * 1024, "row-shift wgrad exceeds shared memory");
-  static constexpr bool kCat6 = (BNW == 16);            // all six (row, plane) slots in one N = 96 operand
-  static constexpr int kMGroups = (CN == 64) ? 2 : 1;
-  static constexpr int kAccCols = kCat6 ? 96 : 3 * BNW;
-  static constexpr uint32_t kNeed = kMGroups * kAccCols;
-  static constexpr uint32_t kTmemCols = kNeed <= 128 ? 128 : (kNeed <= 256 ? 256 : 512);
-  static_assert(kNeed <= 512, "row-shift wgrad exceeds TMEM");
-};
-
-__device__ __forceinline__ void tma_load_5d(const CUtensorMap* tm, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3,
-                                            int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
-
-template <int CN, int BNW>
-__global__ void __launch_bounds__(192, 1) k_conv_wgrad_rows(const __grid_constant__ CUtensorMap tm_g,
-                                                            const __grid_constant__ CUtensorMap tm_x_hi,
-                                                            const __grid_constant__ CUtensorMap tm_x_lo,
-                                                            float* __restrict__ gw, int N, int H, int W, int Cin, int Cout,
-                                                            int tiles_w, int tiles_h, int tiles_per_cta) {
-  using C = WgRowsCfg<CN, BNW>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* se = smem + C::kStages * C::kStage;            // epilogue staging
-  uint64_t* bars = reinterpret_cast<uint64_t*>(se + C::kEpiBytes);
-  uint64_t* full = bars;
-  uint64_t* empty = full + C::kStages;
-  uint64_t* tmem_full = empty + C::kStages;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full + 1);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int co0 = blockIdx.y * BNW;
-  const int ci0 = blockIdx.z * CN;
-  const int total_tiles = N * tiles_h * tiles_w;
-  const int t_begin = (int)blockIdx.x * tiles_per_cta;
-  const int t_end = min(total_tiles, t_begin + tiles_per_cta);
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tm_g); prefetch_tmap(&tm_x_hi); prefetch_tmap(&tm_x_lo);
-    for (int s = 0; s < C::kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(tmem_full, 1);
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc(tmem_ptr, C::kTmemCols);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int st = 0; uint32_t ph = 0;
-      for (int t = t_begin; t < t_end; ++t) {
-        int mt = t;
-        const int tw_i = mt % tiles_w; mt /= tiles_w;
-        const int th_i = mt % tiles_h;
-        const int n = mt / tiles_h;
-        const int w0 = tw_i * C::TW, h0 = th_i * C::TH;
-        mbar_wait(&empty[st], ph ^ 1, 330 + st);
-        uint8_t* base = smem + st * C::kStage;
-        mbar_expect_tx(&full[st], 2 * C::kXRaw + C::kGRaw);
-        tma_load_4d(&tm_x_hi, &full[st], base, ci0, w0 - 1, h0, n);
-        tma_load_4d(&tm_x_lo, &full[st], base + C::kX, ci0, w0 - 1, h0, n);
-        tma_load_5d(&tm_g, &full[st], base + 2 * C::kX, co0, w0, 0, h0 - 1, n);
-        if (++st == C::kStages) { st = 0; ph ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(128, C::kAccCols, 1, 1);
-      constexpr uint32_t la = swizzle_layout_for(CN), lb = swizzle_layout_for(BNW);
-      constexpr uint32_t px = C::kPx;
-      constexpr uint32_t sbo_a = 8 * px, sbo_b = 8 * BNW * 2; // stride between 8-pixel groups along K
-      int st = 0; uint32_t ph = 0;
-      for (int t = t_begin; t < t_end; ++t) {
-        mbar_wait(&full[st], ph, 340 + st);
-        tc_fence_after();
-        const uint32_t base = smem_u32(smem + st * C::kStage);
-        const uint32_t gb = base + 2 * C::kX;
-        // B: N atoms = gy box slots (row, plane) -> 2*row + plane.  kCat6: six consecutive slots; else three slots of one plane
-        const uint64_t db0 = make_desc(gb, (C::kCat6 ? 1 : 2) * C::kGRow, sbo_b, lb);
-#pragma unroll
-        for (int r = 0; r < C::TH; ++r) {                     // K-step = x row r (16 pixels), gy rows r .. r+2 of the box
-          const uint64_t dbh = desc_add(db0, (2 * r) * C::kGRow);
-          const uint64_t dbl = desc_add(db0, (2 * r + 1) * C::kGRow);
-#pragma unroll
-          for (int mg = 0; mg < C::kMGroups; ++mg) {
-            const uint32_t xa_hi = base + (r * C::BW + 2 * mg) * px;       // group 1 (CN = 64): atom 0 = kw 2
-            const uint64_t dah = make_desc(xa_hi, px, sbo_a, la), dal = make_desc(xa_hi + C::kX, px, sbo_a, la);
-            const uint32_t d = tmem_base + mg * C::kAccCols;
-            const uint32_t accum = (t != t_begin) || (r != 0);
-            if constexpr (C::kCat6) {
-              umma_bf16(d, dah, dbh, idesc, accum);
-              umma_bf16(d, dal, dbh, idesc, 1);              // + x_lo.gy_lo, free under the issue floor
-            } else {
-              umma_bf16(d, dah, dbh, idesc, accum);
-              umma_bf16(d, dah, dbl, idesc, 1);
-              umma_bf16(d, dal, dbh, idesc, 1);
-            }
-          }
-        }
-        umma_commit(&empty[st]);
-        if (++st == C::kStages) { st = 0; ph ^= 1; }
-      }
-      umma_commit(tmem_full);
-    }
-  } else if (t_begin < t_end) {
-    // TMEM lane m = (atom = m / CN -> kw, ci = m % CN); columns: kCat6 (2j+plane)*16 + co, else j*BNW + co; kh = 2 - j
-    const int q = warp & 3;
-    uint8_t* stg = se + q * (32 * C::kEpiPitch);
-    mbar_wait(tmem_full, 0, 350);
-    tc_fence_after();
-    for (int mg = 0; mg < C::kMGroups; ++mg) {
-#pragma unroll 1
-      for (int j = 0; j < 3; ++j) {
-#pragma unroll 1
-        for (int c = 0; c < BNW; c += 16) {
-          float v[16];
-          const uint32_t t0 = tmem_base + ((uint32_t)(q * 32) << 16) + mg * C::kAccCols;
-          if constexpr (C::kCat6) {
-            float u[16];
-            tmem_ld16(t0 + (2 * j) * 16, v);
-            tmem_ld16(t0 + (2 * j + 1) * 16, u);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] += u[i];
-          } else {
-            tmem_ld16(t0 + j * BNW + c, v);
-          }
-#pragma unroll
-          for (int i = 0; i < 16; i += 4)
-            *reinterpret_cast<float4*>(stg + lane * C::kEpiPitch + i * 4) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-          __syncwarp();
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int idx = i * 32 + lane;
-            const int row = idx >> 2, quad = idx & 3;
-            const int m = q * 32 + row;
-            const int atom = m / CN, ci = ci0 + (m % CN);
-            const int kw = (CN == 64) ? (mg == 0 ? atom : (atom == 0 ? 2 : -1)) : (atom < 3 ? atom : -1);
-            if (kw >= 0 && ci < Cin) {
-              const int tap = (2 - j) * 3 + kw;
-              const float4 val = *reinterpret_cast<const float4*>(stg + row * C::kEpiPitch + quad * 16);
-              atomicAdd(reinterpret_cast<float4*>(gw + ((int64_t)tap * Cin + ci) * Cout + co0 + c + quad * 4), val);
-            }
-          }
-          __syncwarp();
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, C::kTmemCols);
-}
-
-// ----------------------------------------------------------------------------------------------------
-// Halo-tile forward / dgrad kernel for the small-channel, high-resolution layers (Cin*Cout <= 2048: the
-// 16..64-channel layers at 64^2..256^2 that carry >80 % of the activation bytes and are HBM/L2 bound).
-//
-// The tap-per-TMA kernel above re-reads every input pixel 9 times from L2.  Here each output tile of 16 x (8*SUB)
-// pixels loads its 18 x (8*SUB+2) input halo ONCE, as [8-channel chunk][halo row][halo col][8 ch] (one TMA box per
-// chunk and plane), which is exactly the no-swizzle K-major UMMA layout with 16-byte rows:  row m = th*8+tw of the
-// tap-(kh,kw) operand of sub-tile s sits at  halo + ((th+kh)*HWID + (8*s+tw+kw))*16  =>  the 9*SUB im2col operands
-// are the SAME bytes seen through descriptors that differ only in their start address (SBO = one halo row, LBO = one
-// channel chunk).  (The swizzled pixel-major variant -- shifted views of a 32/64/128B-swizzled halo, base_offset 0 --
-// was validated too and runs at the same speed, see DESIGN.md 3.2; it is not kept in the kernel.)
-// The split-bf16 weights of all nine taps stay resident in shared memory as [tap][chunk][B_hi rows | B_lo rows][8], so
-// [B_hi | B_lo] is ONE N = 2*BN operand (2 MMAs per K-step instead of 3).  CTAs are persistent (one per SM, static
-// round-robin over tiles) with a multi-stage halo ring and two TMEM accumulator stages; SUB M=128 sub-tiles share one
-// halo load and one commit/epilogue hand-over, which amortises the ~900-cycle per-hand-over constant measured with
-// SUB = 1.  The epilogue adds the hi.lo half, fuses bias + leaky-ReLU (discriminator layers), stages each warp's 32
-// pixel rows in padded shared memory and drains them with fully coalesced 512-byte warp stores (optionally also as
-// split-bf16 planes for the next conv) while the next tile's MMAs run.
-// ----------------------------------------------------------------------------------------------------
-template <int CIN, int BN, int SUB_>
-struct HaloCfg {
-  // SUB M=128 sub-tiles per halo tile, bounded by TMEM (4*SUB*BN <= 512 columns) and by the halo stage size in smem
-  static constexpr int SUB = SUB_;
-  static_assert(4 * SUB * BN <= 512, "halo kernel exceeds TMEM");
-  static constexpr int TH = 16, TW = 8 * SUB, HH = TH + 2, HWID = TW + 2;
-  static constexpr int kChunks = CIN / 8;
-  static constexpr int kChunkBytes = HH * HWID * 16;              // one 8-channel chunk of one plane
-  static constexpr int kChunkStride = ((kChunkBytes + 127) / 128) * 128;
-  static constexpr int kPlane = kChunks * kChunkStride;
-  static constexpr int kStage = ((2 * kPlane + 1023) / 1024) * 1024;   // hi + lo
-  static constexpr int kWTap = CIN * BN * 2;                      // bytes per tap, one plane: [chunk][BN][8]
-  static constexpr int kWBytes = ((2 * 9 * kWTap + 1023) / 1024) * 1024;
-  static constexpr int kEpiPitch = BN * 4 + 16;                   // padded row: conflict-free float4 staging
-  static constexpr int kEpiWarp = 32 * kEpiPitch;                 // one epilogue warp owns 32 output pixels
-  static constexpr int kEpiBytes = ((8 * kEpiWarp + 1023) / 1024) * 1024;   // two epilogue groups of 4 warps
-  static constexpr int kStagesRaw = (200 * 1024 - kWBytes - kEpiBytes - 2048) / kStage;
-  static constexpr int kStages = kStagesRaw > 6 ? 6 : (kStagesRaw < 2 ? 2 : kStagesRaw);
-  static constexpr int kBytes = kWBytes + kStages * kStage + kEpiBytes + 1024 + 512;
-  static_assert(kBytes <= 227 * 1024, "halo kernel exceeds shared memory");
-  static constexpr int kStageCols = SUB * 2 * BN;                 // per sub-tile: [hi.hi+lo.hi | hi.lo]
-  static constexpr uint32_t kTmemCols = (2 * kStageCols <= 64) ? 64 : (2 * kStageCols <= 128 ? 128 : (2 * kStageCols <= 256 ? 256 : 512));
-};
-
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// EPI: which epilogue is compiled in -- 0 plain (dgrad / generic forward; bias + leaky-ReLU, planes and the sign mask are
-// run-time options of it), 1 = + instance-norm statistics records, 2 = evaluation-mode affine + leaky-ReLU + pixel norm.
-// Separate instantiations: the options of one mode cost registers and issue slots in the drain loop of the others (measured
-// +0.4 ms per training step when the inference epilogue was a run-time branch).
-template <int CIN, int BN, int SUBT, int EPI>
-__global__ void __launch_bounds__(320, 1) k_conv_halo_tc(const __grid_constant__ CUtensorMap tm_hi,
-                                                         const __grid_constant__ CUtensorMap tm_lo,
-                                                         const __nv_bfloat16* __restrict__ w_planes,  // [2][9][BN][CIN]
-                                                         float* __restrict__ y, int N, int H, int W, int tiles_w,
-                                                         int tiles_h, const float* __restrict__ bias, int act,
-                                                         void* __restrict__ z_planes, float4* __restrict__ stats_,
-                                                         uint8_t* __restrict__ act_mask_, const float* __restrict__ aff_a_) {
-  float4* const stats = (EPI == 1) ? stats_ : nullptr;
-  uint8_t* const act_mask = (EPI == 0) ? act_mask_ : nullptr;
-  const float* const aff_a = (EPI == 2) ? aff_a_ : nullptr;
-  // aff_a != null: inference-mode generator layer fused into the epilogue -- z = pixel_norm?(lrelu?(aff_a[c] * conv + bias[c]))
-  // with the per-channel affine of a normaliser in evaluation mode (moving statistics); act bit 0 = leaky-ReLU, bit 1 =
-  // pixel norm (a TMEM lane holds all BN = Cout channels of its pixel, so the pixel's mean square is a register sum)
-  using C = HaloCfg<CIN, BN, SUBT>;
-  constexpr int kStages = C::kStages;
-  constexpr int SUB = C::SUB;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sw = smem;                                  // weights: [tap][chunk][hi rows | lo rows][8] bf16
-  uint8_t* sh = smem + C::kWBytes;                     // halo ring: [stage][plane][chunk][18][HWID][8] bf16
-  uint8_t* se = sh + kStages * C::kStage;              // epilogue staging: [4 warps][32 pixels][BN fp32 + pad]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(se + C::kEpiBytes);
-  uint64_t* full = bars;                    // [kStages]
-  uint64_t* empty = full + kStages;         // [kStages]
-  uint64_t* tfull = empty + kStages;        // [2] accumulator stage ready
-  uint64_t* tempty = tfull + 2;             // [2] accumulator stage drained (4 epilogue warps arrive)
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tempty + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int total_tiles = N * tiles_h * tiles_w;
-
-  // resident weights: global [plane][tap][co][ci] -> smem [tap][ci/8][plane*BN + co][ci%8], 16 bytes at a time:
-  // rows 0..BN-1 of a (tap, chunk) block are B_hi, rows BN..2BN-1 are B_lo
-  {
-    constexpr int kVecPerPlane = 9 * BN * C::kChunks;
-    const uint4* src = reinterpret_cast<const uint4*>(w_planes);
-    for (int i = threadIdx.x; i < 2 * kVecPerPlane; i += blockDim.x) {
-      const int plane = i / kVecPerPlane;
-      int r = i - plane * kVecPerPlane;
-      const int chunk = r % C::kChunks; r /= C::kChunks;
-      const int co = r % BN;
-      const int tap = r / BN;
-      const uint4 v = src[i];
-      *reinterpret_cast<uint4*>(sw + tap * (2 * C::kWTap) + (chunk * 2 * BN + plane * BN + co) * 16) = v;
-    }
-  }
-  fence_proxy_async();
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tm_hi); prefetch_tmap(&tm_lo);
-    for (int s = 0; s < kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tfull[s], 1); mbar_init(&tempty[s], 4); }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc(tmem_ptr, C::kTmemCols);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        int t = tile;
-        const int tw_i = t % tiles_w; t /= tiles_w;
-        const int th_i = t % tiles_h;
-        const int n = t / tiles_h;
-        const int w0 = tw_i * C::TW - 1, h0 = th_i * C::TH - 1;
-        mbar_wait(&empty[stage], phase ^ 1, 100 + stage);
-        uint8_t* dst = sh + stage * C::kStage;
-        mbar_expect_tx(&full[stage], 2 * C::kChunks * C::kChunkBytes);
-#pragma unroll
-        for (int c = 0; c < C::kChunks; ++c) {
-          tma_load_4d(&tm_hi, &full[stage], dst + c * C::kChunkStride, c * 8, w0, h0, n);
-          tma_load_4d(&tm_lo, &full[stage], dst + C::kPlane + c * C::kChunkStride, c * 8, w0, h0, n);
-        }
-        if (++stage == kStages) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc1 = make_idesc(128, BN, 0, 0);        // A_lo . B_hi
-      constexpr uint32_t idesc2 = make_idesc(128, 2 * BN, 0, 0);    // A_hi . [B_hi | B_lo]
-      constexpr uint32_t sbo_a = C::HWID * 16, lbo_a = C::kChunkStride;   // halo row / channel chunk
-      constexpr uint32_t sbo_b = 128, lbo_b = 2 * BN * 16;
-      const uint64_t wdesc = make_desc(smem_u32(sw), lbo_b, sbo_b, 0);
-      int stage = 0, as = 0; uint32_t phase = 0, aphase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        mbar_wait(&tempty[as], aphase ^ 1, 110 + as);
-        mbar_wait(&full[stage], phase, 120 + stage);
-        tc_fence_after();
-        const uint32_t a_hi = smem_u32(sh + stage * C::kStage);
-        const uint64_t ahd = make_desc(a_hi, lbo_a, sbo_a, 0), ald = make_desc(a_hi + C::kPlane, lbo_a, sbo_a, 0);
-        const uint32_t d0 = tmem_base + as * C::kStageCols;
-#pragma unroll
-        for (int sub = 0; sub < SUB; ++sub) {
-          const uint32_t d = d0 + sub * 2 * BN;
-#pragma unroll
-          for (int tap = 0; tap < 9; ++tap) {
-#pragma unroll
-            for (int ks = 0; ks < CIN / 16; ++ks) {
-              const uint32_t offa = ((tap / 3) * C::HWID + (8 * sub + tap % 3)) * 16 + ks * 2 * lbo_a;
-              const uint64_t db = desc_add(wdesc, tap * (2 * C::kWTap) + ks * 2 * lbo_b);
-              umma_bf16(d, desc_add(ahd, offa), db, idesc2, (tap | ks) != 0);   // cols [0,BN) += hi.hi ; [BN,2BN) += hi.lo
-              // cols [0,BN) += lo.hi; at N = 2*BN <= 64 the MMA costs the same 54.5-cycle issue floor, so lo.lo comes free
-              umma_bf16(d, desc_add(ald, offa), db, (2 * BN <= 64) ? idesc2 : idesc1, 1);
-            }
-          }
-        }
-        umma_commit(&empty[stage]);
-        umma_commit(&tfull[as]);
-        if (++stage == kStages) { stage = 0; phase ^= 1; }
-        if (++as == 2) { as = 0; aphase ^= 1; }
-      }
-    }
-  } else {
-    // two epilogue groups of four warps (one warp per TMEM lane quarter): group g drains accumulator stage g, i.e.
-    // every other tile, so two tiles' epilogues and the next tile's MMAs are in flight at once
-    const int q = warp & 3;
-    const int grp = (warp - 2) >> 2;
-    uint8_t* stg = se + (grp * 4 + q) * C::kEpiWarp;   // this warp's 32 pixel rows
-    constexpr int kQuads = BN / 4;                     // float4 per pixel
-    uint32_t aphase = 0;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-      if ((it & 1) != grp) continue;
-      int t = tile;
-      const int tw_i = t % tiles_w; t /= tiles_w;
-      const int th_i = t % tiles_h;
-      const int n = t / tiles_h;
-      mbar_wait(&tfull[grp], aphase, 130 + grp);
-      aphase ^= 1;
-      tc_fence_after();
-      // normaliser statistics from the epilogue (stats != null): in the drain loop a lane always owns the same four
-      // channels (32 % kQuads == 0), so it sums (v - p) and (v - p)^2 over its pixels of the tile's SUB sub-tiles around the
-      // pivot p = this warp's first pixel; one {count, p, S1, S2} record per (warp, channel) goes to global memory and
-      // twg_norm_finalize_partials merges the records (no atomics, no second pass over y)
-      float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f}, cnt = 0.f;
-      float4 pv = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll 1
-      for (int sub = 0; sub < SUB; ++sub) {
-        // TMEM lane (= pixel q*32+lane of this sub-tile) -> registers: all 2*BN columns ([hi.hi+lo.hi | hi.lo]) are
-        // requested back to back and waited for once, then the halves are added and the pixel row is staged
-        uint32_t r[2 * BN];
-        const uint32_t t0 = tmem_base + ((uint32_t)(q * 32) << 16) + grp * C::kStageCols + sub * 2 * BN;
-#pragma unroll
-        for (int c = 0; c < 2 * BN; c += 16) tmem_ld16_issue(t0 + c, r + c);
-        tmem_ld_wait();
-        if (sub == SUB - 1) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tempty[grp]);     // accumulator stage free for the MMA warp again
-        }
-        float rinv = 1.f;
-        if (aff_a) {
-          float ss = 0.f;
-#pragma unroll
-          for (int c = 0; c < BN; ++c) {
-            float t = __uint_as_float(r[c]) + __uint_as_float(r[BN + c]);
-            t = fmaf(__ldg(aff_a + c), t, __ldg(bias + c));
-            if (act & 1) t = lrelu(t);
-            ss = fmaf(t, t, ss);
-            r[c] = __float_as_uint(t);
-          }
-          if (act & 2) rinv = rsqrtf(ss * (1.f / (float)BN) + kPixEps);
-        }
-#pragma unroll
-        for (int c = 0; c < BN; c += 4) {
-          float v[4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            if (aff_a) {
-              v[j] = __uint_as_float(r[c + j]) * rinv;
-            } else {
-              v[j] = __uint_as_float(r[c + j]) + __uint_as_float(r[BN + c + j]);
-              if (bias) {   // fused discriminator epilogue: + bias, leaky-ReLU
-                v[j] += __ldg(bias + c + j);
-                if (act & 1) v[j] = lrelu(v[j]);
-              }
-            }
-          }
-          *reinterpret_cast<float4*>(stg + lane * C::kEpiPitch + c * 4) = make_float4(v[0], v[1], v[2], v[3]);
-        }
-        __syncwarp();
-        if (stats && sub == 0) pv = *reinterpret_cast<const float4*>(stg + (lane % kQuads) * 16);   // pixel 0 of this warp
-        // coalesced drain: consecutive lanes write consecutive 16 B of consecutive pixels (8 pixels of a tile row are
-        // 8*BN*4 contiguous bytes in NHWC)
-#pragma unroll
-        for (int i = 0; i < kQuads; ++i) {
-          const int idx = i * 32 + lane;
-          const int pl = idx / kQuads, qd = idx % kQuads;            // pixel within the warp's 32, float4 within pixel
-          const int m = q * 32 + pl;
-          const int h = th_i * C::TH + m / 8, w = tw_i * C::TW + sub * 8 + m % 8;
-          const float4 val = *reinterpret_cast<const float4*>(stg + pl * C::kEpiPitch + qd * 16);
-          if (h < H && w < W) {
-            const int64_t e = (((int64_t)n * H + h) * W + w) * BN + qd * 4;
-            if (y) *reinterpret_cast<float4*>(y + e) = val;
-            if (z_planes) st_planes4(z_planes, (int64_t)N * H * W * BN, e >> 2, val);
-            // sign mask of the activation (4 bits per float4): the activation backward reads 0.25 B instead of 4 B per element
-            if (act_mask)
-              act_mask[e >> 2] = (uint8_t)((val.x > 0.f ? 1 : 0) | (val.y > 0.f ? 2 : 0) | (val.z > 0.f ? 4 : 0) | (val.w > 0.f ? 8 : 0));
-            if (stats) {
-              const float d0 = val.x - pv.x, d1 = val.y - pv.y, d2 = val.z - pv.z, d3 = val.w - pv.w;
-              s1[0] += d0; s1[1] += d1; s1[2] += d2; s1[3] += d3;
-              s2[0] = fmaf(d0, d0, s2[0]); s2[1] = fmaf(d1, d1, s2[1]); s2[2] = fmaf(d2, d2, s2[2]); s2[3] = fmaf(d3, d3, s2[3]);
-              cnt += 1.f;
-            }
-          }
-        }
-        __syncwarp();
-      }
-      if (stats) {
-        // lanes with equal lane % kQuads hold the same channel quad: fold them, then lanes 0..kQuads-1 write the records
-#pragma unroll
-        for (int off = kQuads; off < 32; off <<= 1) {
-          cnt += __shfl_xor_sync(0xffffffffu, cnt, off);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            s1[j] += __shfl_xor_sync(0xffffffffu, s1[j], off);
-            s2[j] += __shfl_xor_sync(0xffffffffu, s2[j], off);
-          }
-        }
-        if (lane < kQuads) {
-          const int slot = (th_i * tiles_w + tw_i) * 4 + q;
-          float4* dst = stats + ((int64_t)n * (tiles_h * tiles_w * 4) + slot) * BN + lane * 4;
-          dst[0] = make_float4(cnt, pv.x, s1[0], s2[0]);
-          dst[1] = make_float4(cnt, pv.y, s1[1], s2[1]);
-          dst[2] = make_float4(cnt, pv.z, s1[2], s2[2]);
-          dst[3] = make_float4(cnt, pv.w, s1[3], s2[3]);
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, C::kTmemCols);
-}
-
-// ----------------------------------------------------------------------------------------------------
-// Wide-layer halo kernel (Cin a multiple of 64, Cout >= 64, 3x3 SAME, H, W >= 16): forward / dgrad.
-//
-// The tap-per-TMA kernel above re-fetches the activation tile once per tap (nine 32 KB fills per 64-channel chunk) and
-// runs one CTA per tile, so TMEM allocation, barrier set-up, pipeline fill and the whole epilogue are exposed per tile;
-// ncu puts its tensor pipe at 55-65 % (profiles/r02_ncu_summary.md).  Here
-//   * each output tile of 16 x 8 pixels loads its 18 x 10 halo ONCE per 64-channel chunk (one TMA box per plane,
-//     128B-swizzled rows of 64 channels): the nine im2col operands are the same bytes seen through descriptors whose
-//     start address is advanced by (kh*10 + kw) rows -- shifted views of a swizzled tile are valid operands because the
-//     swizzle acts on absolute shared-memory address bits (DESIGN.md 3.2); SBO = one halo row (10 pixels);
-//   * only the weights stream per tap ([B_hi | B_lo] as ONE N = 2*BN operand, as in the tap kernel);
-//   * CTAs are persistent (static round-robin over (tile, Cout block) items) with two TMEM accumulator stages, so the
-//     epilogue of one item overlaps the MMAs of the next, and two epilogue warp groups alternate over items.
-// Shared-memory traffic per 64-channel chunk drops from 576 KB of TMA fill to 46 + 288 KB.
-// ----------------------------------------------------------------------------------------------------
-template <int BN>
-struct HTapCfg {
-  static constexpr int TH = 16, TW = 8, HH = 18, HWID = 10;
-  static constexpr int kPlaneRaw = HH * HWID * 128;                       // one plane of one 64-channel chunk: 23040 B
-  static constexpr int kPlane = (kPlaneRaw + 1023) / 1024 * 1024;
-  static constexpr int kHaloStage = 2 * kPlane;                           // hi + lo
-  static constexpr int kHaloStages = 2;
-  static constexpr int kBTile = BN * 128;                                 // one plane of one (chunk, tap) weight tile
-  static constexpr int kBStage = 2 * kBTile;
-  static constexpr int kBStages = (BN >= 128) ? 3 : 4;
-  static constexpr int kBytes = kHaloStages * kHaloStage + kBStages * kBStage + 1024 + 512;
-  static_assert(kBytes <= 227 * 1024, "wide halo kernel exceeds shared memory");
-  static constexpr uint32_t kAccCols = 2 * BN;                            // [hi.hi + lo.hi | hi.lo]
-  static constexpr uint32_t kTmemCols = (2 * kAccCols <= 256) ? 256 : 512;
-};
-
-template <int BN>
-__global__ void __launch_bounds__(320, 1) k_conv_htap_tc(const __grid_constant__ CUtensorMap tm_a_hi,
-                                                         const __grid_constant__ CUtensorMap tm_a_lo,
-                                                         const __grid_constant__ CUtensorMap tm_b_hi,
-                                                         const __grid_constant__ CUtensorMap tm_b_lo,
-                                                         float* __restrict__ y, int N, int H, int W, int Cin, int Cout,
-                                                         int tiles_w, int tiles_h, const float* __restrict__ bias, int act,
-                                                         void* __restrict__ z_planes) {
-  using C = HTapCfg<BN>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sh = smem;                                            // halo ring
-  uint8_t* sb = smem + C::kHaloStages * C::kHaloStage;           // weight ring
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sb + C::kBStages * C::kBStage);
-  uint64_t* hfull = bars;                          // [kHaloStages]
-  uint64_t* hempty = hfull + C::kHaloStages;
-  uint64_t* bfull = hempty + C::kHaloStages;       // [kBStages]
-  uint64_t* bempty = bfull + C::kBStages;
-  uint64_t* tfull = bempty + C::kBStages;          // [2]
-  uint64_t* tempty = tfull + 2;                    // [2] (4 epilogue warps arrive)
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tempty + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int chunks = Cin / 64, nblk = Cout / BN;
-  const int total_items = N * tiles_h * tiles_w * nblk;          // Cout block fastest: neighbours share the halo in L2
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_a_lo); prefetch_tmap(&tm_b_hi); prefetch_tmap(&tm_b_lo);
-    for (int s = 0; s < C::kHaloStages; ++s) { mbar_init(&hfull[s], 1); mbar_init(&hempty[s], 1); }
-    for (int s = 0; s < C::kBStages; ++s) { mbar_init(&bfull[s], 1); mbar_init(&bempty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tfull[s], 1); mbar_init(&tempty[s], 4); }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc(tmem_ptr, C::kTmemCols);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int hs = 0, bs = 0; uint32_t hph = 0, bph = 0;
-      for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-        int t = item;
-        const int nb = t % nblk; t /= nblk;
-        const int tw_i = t % tiles_w; t /= tiles_w;
-        const int th_i = t % tiles_h;
-        const int n = t / tiles_h;
-        const int w0 = tw_i * C::TW - 1, h0 = th_i * C::TH - 1;
-        for (int cc = 0; cc < chunks; ++cc) {
-          mbar_wait(&hempty[hs], hph ^ 1, 200 + hs);
-          uint8_t* dst = sh + hs * C::kHaloStage;
-          mbar_expect_tx(&hfull[hs], 2 * C::kPlaneRaw);
-          tma_load_4d(&tm_a_hi, &hfull[hs], dst, cc * 64, w0, h0, n);
-          tma_load_4d(&tm_a_lo, &hfull[hs], dst + C::kPlane, cc * 64, w0, h0, n);
-          if (++hs == C::kHaloStages) { hs = 0; hph ^= 1; }
-          for (int tap = 0; tap < 9; ++tap) {
-            mbar_wait(&bempty[bs], bph ^ 1, 210 + bs);
-            uint8_t* db = sb + bs * C::kBStage;
-            mbar_expect_tx(&bfull[bs], C::kBStage);
-            tma_load_2d(&tm_b_hi, &bfull[bs], db, cc * 64, tap * Cout + nb * BN);
-            tma_load_2d(&tm_b_lo, &bfull[bs], db + C::kBTile, cc * 64, tap * Cout + nb * BN);
-            if (++bs == C::kBStages) { bs = 0; bph ^= 1; }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc1 = make_idesc(128, BN, 0, 0);        // A_lo . B_hi
-      constexpr uint32_t idesc2 = make_idesc(128, 2 * BN, 0, 0);    // A_hi . [B_hi | B_lo]
-      constexpr uint32_t sbo_a = C::HWID * 128;                     // next 8-pixel group of the tile = next halo row
-      constexpr uint32_t sbo_b = 8 * 128;
-      int hs = 0, bs = 0, as = 0; uint32_t hph = 0, bph = 0, aph = 0;
-      for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-        mbar_wait(&tempty[as], aph ^ 1, 220 + as);
-        tc_fence_after();
-        const uint32_t d = tmem_base + as * C::kAccCols;
-        for (int cc = 0; cc < chunks; ++cc) {
-          mbar_wait(&hfull[hs], hph, 230 + hs);
-          tc_fence_after();
-          const uint32_t a_hi = smem_u32(sh + hs * C::kHaloStage);
-          const uint64_t dah = make_desc(a_hi, 16, sbo_a, 2), dal = make_desc(a_hi + C::kPlane, 16, sbo_a, 2);
-          for (int tap = 0; tap < 9; ++tap) {
-            mbar_wait(&bfull[bs], bph, 240 + bs);
-            tc_fence_after();
-            const uint32_t b_hi = smem_u32(sb + bs * C::kBStage);
-            const uint64_t dbh = make_desc(b_hi, 16, sbo_b, 2);
-            const uint32_t offa = ((tap / 3) * C::HWID + (tap % 3)) * 128;
-#pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
-              const uint32_t off = ks * 32;    // 16 bf16 along K inside the swizzle atom
-              umma_bf16(d, desc_add(dah, offa + off), desc_add(dbh, off), idesc2, (cc | tap | ks) != 0);
-              umma_bf16(d, desc_add(dal, offa + off), desc_add(dbh, off), idesc1, 1);
-            }
-            umma_commit(&bempty[bs]);
-            if (++bs == C::kBStages) { bs = 0; bph ^= 1; }
-          }
-          umma_commit(&hempty[hs]);
-          if (++hs == C::kHaloStages) { hs = 0; hph ^= 1; }
-        }
-        umma_commit(&tfull[as]);
-        if (++as == 2) { as = 0; aph ^= 1; }
-      }
-    }
-  } else {
-    // two epilogue groups of four warps: group g drains accumulator stage g, i.e. every other item
-    const int q = warp & 3;
-    const int grp = (warp - 2) >> 2;
-    uint32_t aph = 0;
-    int it = 0;
-    const int m = q * 32 + lane;                       // TMEM lane = pixel of the tile: row m/8, column m%8
-    for (int item = blockIdx.x; item < total_items; item += gridDim.x, ++it) {
-      if ((it & 1) != grp) continue;
-      int t = item;
-      const int nb = t % nblk; t /= nblk;
-      const int tw_i = t % tiles_w; t /= tiles_w;
-      const int th_i = t % tiles_h;
-      const int n = t / tiles_h;
-      const int h = th_i * C::TH + (m >> 3), w = tw_i * C::TW + (m & 7);
-      const bool ok = h < H && w < W;
-      const int co0 = nb * BN;
-      mbar_wait(&tfull[grp], aph, 250 + grp);
-      aph ^= 1;
-      tc_fence_after();
-      float* dst = y + ((((int64_t)n * H + h) * W + w) * Cout + co0);
-      const uint32_t t0 = tmem_base + ((uint32_t)(q * 32) << 16) + grp * C::kAccCols;
-      constexpr int CH = 32;                            // columns per TMEM round trip
-#pragma unroll 1
-      for (int c = 0; c < BN; c += CH) {
-        uint32_t r[CH], r2[CH];
-#pragma unroll
-        for (int cc = 0; cc < CH; cc += 16) tmem_ld16_issue(t0 + c + cc, r + cc);
-#pragma unroll
-        for (int cc = 0; cc < CH; cc += 16) tmem_ld16_issue(t0 + BN + c + cc, r2 + cc);
-        tmem_ld_wait();
-        if (c + CH >= BN) {                             // last chunk read: the accumulator stage is free again
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tempty[grp]);
-        }
-        if (ok) {
-#pragma unroll
-          for (int j = 0; j < CH; j += 4) {
-            float v[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              v[e] = __uint_as_float(r[j + e]) + __uint_as_float(r2[j + e]);
-              if (bias) {
-                v[e] += __ldg(bias + co0 + c + j + e);
-                if (act) v[e] = lrelu(v[e]);
-              }
-            }
-            const float4 o = make_float4(v[0], v[1], v[2], v[3]);
-            *reinterpret_cast<float4*>(dst + c + j) = o;
-            if (z_planes) st_planes4(z_planes, (int64_t)N * H * W * Cout, ((dst - y) + c + j) >> 2, o);
-          }
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, C::kTmemCols);
-}
-
-// ----------------------------------------------------------------------------------------------------
-// Wide-layer halo kernel on CTA PAIRS (tcgen05 cta_group::2), Cout % 128 == 0.  k_conv_htap_tc is bound by shared-memory
-// bandwidth: per K-step an SM reads 20 KB of operands (A twice, the N = 256 weight operand, the N = 128 one) in 192
-// tensor cycles = 107 B/clk, plus ~48 B/clk of TMA fill, against 128 B/clk.  A CTA pair issues ONE M = 256 MMA over
-// both SMs' pixel tiles; each SM holds (and re-reads, and re-fills) only HALF of the weight rows:
-//   per SM and K-step: 3 x (A 4 KB + B 2 KB) = 18 KB / 192 cycles = 94 B/clk, fill 46 KB halo + 144 KB weights per
-//   64-channel chunk = 27 B/clk  ->  under the shared-memory limit, the tensor pipe becomes the bound.
-// Three N = 128 MMAs per K-step (x_lo.w_hi, x_hi.w_lo, x_hi.w_hi) accumulate into the SAME 128 TMEM columns -- the same
-// tensor time as the N-concatenated pair of the single-CTA kernels (128 + 64 cycles), but 128 instead of 384 columns
-// per accumulator stage, so two stages fit and the epilogue of one item overlaps the MMAs of the next.
-// Roles per CTA: warp 0 TMA producer (own halo, own half of the weight tile; all bytes complete on the LEADER's
-// barriers), warp 1 lane 0 of the leader issues the pair's MMAs and multicast-commits stage releases / accumulator hand-over
-// to both CTAs, warps 2-9 two epilogue groups (each CTA drains its own 128 TMEM lanes; the release of an accumulator stage
-// is a remote arrive on the leader's barrier).  PTX forms: cute/arch/{copy_sm100_tma,mma_sm100_umma}.hpp; first
-// validated in scripts/dev/tap2sm_probe.cu (profiles/r01_tap2sm_probe.txt).
-// ----------------------------------------------------------------------------------------------------
-constexpr uint32_t kPeerMask = 0xFEFFFFFFu;   // clears the CTA-rank bit of a shared::cluster address (pair leader = even rank)
-
-__device__ __forceinline__ void tma4_pair(const CUtensorMap* tm, uint64_t* leader_bar, void* dst, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-               ::"r"(smem_u32(dst)), "l"(tm), "r"(smem_u32(leader_bar) & kPeerMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma2_pair(const CUtensorMap* tm, uint64_t* leader_bar, void* dst, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-               ::"r"(smem_u32(dst)), "l"(tm), "r"(smem_u32(leader_bar) & kPeerMask), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void umma_bf16_pair(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrives on `bar` (same offset) in BOTH CTAs of the pair once the pair's previously issued MMAs are done
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {     // arrive on the LEADER CTA's copy of `bar`
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerMask) : "memory");
-}
-
-struct HTap2Cfg {
-  static constexpr int BN = 128, HALF = 64;
-  static constexpr int TH = 16, TW = 8, HH = 18, HWID = 10;
-  static constexpr int kPlaneRaw = HH * HWID * 128;
-  static constexpr int kPlane = (kPlaneRaw + 1023) / 1024 * 1024;
-  static constexpr int kHaloStage = 2 * kPlane;
-  static constexpr int kHaloStages = 2;
-  static constexpr int kBHalf = HALF * 128;                   // this CTA's 64 weight rows of one plane
-  static constexpr int kBStage = 2 * kBHalf;
-  static constexpr int kBStages = 6;
-  static constexpr int kBytes = kHaloStages * kHaloStage + kBStages * kBStage + 1024 + 512;
-  static constexpr uint32_t kAccCols = 128;
-  static constexpr uint32_t kTmemCols = 256;
-};
-
-__global__ void __launch_bounds__(320, 1) k_conv_htap2_tc(const __grid_constant__ CUtensorMap tm_a_hi,
-                                                          const __grid_constant__ CUtensorMap tm_a_lo,
-                                                          const __grid_constant__ CUtensorMap tm_b_hi,
-                                                          const __grid_constant__ CUtensorMap tm_b_lo,
-                                                          float* __restrict__ y, int N, int H, int W, int Cin, int Cout,
-                                                          int tiles_w, int tiles_h, const float* __restrict__ bias, int act,
-                                                          void* __restrict__ z_planes) {
-  using C = HTap2Cfg;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sh = smem;
-  uint8_t* sb = smem + C::kHaloStages * C::kHaloStage;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sb + C::kBStages * C::kBStage);
-  uint64_t* hfull = bars;                          // leader's copy is used: both CTAs' halo bytes
-  uint64_t* hempty = hfull + C::kHaloStages;       // per CTA, released by the leader's multicast commit
-  uint64_t* bfull = hempty + C::kHaloStages;       // leader's
-  uint64_t* bempty = bfull + C::kBStages;          // per CTA
-  uint64_t* tfull = bempty + C::kBStages;          // [2] per CTA (multicast commit)
-  uint64_t* tempty = tfull + 2;                    // [2] leader's: 4 epilogue warps of each CTA arrive
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tempty + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int cluster_id = blockIdx.x >> 1, num_clusters = gridDim.x >> 1;
-  const int chunks = Cin / 64, nblk = Cout / C::BN;
-  const int total_tiles = N * tiles_h * tiles_w;
-  const int pairs = (total_tiles + 1) / 2;
-  const int total_items = pairs * nblk;              // Cout block fastest
-
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_a_lo); prefetch_tmap(&tm_b_hi); prefetch_tmap(&tm_b_lo);
-    for (int s = 0; s < C::kHaloStages; ++s) { mbar_init(&hfull[s], 1); mbar_init(&hempty[s], 1); }
-    for (int s = 0; s < C::kBStages; ++s) { mbar_init(&bfull[s], 1); mbar_init(&bempty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tfull[s], 1); mbar_init(&tempty[s], 8); }
-    fence_barrier_init();
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "r"(C::kTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int hs = 0, bs = 0; uint32_t hph = 0, bph = 0;
-      for (int item = cluster_id; item < total_items; item += num_clusters) {
-        const int nb = item % nblk;
-        int t = 2 * (item / nblk) + (int)rank;        // this CTA's tile; past the last one: n >= N, TMA fills zeros
-        const int tw_i = t % tiles_w; t /= tiles_w;
-        const int th_i = t % tiles_h;
-        const int n = t / tiles_h;
-        const int w0 = tw_i * C::TW - 1, h0 = th_i * C::TH - 1;
-        for (int cc = 0; cc < chunks; ++cc) {
-          mbar_wait(&hempty[hs], hph ^ 1, 400 + hs);
-          uint8_t* dst = sh + hs * C::kHaloStage;
-          if (rank == 0) mbar_expect_tx(&hfull[hs], 2 * 2 * C::kPlaneRaw);       // both CTAs' halos
-          tma4_pair(&tm_a_hi, &hfull[hs], dst, cc * 64, w0, h0, n);
-          tma4_pair(&tm_a_lo, &hfull[hs], dst + C::kPlane, cc * 64, w0, h0, n);
-          if (++hs == C::kHaloStages) { hs = 0; hph ^= 1; }
-          for (int tap = 0; tap < 9; ++tap) {
-            mbar_wait(&bempty[bs], bph ^ 1, 410 + bs);
-            uint8_t* db = sb + bs * C::kBStage;
-            if (rank == 0) mbar_expect_tx(&bfull[bs], 2 * C::kBStage);           // both CTAs' halves
-            tma2_pair(&tm_b_hi, &bfull[bs], db, cc * 64, tap * Cout + nb * C::BN + (int)rank * C::HALF);
-            tma2_pair(&tm_b_lo, &bfull[bs], db + C::kBHalf, cc * 64, tap * Cout + nb * C::BN + (int)rank * C::HALF);
-            if (++bs == C::kBStages) { bs = 0; bph ^= 1; }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && rank == 0) {
-      constexpr uint32_t idesc = make_idesc(256, C::BN, 0, 0);
-      constexpr uint32_t sbo_a = C::HWID * 128, sbo_b = 8 * 128;
-      int hs = 0, bs = 0, as = 0; uint32_t hph = 0, bph = 0, aph = 0;
-      for (int item = cluster_id; item < total_items; item += num_clusters) {
-        mbar_wait(&tempty[as], aph ^ 1, 420 + as);
-        tc_fence_after();
-        const uint32_t d = tmem_base + as * C::kAccCols;
-        for (int cc = 0; cc < chunks; ++cc) {
-          mbar_wait(&hfull[hs], hph, 430 + hs);
-          tc_fence_after();
-          const uint32_t a_hi = smem_u32(sh + hs * C::kHaloStage);
-          const uint64_t dah = make_desc(a_hi, 16, sbo_a, 2), dal = make_desc(a_hi + C::kPlane, 16, sbo_a, 2);
-          for (int tap = 0; tap < 9; ++tap) {
-            mbar_wait(&bfull[bs], bph, 440 + bs);
-            tc_fence_after();
-            const uint32_t b_hi = smem_u32(sb + bs * C::kBStage);
-            const uint64_t dbh = make_desc(b_hi, 16, sbo_b, 2), dbl = make_desc(b_hi + C::kBHalf, 16, sbo_b, 2);
-            const uint32_t offa = ((tap / 3) * C::HWID + (tap % 3)) * 128;
-#pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
-              const uint32_t off = ks * 32;
-              umma_bf16_pair(d, desc_add(dal, offa + off), desc_add(dbh, off), idesc, (cc | tap | ks) != 0);
-              umma_bf16_pair(d, desc_add(dah, offa + off), desc_add(dbl, off), idesc, 1);
-              umma_bf16_pair(d, desc_add(dah, offa + off), desc_add(dbh, off), idesc, 1);
-            }
-            umma_commit_pair(&bempty[bs]);
-            if (++bs == C::kBStages) { bs = 0; bph ^= 1; }
-          }
-          umma_commit_pair(&hempty[hs]);
-          if (++hs == C::kHaloStages) { hs = 0; hph ^= 1; }
-        }
-        umma_commit_pair(&tfull[as]);
-        if (++as == 2) { as = 0; aph ^= 1; }
-      }
-    }
-  } else {
-    const int q = warp & 3;
-    const int grp = (warp - 2) >> 2;
-    uint32_t aph = 0;
-    int it = 0;
-    const int m = q * 32 + lane;
-    for (int item = cluster_id; item < total_items; item += num_clusters, ++it) {
-      if ((it & 1) != grp) continue;
-      const int nb = item % nblk;
-      const int tile = 2 * (item / nblk) + (int)rank;
-      int t = tile;
-      const int tw_i = t % tiles_w; t /= tiles_w;
-      const int th_i = t % tiles_h;
-      const int n = t / tiles_h;
-      const int h = th_i * C::TH + (m >> 3), w = tw_i * C::TW + (m & 7);
-      const bool ok = tile < total_tiles && h < H && w < W;
-      const int co0 = nb * C::BN;
-      mbar_wait(&tfull[grp], aph, 450 + grp);
-      aph ^= 1;
-      tc_fence_after();
-      float* dst = y + ((((int64_t)n * H + h) * W + w) * Cout + co0);
-      const uint32_t t0 = tmem_base + ((uint32_t)(q * 32) << 16) + grp * C::kAccCols;
-      constexpr int CH = 64;
-#pragma unroll 1
-      for (int c = 0; c < C::BN; c += CH) {
-        uint32_t r[CH];
-#pragma unroll
-        for (int cc = 0; cc < CH; cc += 16) tmem_ld16_issue(t0 + c + cc, r + cc);
-        tmem_ld_wait();
-        if (c + CH >= C::BN) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_leader(&tempty[grp]);
-        }
-        if (ok) {
-#pragma unroll
-          for (int j = 0; j < CH; j += 4) {
-            float v[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              v[e] = __uint_as_float(r[j + e]);
-              if (bias) {
-                v[e] += __ldg(bias + co0 + c + j + e);
-                if (act) v[e] = lrelu(v[e]);
-              }
-            }
-            const float4 o = make_float4(v[0], v[1], v[2], v[3]);
-            *reinterpret_cast<float4*>(dst + c + j) = o;
-            if (z_planes) st_planes4(z_planes, (int64_t)N * H * W * Cout, ((dst - y) + c + j) >> 2, o);
-          }
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();          // the peer's shared memory / TMEM / barriers are in use until the pair is done
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(C::kTmemCols) : "memory");
 }
 
 // ----------------------------------------------------------------------------------------------------
@@ -1826,187 +645,12 @@ static int make_w_map(CUtensorMap* tm, const void* base, int rows, int K, int cc
   return TWG_OK;
 }
 
-// NHWC bf16 plane seen 8 channels at a time: dims {C, W, H, N}, box {8, halo width, 18, 1}, no swizzle
-static int make_halo_map(CUtensorMap* tm, const void* base, int N, int H, int W, int C, int hwid) {
-  PFN_tmapEncodeTiled enc = get_encode();
-  if (!enc) return fail(TWG_ERR_CUDA, "cuTensorMapEncodeTiled unavailable");
-  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-  cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  cuuint32_t box[4] = {8, (cuuint32_t)hwid, 18, 1};
-  cuuint32_t es[4] = {1, 1, 1, 1};
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(TWG_ERR_CUDA, "cuTensorMapEncodeTiled(halo) failed: %d", (int)r);
-  return TWG_OK;
-}
-
-static bool g_use_halo = true;   // A/B switch (twg_set_option key 1)
-
-static bool halo_shape_ok(int H, int W, int K, int Nc, int k, int pad) {
+// Shapes whose forward epilogue also offers the instance-norm statistics, the activation sign mask and the evaluation-mode
+// affine: the small-channel high-resolution layers (one output-channel block, 16 x 8 pixel tiles inside one image).
+// They never split K, so every epilogue variant computes bit-identical outputs.
+static bool epi_shape_ok(int H, int W, int K, int Nc, int k, int pad) {
   auto small = [](int c) { return c == 16 || c == 32 || c == 64; };
   return k == 3 && pad == 1 && small(K) && small(Nc) && K * Nc <= 2048 && H >= 16 && W >= 16;
-}
-
-static int g_halo_sub = 0;       // 0 = per-shape default; 1/2/4 forces the sub-tile count (twg_set_option key 2)
-
-template <int CIN, int BN, int SUB, int EPI>
-static int launch_halo_epi(const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo, const __nv_bfloat16* w_planes, float* y,
-                           int N, int H, int W, const float* bias, int act, void* z_planes, cudaStream_t st,
-                           float4* stats, uint8_t* act_mask, const float* aff_a) {
-  using C = HaloCfg<CIN, BN, SUB>;
-  auto kern = k_conv_halo_tc<CIN, BN, SUB, EPI>;
-  static std::once_flag once;                 // one-time attribute set-up, safe from several host threads
-  static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [&] { attr_err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kBytes); });
-  if (attr_err != cudaSuccess) return fail(TWG_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(attr_err));
-  CUtensorMap th, tl;
-  int rc;
-  if ((rc = make_halo_map(&th, a_hi, N, H, W, CIN, C::HWID))) return rc;
-  if ((rc = make_halo_map(&tl, a_lo, N, H, W, CIN, C::HWID))) return rc;
-  const int tiles_w = (int)cdiv(W, C::TW), tiles_h = (int)cdiv(H, C::TH);
-  const int64_t total = (int64_t)N * tiles_w * tiles_h;
-  const unsigned grid = (unsigned)(total < kNumSMs ? total : kNumSMs);
-  kern<<<grid, 320, C::kBytes, st>>>(th, tl, w_planes, y, N, H, W, tiles_w, tiles_h, bias, act, z_planes, stats, act_mask, aff_a);
-  return check_launch("twg_conv halo");
-}
-
-// Sub-tile count per shape.  More sub-tiles amortise the per-tile hand-over (TMA issue, commit, barrier round trip)
-// but coarsen the tile grid (wave quantisation over 148 SMs) and the MMA/epilogue interleave; CIN = 64 has room for
-// one sub-tile only (halo stage size in shared memory).
-template <int CIN, int BN, int SUB>
-static int launch_halo_sub(const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo, const __nv_bfloat16* w_planes, float* y,
-                           int N, int H, int W, const float* bias, int act, void* z_planes, cudaStream_t st,
-                           float4* stats, uint8_t* act_mask, const float* aff_a) {
-  if (aff_a) return launch_halo_epi<CIN, BN, SUB, 2>(a_hi, a_lo, w_planes, y, N, H, W, bias, act, z_planes, st, stats, act_mask, aff_a);
-  if (stats) return launch_halo_epi<CIN, BN, SUB, 1>(a_hi, a_lo, w_planes, y, N, H, W, bias, act, z_planes, st, stats, act_mask, aff_a);
-  return launch_halo_epi<CIN, BN, SUB, 0>(a_hi, a_lo, w_planes, y, N, H, W, bias, act, z_planes, st, stats, act_mask, aff_a);
-}
-
-// sub-tile count of the halo kernel for a shape (A/B: profiles/r01_halo_subtiles.txt)
-static int halo_pick_sub(int CIN, int BN, int W, bool planes_out) {
-  if (CIN >= 64) return 1;
-  int sub = g_halo_sub;
-  if (sub == 0) {
-    sub = (W < 64) ? 1 : ((CIN == 16 && BN <= 32) ? 4 : 2);
-    if (planes_out) sub = (BN > CIN) ? 1 : (sub > 2 ? 2 : sub);   // the heavier plane-emitting epilogue prefers finer tiles
-  }
-  if (sub >= 4) return (BN <= 32 && CIN == 16) ? 4 : 2;
-  return sub >= 2 ? 2 : 1;
-}
-
-template <int CIN, int BN>
-static int launch_halo(const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo, const __nv_bfloat16* w_planes, float* y,
-                       int N, int H, int W, const float* bias, int act, void* z_planes, cudaStream_t st,
-                       float4* stats = nullptr, uint8_t* act_mask = nullptr, const float* aff_a = nullptr) {
-  const int sub = halo_pick_sub(CIN, BN, W, z_planes != nullptr);
-  if constexpr (CIN < 64) {
-    if constexpr (BN <= 32 && CIN == 16) {
-      if (sub == 4) return launch_halo_sub<CIN, BN, 4>(a_hi, a_lo, w_planes, y, N, H, W, bias, act, z_planes, st, stats, act_mask, aff_a);
-    }
-    if (sub >= 2) return launch_halo_sub<CIN, BN, 2>(a_hi, a_lo, w_planes, y, N, H, W, bias, act, z_planes, st, stats, act_mask, aff_a);
-  }
-  return launch_halo_sub<CIN, BN, 1>(a_hi, a_lo, w_planes, y, N, H, W, bias, act, z_planes, st, stats, act_mask, aff_a);
-}
-
-// NHWC bf16 plane, 64 channels at a time, 18 x 10 halo of a 16 x 8 tile: dims {C, W, H, N}, box {64, 10, 18, 1}, 128B swizzle
-static int make_htap_map(CUtensorMap* tm, const void* base, int N, int H, int W, int C) {
-  PFN_tmapEncodeTiled enc = get_encode();
-  if (!enc) return fail(TWG_ERR_CUDA, "cuTensorMapEncodeTiled unavailable");
-  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-  cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  cuuint32_t box[4] = {64, 10, 18, 1};
-  cuuint32_t es[4] = {1, 1, 1, 1};
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(TWG_ERR_CUDA, "cuTensorMapEncodeTiled(wide halo) failed: %d", (int)r);
-  return TWG_OK;
-}
-
-static int g_use_htap = 1;       // twg_set_option key 6: wide-layer halo kernel (0 = tap-per-TMA kernel everywhere)
-
-static bool htap_shape_ok(int N, int H, int W, int K, int Nc, int k, int pad) {
-  if (!(k == 3 && pad == 1 && K % 64 == 0 && (Nc == 64 || Nc % 128 == 0) && H >= 16 && W >= 16)) return false;
-  // persistent kernel: wants enough (tile, Cout block) items to keep the SMs busy; small launches stay on the
-  // tap-per-TMA kernel, which splits K to fill the machine
-  const int BN = Nc >= 128 ? 128 : 64;
-  const int64_t items = (int64_t)N * cdiv(H, 16) * cdiv(W, 8) * (Nc / BN);
-  return items >= 96;
-}
-
-template <int BN>
-static int launch_htap(const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo, const __nv_bfloat16* w_hi,
-                       const __nv_bfloat16* w_lo, float* y, int N, int H, int W, int K, int Nc, const float* bias, int act,
-                       void* z_planes, cudaStream_t st) {
-  using C = HTapCfg<BN>;
-  auto kern = k_conv_htap_tc<BN>;
-  static std::once_flag once;
-  static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [&] { attr_err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kBytes); });
-  if (attr_err != cudaSuccess) return fail(TWG_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(attr_err));
-  CUtensorMap ah, al, bh, bl;
-  int rc;
-  if ((rc = make_htap_map(&ah, a_hi, N, H, W, K))) return rc;
-  if ((rc = make_htap_map(&al, a_lo, N, H, W, K))) return rc;
-  if ((rc = make_w_map(&bh, w_hi, 9 * Nc, K, 64, BN))) return rc;
-  if ((rc = make_w_map(&bl, w_lo, 9 * Nc, K, 64, BN))) return rc;
-  const int tiles_w = (int)cdiv(W, C::TW), tiles_h = (int)cdiv(H, C::TH);
-  const int64_t items = (int64_t)N * tiles_w * tiles_h * (Nc / BN);
-  const unsigned grid = (unsigned)(items < kNumSMs ? items : kNumSMs);
-  kern<<<grid, 320, C::kBytes, st>>>(ah, al, bh, bl, y, N, H, W, K, Nc, tiles_w, tiles_h, bias, act, z_planes);
-  return check_launch("twg_conv wide halo");
-}
-
-// twg_set_option key 8: CTA-pair variant of the wide-layer halo kernel (Cout % 128 == 0).  Correct on the first hardware
-// run, but SLOWER than the single-CTA halo kernel at every bench shape (profiles/r02_conv_ab_cta_pair.txt: 32x32 128->128
-// x64: 57.9 vs 47.6 us; 16x16 512->256: 98.9 vs 78.3 us) -- the same ~335 TFLOP/s the round-1 probe reached; off by default.
-static int g_use_htap2 = 0;
-
-static int launch_htap2(const __nv_bfloat16* a_hi, const __nv_bfloat16* a_lo, const __nv_bfloat16* w_hi,
-                        const __nv_bfloat16* w_lo, float* y, int N, int H, int W, int K, int Nc, const float* bias, int act,
-                        void* z_planes, cudaStream_t st) {
-  using C = HTap2Cfg;
-  auto kern = k_conv_htap2_tc;
-  static std::once_flag once;
-  static cudaError_t attr_err = cudaSuccess;
-  static int max_clusters = 0;
-  std::call_once(once, [&] {
-    attr_err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kBytes);
-    if (attr_err != cudaSuccess) return;
-    cudaLaunchConfig_t q = {};
-    q.gridDim = dim3(kNumSMs); q.blockDim = dim3(320); q.dynamicSmemBytes = C::kBytes;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    q.attrs = at; q.numAttrs = 1;
-    int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, kern, &q) == cudaSuccess && n > 0) max_clusters = n;
-    else { max_clusters = kNumSMs / 2; (void)cudaGetLastError(); }
-  });
-  if (attr_err != cudaSuccess) return fail(TWG_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(attr_err));
-  CUtensorMap ah, al, bh, bl;
-  int rc;
-  if ((rc = make_htap_map(&ah, a_hi, N, H, W, K))) return rc;
-  if ((rc = make_htap_map(&al, a_lo, N, H, W, K))) return rc;
-  if ((rc = make_w_map(&bh, w_hi, 9 * Nc, K, 64, C::HALF))) return rc;
-  if ((rc = make_w_map(&bl, w_lo, 9 * Nc, K, 64, C::HALF))) return rc;
-  const int tiles_w = (int)cdiv(W, C::TW), tiles_h = (int)cdiv(H, C::TH);
-  const int64_t pairs = ((int64_t)N * tiles_w * tiles_h + 1) / 2;
-  const int64_t items = pairs * (Nc / C::BN);
-  int64_t clusters = items < max_clusters ? items : max_clusters;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(2 * clusters));
-  cfg.blockDim = dim3(320);
-  cfg.dynamicSmemBytes = C::kBytes;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr; cfg.numAttrs = 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ah, al, bh, bl, y, N, H, W, K, Nc, tiles_w, tiles_h, bias, act, z_planes);
-  if (e != cudaSuccess) return fail(TWG_ERR_CUDA, "wide halo pair launch: %s", cudaGetErrorString(e));
-  return check_launch("twg_conv wide halo pair");
 }
 
 static int pow2_le(int v) {
@@ -2050,63 +694,20 @@ int64_t conv_tc_workspace(int N, int H, int W, int Cin, int Cout, int k, int pad
   return 2 * align_up(px * cmax * 4, 1024) + align_up((int64_t)k * k * Cin * Cout * 4, 1024) + 4096;
 }
 
-static int g_fwd_ts = 0;   // experiment switch (twg_set_option key 3): A operand of the wide kernel staged in TMEM
-
-static int g_fwd_cluster = 0;   // twg_set_option key 4: 2-CTA clusters with TMA-multicast weight tiles in the wide tap kernel
-
-template <int CC, int BN, bool TS, int CL = 1>
-static int launch_fwd_tc_m(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
-                         float* y, const TcGeom& g, const float* bias, int act, void* z_planes, cudaStream_t st) {
+template <int CC, int BN>
+static int launch_fwd(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl, float* y,
+                      const TcGeom& g, const float* bias, int act, void* z_planes, float4* stats, uint8_t* act_mask,
+                      const float* aff_a, cudaStream_t st) {
   using SM = FwdSmem<CC, BN>;
-  auto kern = k_conv_fwd_tc<CC, BN, TS, CL>;
+  auto kern = k_conv_fwd_wgmma<CC, BN>;
   static std::once_flag once;                 // one-time attribute set-up, safe from several host threads
   static cudaError_t attr_err = cudaSuccess;
   std::call_once(once, [&] { attr_err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::kBytes); });
   if (attr_err != cudaSuccess) return fail(TWG_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(attr_err));
   const int tiles = g.tiles_w * g.tiles_h * g.tiles_n, nblk = g.Cout / BN;
-  const int num_kb = g.k * g.k * (g.Cin / CC);
-  int splits = 1;
-  if (!bias && tiles * nblk * 2 <= kNumSMs) {          // under-filled grid: split the K loop (>= 4 k-blocks per split)
-    splits = (2 * kNumSMs) / (tiles * nblk);
-    if (splits > num_kb / 4) splits = num_kb / 4;
-    if (splits < 1) splits = 1;
-  }
-  const int kbps = (num_kb + splits - 1) / splits;
-  splits = (num_kb + kbps - 1) / kbps;
-  if (splits > 1) {
-    const int64_t px = (int64_t)g.N * g.H * g.W;
-    cudaMemsetAsync(y, 0, sizeof(float) * px * g.Cout, st);
-  }
-  if (z_planes && splits != 1) return fail(TWG_ERR_INVALID, "fused plane output is incompatible with split-K");
-  if constexpr (CL == 1) {
-    dim3 grid((unsigned)tiles, (unsigned)nblk, (unsigned)splits);
-    kern<<<grid, 192, SM::kBytes, st>>>(ah, al, bh, bl, y, g, bias, act, kbps, z_planes);
-  } else {
-    // pixel tiles in pairs; a padding CTA past the last tile loads zero-filled boxes and stores nothing
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)((tiles + CL - 1) / CL * CL), (unsigned)nblk, (unsigned)splits);
-    cfg.blockDim = dim3(192);
-    cfg.dynamicSmemBytes = SM::kBytes;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CL; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    void* zp = z_planes;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, kern, ah, al, bh, bl, y, g, bias, act, kbps, zp);
-    if (e != cudaSuccess) return fail(TWG_ERR_CUDA, "cluster launch: %s", cudaGetErrorString(e));
-  }
+  dim3 grid((unsigned)tiles, (unsigned)nblk);
+  kern<<<grid, kThreads, SM::kBytes, st>>>(ah, al, bh, bl, y, g, bias, act, z_planes, stats, act_mask, aff_a);
   return check_launch("twg_conv tc");
-}
-
-template <int CC, int BN>
-static int launch_fwd_tc(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
-                         float* y, const TcGeom& g, const float* bias, int act, void* z_planes, cudaStream_t st, int cl) {
-  if constexpr (CC == 64 && (BN == 64 || BN == 128)) {
-    if (cl == 2) return launch_fwd_tc_m<CC, BN, false, 2>(ah, al, bh, bl, y, g, bias, act, z_planes, st);
-  }
-  if (CC == 64 && BN == 128 && g_fwd_ts) return launch_fwd_tc_m<64, 128, true>(ah, al, bh, bl, y, g, bias, act, z_planes, st);
-  return launch_fwd_tc_m<CC, BN, false>(ah, al, bh, bl, y, g, bias, act, z_planes, st);
 }
 
 static unsigned split_blocks(int64_t n4) {
@@ -2138,17 +739,16 @@ bool conv_tc_supported(int N, int H, int W, int Cin, int Cout, int k, int pad) {
   return pick_tile(g);
 }
 
-// Records per image the forward halo kernel writes when asked for epilogue statistics (0: this shape runs on a kernel
-// that has none): one {count, pivot, S1, S2} per (tile, epilogue warp, channel).
+// Records per image the forward kernel writes when asked for epilogue statistics (0: not offered for this shape): one
+// {count, pivot, S1, S2} per (16 x 8 tile, consumer warp, channel).
 int conv_fwd_stats_slots(int N, int H, int W, int Cin, int Cout, int k, int pad) {
-  if (!tc_shape_ok(N, H, W, Cin, Cout, k, pad) || !g_use_halo || !halo_shape_ok(H, W, Cin, Cout, k, pad)) return 0;
-  const int tw = 8 * halo_pick_sub(Cin, Cout, W, false);
-  return (int)(cdiv(H, 16) * cdiv(W, tw) * 4);
+  if (!tc_shape_ok(N, H, W, Cin, Cout, k, pad) || !epi_shape_ok(H, W, Cin, Cout, k, pad)) return 0;
+  return (int)(cdiv(H, 8) * cdiv(W, 16) * kConsumerWarps);
 }
 
-// whether the fused bias + leaky-ReLU epilogue of this forward shape can also write the activation's sign mask (halo kernel)
+// whether the fused bias + leaky-ReLU epilogue of this forward shape can also write the activation's sign mask
 bool conv_fwd_has_act_mask(int N, int H, int W, int Cin, int Cout, int k, int pad) {
-  return tc_shape_ok(N, H, W, Cin, Cout, k, pad) && g_use_halo && halo_shape_ok(H, W, Cin, Cout, k, pad);
+  return tc_shape_ok(N, H, W, Cin, Cout, k, pad) && epi_shape_ok(H, W, Cin, Cout, k, pad);
 }
 
 // core: activation planes [2][N,H,W,Kc] (Kc = Cin for forward, Cout for dgrad), weight planes from split_weight_planes
@@ -2175,30 +775,19 @@ int conv_fwd_tc_planes(const void* a_planes, const void* w_planes, float* y, int
   const __nv_bfloat16* a_lo = a_hi + px * g.Cin;
   const __nv_bfloat16* w_hi = reinterpret_cast<const __nv_bfloat16*>(w_planes);
   const __nv_bfloat16* w_lo = w_hi + (int64_t)taps * Cin * Cout;
-  if (g_use_halo && halo_shape_ok(H, W, g.Cin, g.Cout, k, pad)) {
-#define TWG_HALO_CASE(ci, bn) \
-    if (g.Cin == ci && g.Cout == bn) return launch_halo<ci, bn>(a_hi, a_lo, w_hi, y, N, H, W, bias, act, z_planes, st, stats, act_mask, aff_a);
-    TWG_HALO_CASE(16, 16) TWG_HALO_CASE(16, 32) TWG_HALO_CASE(16, 64) TWG_HALO_CASE(32, 16) TWG_HALO_CASE(32, 32)
-    TWG_HALO_CASE(32, 64) TWG_HALO_CASE(64, 16) TWG_HALO_CASE(64, 32)
-#undef TWG_HALO_CASE
-  }
-  if (g_use_htap && htap_shape_ok(N, H, W, g.Cin, g.Cout, k, pad)) {
-    if (g.Cout >= 128 && g_use_htap2) return launch_htap2(a_hi, a_lo, w_hi, w_lo, y, N, H, W, g.Cin, g.Cout, bias, act, z_planes, st);
-    if (g.Cout >= 128) return launch_htap<128>(a_hi, a_lo, w_hi, w_lo, y, N, H, W, g.Cin, g.Cout, bias, act, z_planes, st);
-    return launch_htap<64>(a_hi, a_lo, w_hi, w_lo, y, N, H, W, g.Cin, g.Cout, bias, act, z_planes, st);
-  }
   const int CC = chunk_for(g.Cin);
+  // No split-K: its fp32 atomics would add the partial tiles in a different order on every run.  The tile shape depends on
+  // the layer only, never on the batch, so a sample's output is the same whichever batch it is computed in.
   const int BN = g.Cout >= 128 ? 128 : g.Cout;
   CUtensorMap ah, al, bh, bl;
   int rc;
-  // 2-CTA cluster variant: each CTA of a pair fetches half of the weight tile (box = BN/2 rows) and multicasts it
-  const int cl = (g_fwd_cluster && CC == 64 && BN >= 64 && !g_fwd_ts) ? 2 : 1;
   if ((rc = make_act_map(&ah, a_hi, N, H, W, g.Cin, CC, g.TW, g.TH, g.TN))) return rc;
   if ((rc = make_act_map(&al, a_lo, N, H, W, g.Cin, CC, g.TW, g.TH, g.TN))) return rc;
-  if ((rc = make_w_map(&bh, w_hi, taps * g.Cout, g.Cin, CC, BN / cl))) return rc;
-  if ((rc = make_w_map(&bl, w_lo, taps * g.Cout, g.Cin, CC, BN / cl))) return rc;
+  if ((rc = make_w_map(&bh, w_hi, taps * g.Cout, g.Cin, CC, BN))) return rc;
+  if ((rc = make_w_map(&bl, w_lo, taps * g.Cout, g.Cin, CC, BN))) return rc;
 #define TWG_FWD_CASE(cc, bn) \
-  if (CC == cc && BN == bn) return launch_fwd_tc<cc, bn>(ah, al, bh, bl, y, g, bias, act, z_planes, st, cl);
+  if (CC == cc && BN == bn)  \
+    return launch_fwd<cc, bn>(ah, al, bh, bl, y, g, bias, act, z_planes, stats, act_mask, aff_a, st);
   TWG_FWD_CASE(16, 16) TWG_FWD_CASE(16, 32) TWG_FWD_CASE(16, 64) TWG_FWD_CASE(16, 128)
   TWG_FWD_CASE(32, 16) TWG_FWD_CASE(32, 32) TWG_FWD_CASE(32, 64) TWG_FWD_CASE(32, 128)
   TWG_FWD_CASE(64, 16) TWG_FWD_CASE(64, 32) TWG_FWD_CASE(64, 64) TWG_FWD_CASE(64, 128)
@@ -2222,139 +811,34 @@ int conv_fwd_tc(const float* x, const float* w, float* y, int N, int H, int W, i
   return conv_fwd_tc_planes(base, wbase, y, N, H, W, Cin, Cout, k, pad, dgrad, st);
 }
 
-// The weight gradient always forms all three split-bf16 partial products.  Dropping x_lo.gy (one MMA per K-step fewer on
-// the N-concatenated kernels, and no x_lo fill) was built and measured in round 2: although gw sums over 10^4..10^6 pixels,
-// the real gradients of this step have too little signal above the rounding residue for the statistical argument to hold
-// -- weight-gradient parity fell to 2e-3 .. 3e-3 at 128x128 (profiles/r02_wgrad_products.txt), so it is not offered.
-static int g_use_wgrad_row = 1;      // twg_set_option key 7
-
-// NHWC bf16 plane: dims {C, W, H, N}, box {cc, bw, bh, 1}, swizzle by cc (the kh row box of the row-box wgrad kernel)
-static int make_box_map(CUtensorMap* tm, const void* base, int N, int H, int W, int C, int cc, int bw, int bh) {
-  PFN_tmapEncodeTiled enc = get_encode();
-  if (!enc) return fail(TWG_ERR_CUDA, "cuTensorMapEncodeTiled unavailable");
-  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-  cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  cuuint32_t box[4] = {(cuuint32_t)cc, (cuuint32_t)bw, (cuuint32_t)bh, 1};
-  cuuint32_t es[4] = {1, 1, 1, 1};
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, swz_for(cc), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(TWG_ERR_CUDA, "cuTensorMapEncodeTiled(box) failed: %d", (int)r);
-  return TWG_OK;
-}
-
 template <int CN, int BNW>
-static int launch_wgrad_halo(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, const __nv_bfloat16* g_hi,
-                             const __nv_bfloat16* g_lo, float* gw, int N, int H, int W, int Cin, int Cout, cudaStream_t st) {
-  using C = WgHaloCfg<CN, BNW>;
-  auto kern = k_conv_wgrad_halo<CN, BNW>;
-  static std::once_flag once;
-  static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [&] { attr_err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kBytes); });
-  if (attr_err != cudaSuccess) return fail(TWG_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(attr_err));
-  CUtensorMap gh, gl, xh, xl;
-  int rc;
-  if ((rc = make_act_map(&gh, g_hi, N, H, W, Cout, BNW, C::TW, C::TH, 1))) return rc;
-  if ((rc = make_act_map(&gl, g_lo, N, H, W, Cout, BNW, C::TW, C::TH, 1))) return rc;
-  if ((rc = make_box_map(&xh, x_hi, N, H, W, Cin, CN, C::BW, C::BH))) return rc;
-  if ((rc = make_box_map(&xl, x_lo, N, H, W, Cin, CN, C::BW, C::BH))) return rc;
-  const int tiles_w = (int)cdiv(W, C::TW), tiles_h = (int)cdiv(H, C::TH);
-  const int total_tiles = N * tiles_w * tiles_h;
-  const int yb = Cout / BNW, zb = Cin / CN;
-  int64_t want = kNumSMs / ((int64_t)yb * zb);          // one wave (one CTA per SM)
-  if (want < 1) want = 1;
-  int ctas_a, tpc_a, tpc_b = 0, xb;
-  if (C::kSplitSets && want >= 2) {
-    // tap groups {0,1,2} and {3,4} go to different CTAs: 3 : 2 of the MMA work, so 3 : 2 of the CTAs
-    int64_t na = (want * 3 + 2) / 5, nb = want - na;
-    if (nb < 1) { nb = 1; na = want - 1; }
-    if (na > total_tiles) na = total_tiles;
-    if (nb > total_tiles) nb = total_tiles;
-    tpc_a = (int)cdiv(total_tiles, na);
-    tpc_b = (int)cdiv(total_tiles, nb);
-    ctas_a = (int)cdiv(total_tiles, tpc_a);
-    xb = ctas_a + (int)cdiv(total_tiles, tpc_b);
-  } else {
-    if (C::kSplitSets) return fail(TWG_ERR_UNSUPPORTED, "halo wgrad: too many channel blocks for the two-set split");
-    if (want > total_tiles) want = total_tiles;
-    tpc_a = (int)cdiv(total_tiles, want);
-    ctas_a = xb = (int)cdiv(total_tiles, tpc_a);
-  }
-  dim3 grid((unsigned)xb, (unsigned)yb, (unsigned)zb);
-  kern<<<grid, 192, C::kBytes, st>>>(gh, gl, xh, xl, gw, N, H, W, Cin, Cout, tiles_w, tiles_h, tpc_a, ctas_a, tpc_b);
-  return check_launch("twg_conv_wgrad halo");
-}
-
-static int g_use_wgrad_rows = 1;     // twg_set_option key 9
-
-// gy planes as ONE 5-D tensor {C, W, plane, H, N}: the box {cc, 16, 2, rows, 1} lands in shared memory as
-// [row][plane][pixel][channel], i.e. the hi and lo planes interleaved by row (k_conv_wgrad_rows)
-static int make_rows_map(CUtensorMap* tm, const void* hi, int64_t plane_stride_bytes, int N, int H, int W, int C, int cc,
-                         int bw, int bh) {
-  PFN_tmapEncodeTiled enc = get_encode();
-  if (!enc) return fail(TWG_ERR_CUDA, "cuTensorMapEncodeTiled unavailable");
-  if (plane_stride_bytes <= 0 || plane_stride_bytes % 16) return TWG_ERR_UNSUPPORTED;
-  cuuint64_t dims[5] = {(cuuint64_t)C, (cuuint64_t)W, 2, (cuuint64_t)H, (cuuint64_t)N};
-  cuuint64_t strides[4] = {(cuuint64_t)C * 2, (cuuint64_t)plane_stride_bytes, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  cuuint32_t box[5] = {(cuuint32_t)cc, (cuuint32_t)bw, 2, (cuuint32_t)bh, 1};
-  cuuint32_t es[5] = {1, 1, 1, 1, 1};
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(hi), dims, strides, box, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, swz_for(cc), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return TWG_ERR_UNSUPPORTED;   // the caller falls back to the halo kernel
-  return TWG_OK;
-}
-
-template <int CN, int BNW>
-static int launch_wgrad_rows(const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo, const __nv_bfloat16* g_hi,
-                             const __nv_bfloat16* g_lo, float* gw, int N, int H, int W, int Cin, int Cout, cudaStream_t st) {
-  using C = WgRowsCfg<CN, BNW>;
-  auto kern = k_conv_wgrad_rows<CN, BNW>;
-  static std::once_flag once;
-  static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [&] { attr_err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kBytes); });
-  if (attr_err != cudaSuccess) return fail(TWG_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(attr_err));
-  CUtensorMap gm, xh, xl;
-  int rc;
-  if ((rc = make_rows_map(&gm, g_hi, (int64_t)((const uint8_t*)g_lo - (const uint8_t*)g_hi), N, H, W, Cout, BNW, C::TW, C::GH)))
-    return rc;
-  if ((rc = make_box_map(&xh, x_hi, N, H, W, Cin, CN, C::BW, C::TH))) return rc;
-  if ((rc = make_box_map(&xl, x_lo, N, H, W, Cin, CN, C::BW, C::TH))) return rc;
-  const int tiles_w = (int)cdiv(W, C::TW), tiles_h = (int)cdiv(H, C::TH);
-  const int total_tiles = N * tiles_w * tiles_h;
-  const int yb = Cout / BNW, zb = Cin / CN;
-  int64_t want = kNumSMs / ((int64_t)yb * zb);          // one wave (one CTA per SM)
-  if (want < 1) want = 1;
-  if (want > total_tiles) want = total_tiles;
-  const int tpc = (int)cdiv(total_tiles, want);
-  dim3 grid((unsigned)cdiv(total_tiles, tpc), (unsigned)yb, (unsigned)zb);
-  kern<<<grid, 192, C::kBytes, st>>>(gm, xh, xl, gw, N, H, W, Cin, Cout, tiles_w, tiles_h, tpc);
-  return check_launch("twg_conv_wgrad rows");
-}
-
-template <int CN, int BNW>
-static int launch_wgrad_tc2(const CUtensorMap& gh, const CUtensorMap& gl, const CUtensorMap& xh, const CUtensorMap& xl,
-                            float* gw, const TcGeom& g, cudaStream_t st) {
-  using C = Wg2Cfg<CN, BNW>;
-  auto kern = k_conv_wgrad_tc2<CN, BNW>;
+static int launch_wgrad(const CUtensorMap& gh, const CUtensorMap& gl, const CUtensorMap& xh, const CUtensorMap& xl,
+                        float* gw, const TcGeom& g, cudaStream_t st) {
+  using C = WgCfg<CN, BNW>;
+  auto kern = k_conv_wgrad_wgmma<CN, BNW>;
   static std::once_flag once;                 // one-time attribute set-up, safe from several host threads
   static cudaError_t attr_err = cudaSuccess;
   std::call_once(once, [&] { attr_err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kBytes); });
   if (attr_err != cudaSuccess) return fail(TWG_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(attr_err));
   const int total_tiles = g.tiles_w * g.tiles_h * g.tiles_n;
   const int yb = g.Cout / BNW, zb = g.Cin / CN;
-  // one CTA per SM (64 KB stages): the grid must FIT in one wave -- rounding the pixel split up (152 or 160 CTAs on 148
-  // SMs) made the 256-channel layers run two waves, i.e. take twice as long (profiles/r02_conv_ab*.txt)
+  // one CTA per SM (~200 KB of stages): the grid must fit in one wave, or the channel-block-heavy layers run two
   int64_t want = kNumSMs / ((int64_t)yb * zb);
   if (want > total_tiles) want = total_tiles;
   if (want < 1) want = 1;
   const int tiles_per_cta = (int)cdiv(total_tiles, want);
   const int xb = (int)cdiv(total_tiles, tiles_per_cta);
   dim3 grid((unsigned)xb, (unsigned)yb, (unsigned)zb);
-  kern<<<grid, 192, C::kBytes, st>>>(gh, gl, xh, xl, gw, g, tiles_per_cta);
-  return check_launch("twg_conv_wgrad tc2");
+  const int64_t gw_elems = (int64_t)g.k * g.k * g.Cin * g.Cout;
+  float* parts = partials(xb * gw_elems, true, st);
+  if (!parts) return fail(TWG_ERR_UNSUPPORTED, "tensor-core wgrad: weight too large for the split buffer");
+  kern<<<grid, kThreads, C::kBytes, st>>>(gh, gl, xh, xl, parts, g, tiles_per_cta);
+  if (int rc = check_launch("twg_conv_wgrad tc")) return rc;
+  return add_partials(gw, parts, xb, gw_elems, st);
 }
 
+// The weight gradient always forms all three split-bf16 partial products: although gw sums over 10^4..10^6 pixels, the
+// real gradients of this step have too little signal above the rounding residue to drop x_lo.gy.
 int conv_wgrad_tc_planes(const void* x_planes, const void* g_planes, float* gw, int N, int H, int W, int Cin, int Cout,
                          int k, int pad, int accumulate, cudaStream_t st) {
   if (!tc_shape_ok(N, H, W, Cin, Cout, k, pad)) return fail(TWG_ERR_UNSUPPORTED, "tensor-core wgrad: shape not covered");
@@ -2367,29 +851,10 @@ int conv_wgrad_tc_planes(const void* x_planes, const void* g_planes, float* gw, 
   const __nv_bfloat16* g_hi = reinterpret_cast<const __nv_bfloat16*>(g_planes);
   const __nv_bfloat16* g_lo = g_hi + px * Cout;
   if (!accumulate) cudaMemsetAsync(gw, 0, sizeof(float) * k * k * Cin * Cout, st);
-  if (g_use_wgrad_row && k == 3 && pad == 1 && W >= 16 && H >= 8) {
-    const int CNh = chunk_for(Cin), BNh = Cout >= 64 ? 64 : Cout;
-    if (g_use_wgrad_rows) {      // narrow layers: all nine taps in one MMA per partial product (row-shift kernel)
-#define TWG_WGR_CASE(cn, bn) \
-      if (CNh == cn && BNh == bn) { \
-        const int rcr = launch_wgrad_rows<cn, bn>(x_hi, x_lo, g_hi, g_lo, gw, N, H, W, Cin, Cout, st); \
-        if (rcr != TWG_ERR_UNSUPPORTED) return rcr; \
-      }
-      TWG_WGR_CASE(16, 16) TWG_WGR_CASE(16, 32) TWG_WGR_CASE(16, 64) TWG_WGR_CASE(32, 16) TWG_WGR_CASE(32, 32)
-      TWG_WGR_CASE(32, 64) TWG_WGR_CASE(64, 16) TWG_WGR_CASE(64, 32)
-#undef TWG_WGR_CASE
-    }
-#define TWG_WGH_CASE(cn, bn) \
-    if (CNh == cn && BNh == bn) { \
-      const int rch = launch_wgrad_halo<cn, bn>(x_hi, x_lo, g_hi, g_lo, gw, N, H, W, Cin, Cout, st); \
-      if (rch != TWG_ERR_UNSUPPORTED) return rch;      /* else: the tap-stacked kernel below */ \
-    }
-    TWG_WGH_CASE(16, 16) TWG_WGH_CASE(16, 32) TWG_WGH_CASE(16, 64) TWG_WGH_CASE(32, 16) TWG_WGH_CASE(32, 32) TWG_WGH_CASE(32, 64)
-    TWG_WGH_CASE(64, 16) TWG_WGH_CASE(64, 32) TWG_WGH_CASE(64, 64)
-#undef TWG_WGH_CASE
-  }
   const int CN = chunk_for(Cin);                      // channels per tap in the stacked A operand
-  const int BNW = Cout >= 64 ? 64 : Cout;             // output-channel block (N of the MMA)
+  // output-channel block (N of the MMA): 64 channels, 32 for 64-channel chunks, whose five tap groups of accumulators
+  // would not fit in registers at 64
+  const int BNW = (Cout >= 64 && CN < 64) ? 64 : (Cout >= 32 ? 32 : Cout);
   CUtensorMap gh, gl, xh, xl;
   int rc;
   if ((rc = make_act_map(&gh, g_hi, N, H, W, Cout, BNW, g.TW, g.TH, g.TN))) return rc;
@@ -2397,10 +862,10 @@ int conv_wgrad_tc_planes(const void* x_planes, const void* g_planes, float* gw, 
   if ((rc = make_act_map(&xh, x_hi, N, H, W, Cin, CN, g.TW, g.TH, g.TN))) return rc;
   if ((rc = make_act_map(&xl, x_lo, N, H, W, Cin, CN, g.TW, g.TH, g.TN))) return rc;
 #define TWG_WG_CASE(cn, bn) \
-  if (CN == cn && BNW == bn) return launch_wgrad_tc2<cn, bn>(gh, gl, xh, xl, gw, g, st);
+  if (CN == cn && BNW == bn) return launch_wgrad<cn, bn>(gh, gl, xh, xl, gw, g, st);
   TWG_WG_CASE(16, 16) TWG_WG_CASE(16, 32) TWG_WG_CASE(16, 64)
   TWG_WG_CASE(32, 16) TWG_WG_CASE(32, 32) TWG_WG_CASE(32, 64)
-  TWG_WG_CASE(64, 16) TWG_WG_CASE(64, 32) TWG_WG_CASE(64, 64)
+  TWG_WG_CASE(64, 16) TWG_WG_CASE(64, 32)
 #undef TWG_WG_CASE
   return fail(TWG_ERR_UNSUPPORTED, "tensor-core wgrad: no kernel for CN=%d BNW=%d", CN, BNW);
 }
@@ -2418,14 +883,5 @@ int conv_wgrad_tc(const float* x, const float* gy, float* gw, int N, int H, int 
   if ((rc = split_act_planes(gy, gbase, px * Cout, st))) return rc;
   return conv_wgrad_tc_planes(base, gbase, gw, N, H, W, Cin, Cout, k, pad, accumulate, st);
 }
-
-void set_use_halo(bool on) { g_use_halo = on; }
-void set_halo_mode(int sub) { g_halo_sub = (sub == 1 || sub == 2 || sub == 4) ? sub : 0; }
-void set_fwd_ts(int v) { g_fwd_ts = v; }
-void set_fwd_cluster(int v) { g_fwd_cluster = v ? 1 : 0; }
-void set_use_htap(int v) { g_use_htap = v ? 1 : 0; }
-void set_use_htap2(int v) { g_use_htap2 = v ? 1 : 0; }
-void set_use_wgrad_row(int v) { g_use_wgrad_row = v ? 1 : 0; }
-void set_use_wgrad_rows(int v) { g_use_wgrad_rows = v ? 1 : 0; }
 
 }  // namespace twg

@@ -32,6 +32,33 @@ int check_launch(const char* what) {
   return TWG_OK;
 }
 
+constexpr int64_t kPartialFloats = 8 << 20;        // 32 MB: the largest user is the tensor-core weight gradient (<= ~5 M)
+__device__ float g_partials[kPartialFloats];
+
+float* partials(int64_t n, bool zero, cudaStream_t st) {
+  if (n > kPartialFloats) return nullptr;
+  void* p = nullptr;
+  if (cudaGetSymbolAddress(&p, g_partials) != cudaSuccess) return nullptr;
+  if (zero) cudaMemsetAsync(p, 0, sizeof(float) * n, st);
+  return static_cast<float*>(p);
+}
+
+__global__ void __launch_bounds__(256) k_add_partials(float* __restrict__ out, const float* __restrict__ parts, int nb,
+                                                      int64_t n) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    float s = 0.f;
+    for (int b = 0; b < nb; ++b) s += parts[(int64_t)b * n + i];
+    out[i] += s;
+  }
+}
+
+int add_partials(float* out, const float* parts, int nb, int64_t n, cudaStream_t st) {
+  int64_t blocks = cdiv(n, 256);
+  if (blocks > 4 * kNumSMs) blocks = 4 * kNumSMs;
+  k_add_partials<<<(unsigned)blocks, 256, 0, st>>>(out, parts, nb, n);
+  return check_launch("add_partials");
+}
+
 // ------------------------------------------------------------------------------------------------
 // Channel-vector geometry: a pixel's C channels are C/4 float4; G lanes cooperate on one pixel,
 // each lane owning V float4 (lane, lane+32, ...).
@@ -154,15 +181,11 @@ __global__ void __launch_bounds__(256) k_moments_scalar(const float* __restrict_
   }
 }
 
+// One block per sample covers all HW pixels, so every per-(n, c) sum has exactly one writer and comes out the same on
+// every run (several blocks per sample would add their partials in a varying order).
 static int pick_chunk(int HW, int N, int pixels_per_pass) {
-  // aim for ~8 blocks per SM, at least 8 passes of the block over its chunk
-  int64_t target_blocks = 8 * kNumSMs;
-  int64_t per_sample = cdiv(target_blocks, N);
-  int64_t chunk = cdiv(HW, per_sample);
-  int64_t min_chunk = (int64_t)pixels_per_pass * 8;
-  if (chunk < min_chunk) chunk = min_chunk;
-  if (chunk > HW) chunk = HW;
-  return (int)chunk;
+  (void)N; (void)pixels_per_pass;
+  return HW;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -321,18 +344,21 @@ __global__ void __launch_bounds__(256) k_norm_bwd_coeffs_inst(float* __restrict_
                                                               float* __restrict__ gbeta0, float* __restrict__ ggamma1,
                                                               float* __restrict__ gbeta1, unsigned dom_mask, int gs, int N,
                                                               int HW, int C) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= N * C) return;
-  const int n = idx / C, c = idx - n * C;
-  const int dom = (dom_mask >> (n / gs)) & 1u;
-  const float t1 = red[idx * 2], t2 = red[idx * 2 + 1];
-  float* gg = dom ? ggamma1 : ggamma0;
-  float* gb = dom ? gbeta1 : gbeta0;
-  if (gg) atomicAdd(&gg[c], t2);
-  if (gb) atomicAdd(&gb[c], t1);
+  // one thread per channel adds the samples in order (deterministic parameter gradients)
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
   const float inv = 1.f / (float)HW;
-  red[idx * 2] = t1 * inv;
-  red[idx * 2 + 1] = t2 * inv;
+  for (int n = 0; n < N; ++n) {
+    const int idx = n * C + c;
+    const int dom = (dom_mask >> (n / gs)) & 1u;
+    const float t1 = red[idx * 2], t2 = red[idx * 2 + 1];
+    float* gg = dom ? ggamma1 : ggamma0;
+    float* gb = dom ? gbeta1 : gbeta0;
+    if (gg) gg[c] += t2;
+    if (gb) gb[c] += t1;
+    red[idx * 2] = t1 * inv;
+    red[idx * 2 + 1] = t2 * inv;
+  }
 }
 
 __global__ void k_norm_eval_affine(const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -826,7 +852,7 @@ __global__ void __launch_bounds__(256) k_lrelu_bwd_colsum_vec(const float* __res
       if (threadIdx.x < s) sm[threadIdx.x] += sm[threadIdx.x + s];
       __syncthreads();
     }
-    if (threadIdx.x < G) atomicAdd(&colsum[(lg + (k / 4) * 32) * 4 + (k & 3)], sm[threadIdx.x]);
+    if (threadIdx.x < G) colsum[(int64_t)blockIdx.x * C + (lg + (k / 4) * 32) * 4 + (k & 3)] = sm[threadIdx.x];
   }
 }
 
@@ -888,11 +914,11 @@ __global__ void __launch_bounds__(256) k_lrelu_bwd_colsum_pool_rows(const float*
       if (threadIdx.x < s_) sm[threadIdx.x] += sm[threadIdx.x + s_];
       __syncthreads();
     }
-    if (threadIdx.x < q) atomicAdd(&colsum[lg * 4 + k], sm[threadIdx.x]);
+    if (threadIdx.x < q) colsum[((int64_t)blockIdx.x << (lq + 2)) + lg * 4 + k] = sm[threadIdx.x];
   }
 }
 
-// out[c] += sum over a chunk of rows; grid.x = row chunks, thread owns (c, row-lane)
+// out[blockIdx.x * C + c] = sum over a chunk of rows (a partial, see add_partials); grid.x = row chunks, thread owns (c, row-lane)
 __global__ void __launch_bounds__(256) k_colsum(const float* __restrict__ g, float* __restrict__ out, int64_t rows,
                                                 int C, int64_t chunk) {
   __shared__ float sm[256];
@@ -913,7 +939,7 @@ __global__ void __launch_bounds__(256) k_colsum(const float* __restrict__ g, flo
       if (threadIdx.x < s) sm[threadIdx.x] += sm[threadIdx.x + s];
       __syncthreads();
     }
-    if (threadIdx.x < Cw && c < C) atomicAdd(&out[c], sm[threadIdx.x]);
+    if (threadIdx.x < Cw && c < C) out[(int64_t)blockIdx.x * C + c] = sm[threadIdx.x];
   }
 }
 
@@ -1353,7 +1379,7 @@ __global__ void __launch_bounds__(256) k_l1(const float* __restrict__ a, const f
     if (grad) grad[i] = d > 0.f ? wn : (d < 0.f ? -wn : 0.f);
   }
   acc = block_sum(acc, sm);
-  if (threadIdx.x == 0) atomicAdd(loss, acc * wn);
+  if (threadIdx.x == 0) loss[blockIdx.x] = acc * wn;     // partial of this block (add_partials)
 }
 
 __global__ void __launch_bounds__(256) k_sum_sq(const float* __restrict__ x, double* __restrict__ out2, int64_t n) {
@@ -1366,7 +1392,7 @@ __global__ void __launch_bounds__(256) k_sum_sq(const float* __restrict__ x, dou
   }
   a1 = block_sum(a1, sm);
   a2 = block_sum(a2, sm);
-  if (threadIdx.x == 0) { atomicAdd(&out2[0], (double)a1); atomicAdd(&out2[1], (double)a2); }
+  if (threadIdx.x == 0) { out2[0] = (double)a1; out2[1] = (double)a2; }     // launched as one block
 }
 
 __global__ void __launch_bounds__(256) k_dragan_xhat(const float* __restrict__ x, const float* __restrict__ alpha,
@@ -1390,7 +1416,7 @@ __global__ void __launch_bounds__(256) k_row_sumsq(const float* __restrict__ g, 
   float acc = 0.f;
   for (int64_t i = i0 + threadIdx.x; i < i1; i += blockDim.x) { float v = g[(int64_t)n * per + i]; acc += v * v; }
   acc = block_sum(acc, sm);
-  if (threadIdx.x == 0) atomicAdd(&ss[n], acc);
+  if (threadIdx.x == 0) ss[(int64_t)blockIdx.x * gridDim.y + n] = acc;     // partial of this block (add_partials)
 }
 
 __global__ void k_grad_penalty_finalize(float* __restrict__ coef, float lambda, float* __restrict__ loss, int N,
@@ -1469,7 +1495,7 @@ __global__ void __launch_bounds__(256) k_fanout_fwd(const float* __restrict__ go
   }
   acc0 = block_sum(acc0, sm);
   acc1 = block_sum(acc1, sm);
-  if (threadIdx.x == 0) { atomicAdd(&loss[0], acc0 * wn); atomicAdd(&loss[1], acc1 * wn); }
+  if (threadIdx.x == 0) { loss[2 * blockIdx.x] = acc0 * wn; loss[2 * blockIdx.x + 1] = acc1 * wn; }   // partials
 }
 
 // gradient w.r.t. the generator output: sum of what the discriminator batches, the second encoder batch and the
@@ -1516,7 +1542,7 @@ __global__ void __launch_bounds__(256) k_l1_groups(const float* __restrict__ a, 
     grad[g * per + i] = d > 0.f ? wn : (d < 0.f ? -wn : 0.f);
   }
   acc = block_sum(acc, sm);
-  if (threadIdx.x == 0) atomicAdd(&loss[g], acc * wn);
+  if (threadIdx.x == 0) loss[(int64_t)blockIdx.x * gridDim.y + g] = acc * wn;     // partial of this block (add_partials)
 }
 
 // out[g*per + i] = grad[g*per + i] * sign * (gl_g ? *gl_g : 0)
@@ -1789,7 +1815,7 @@ int twg_norm_act_bwd_apply_planes(const float* y, const float* a, const float* m
       for (float* o : outs)
         if (o) cudaMemsetAsync(o, 0, sizeof(float) * C, S(stream));
     }
-    k_norm_bwd_coeffs_inst<<<(unsigned)cdiv((int64_t)N * C, 256), 256, 0, S(stream)>>>(const_cast<float*>(red), ggamma0, gbeta0,
+    k_norm_bwd_coeffs_inst<<<(unsigned)cdiv((int64_t)C, 256), 256, 0, S(stream)>>>(const_cast<float*>(red), ggamma0, gbeta0,
                                                                                         ggamma1, gbeta1, (unsigned)dom_mask,
                                                                                         group_size, N, HW, C);
   } else {
@@ -1843,8 +1869,11 @@ int twg_colsum(const float* g, float* out, int64_t rows, int C, int accumulate, 
   if (blocks > 4 * kNumSMs) blocks = 4 * kNumSMs;
   int64_t chunk = cdiv(rows, blocks);
   blocks = cdiv(rows, chunk);
-  k_colsum<<<(unsigned)blocks, 256, 0, S(stream)>>>(g, out, rows, C, chunk);
-  return check_launch("twg_colsum");
+  float* parts = partials(blocks * C, true, S(stream));
+  if (!parts) return fail(TWG_ERR_UNSUPPORTED, "twg_colsum: C=%d too wide", C);
+  k_colsum<<<(unsigned)blocks, 256, 0, S(stream)>>>(g, parts, rows, C, chunk);
+  int rc = check_launch("twg_colsum");
+  return rc ? rc : add_partials(out, parts, (int)blocks, C, S(stream));
 }
 
 int twg_lrelu_bwd_colsum(const float* g, const float* ref, float* out, float* colsum, int64_t rows, int C, int lrelu_on,
@@ -1888,9 +1917,12 @@ int twg_lrelu_bwd_colsum_planes_pool_mask(const float* g, const float* ref, cons
     int rpb = (int)cdiv(img_rows, (int64_t)8 * kNumSMs);
     if (rpb < 1) rpb = 1;
     const unsigned nb = (unsigned)cdiv(img_rows, rpb);
-    if (mk) k_lrelu_bwd_colsum_pool_rows<true><<<nb, 256, 0, S(stream)>>>(g, ref, planes, colsum, img_rows, poolH, poolW, lq, rpb, mk, rows * C);
-    else k_lrelu_bwd_colsum_pool_rows<false><<<nb, 256, 0, S(stream)>>>(g, ref, planes, colsum, img_rows, poolH, poolW, lq, rpb, mk, rows * C);
-    return check_launch("twg_lrelu_bwd_colsum");
+    float* parts = partials((int64_t)nb * C, true, S(stream));
+    if (!parts) return fail(TWG_ERR_UNSUPPORTED, "twg_lrelu_bwd_colsum: C=%d too wide", C);
+    if (mk) k_lrelu_bwd_colsum_pool_rows<true><<<nb, 256, 0, S(stream)>>>(g, ref, planes, parts, img_rows, poolH, poolW, lq, rpb, mk, rows * C);
+    else k_lrelu_bwd_colsum_pool_rows<false><<<nb, 256, 0, S(stream)>>>(g, ref, planes, parts, img_rows, poolH, poolW, lq, rpb, mk, rows * C);
+    int rc = check_launch("twg_lrelu_bwd_colsum");
+    return rc ? rc : add_partials(colsum, parts, (int)nb, C, S(stream));
   }
   const int gpb = 256 / gm.G;
   int64_t blocks = cdiv(rows, (int64_t)gpb * 16);
@@ -1898,13 +1930,16 @@ int twg_lrelu_bwd_colsum_planes_pool_mask(const float* g, const float* ref, cons
   if (blocks < 1) blocks = 1;
   const int64_t chunk = cdiv(rows, blocks);
   blocks = cdiv(rows, chunk);
-#define TWG_LBC(v, m) k_lrelu_bwd_colsum_vec<v, m><<<(unsigned)blocks, 256, 0, S(stream)>>>(g, ref, out, planes, colsum, rows, C, gm.G, chunk, lrelu_on, poolH, poolW, mk)
+  float* parts = partials(blocks * C, true, S(stream));
+  if (!parts) return fail(TWG_ERR_UNSUPPORTED, "twg_lrelu_bwd_colsum: C=%d too wide", C);
+#define TWG_LBC(v, m) k_lrelu_bwd_colsum_vec<v, m><<<(unsigned)blocks, 256, 0, S(stream)>>>(g, ref, out, planes, parts, rows, C, gm.G, chunk, lrelu_on, poolH, poolW, mk)
   const bool use_mask = mk != nullptr && lrelu_on;
   if (gm.V == 1) { if (use_mask) TWG_LBC(1, true); else TWG_LBC(1, false); }
   else if (gm.V == 2) { if (use_mask) TWG_LBC(2, true); else TWG_LBC(2, false); }
   else { if (use_mask) TWG_LBC(4, true); else TWG_LBC(4, false); }
 #undef TWG_LBC
-  return check_launch("twg_lrelu_bwd_colsum");
+  if (int rc = check_launch("twg_lrelu_bwd_colsum")) return rc;
+  return add_partials(colsum, parts, (int)blocks, C, S(stream));
 }
 
 int twg_pool2(const float* x, float* out, int N, int H, int W, int C, float scale, twg_stream_t stream) {
@@ -2030,8 +2065,12 @@ int twg_l1(const float* a, const float* b, float weight, float* loss_out, float*
            twg_stream_t stream) {
   if (!a || !b || !loss_out || n <= 0) return fail(TWG_ERR_INVALID, "twg_l1: bad args");
   if (!accumulate) cudaMemsetAsync(loss_out, 0, sizeof(float), S(stream));
-  k_l1<<<grid_for(n, 8), 256, 0, S(stream)>>>(a, b, weight / (float)n, loss_out, grad_a, n);
-  return check_launch("twg_l1");
+  const unsigned nb = grid_for(n, 8);
+  float* parts = partials(nb, false, S(stream));
+  if (!parts) return fail(TWG_ERR_UNSUPPORTED, "twg_l1: scratch");
+  k_l1<<<nb, 256, 0, S(stream)>>>(a, b, weight / (float)n, parts, grad_a, n);
+  if (int rc = check_launch("twg_l1")) return rc;
+  return add_partials(loss_out, parts, (int)nb, 1, S(stream));
 }
 
 int twg_dragan_xhat(const float* x, const float* alpha, const float* noise, float* xhat, float* scratch2, int N,
@@ -2040,7 +2079,7 @@ int twg_dragan_xhat(const float* x, const float* alpha, const float* noise, floa
   double* s2 = reinterpret_cast<double*>(scratch2);  // caller provides >= 16 bytes, 8-byte aligned
   cudaMemsetAsync(s2, 0, 16, S(stream));
   const int64_t total = (int64_t)N * per_sample;
-  k_sum_sq<<<grid_for(total, 8), 256, 0, S(stream)>>>(x, s2, total);
+  k_sum_sq<<<1, 256, 0, S(stream)>>>(x, s2, total);     // one block: the sums come out the same on every run
   int rc = check_launch("twg_dragan_xhat/sum");
   if (rc) return rc;
   k_dragan_xhat<<<grid_for(total, 4), 256, 0, S(stream)>>>(x, alpha, noise, xhat, s2, N, per_sample);
@@ -2055,9 +2094,11 @@ int twg_grad_penalty(const float* g, float lambda, float* loss_out, float* coef,
   if (blocks > 64) blocks = 64;
   int64_t chunk = cdiv(per_sample, blocks);
   dim3 grid((unsigned)cdiv(per_sample, chunk), N);
-  k_row_sumsq<<<grid, 256, 0, S(stream)>>>(g, coef, per_sample, chunk);
-  int rc = check_launch("twg_grad_penalty/sumsq");
-  if (rc) return rc;
+  float* parts = partials((int64_t)grid.x * N, false, S(stream));
+  if (!parts) return fail(TWG_ERR_UNSUPPORTED, "twg_grad_penalty: scratch");
+  k_row_sumsq<<<grid, 256, 0, S(stream)>>>(g, parts, per_sample, chunk);
+  if (int rc = check_launch("twg_grad_penalty")) return rc;
+  if (int rc = add_partials(coef, parts, (int)grid.x, N, S(stream))) return rc;
   k_grad_penalty_finalize<<<1, 64, 0, S(stream)>>>(coef, lambda, loss_out, N, accumulate);
   return check_launch("twg_grad_penalty");
 }
@@ -2089,8 +2130,12 @@ int twg_fanout_fwd(const float* gout, const float* x, float* ds, float* dt, floa
     return fail(TWG_ERR_INVALID, "twg_fanout_fwd: bad args");
   const int64_t per = (int64_t)B * per_sample;
   cudaMemsetAsync(loss2, 0, 2 * sizeof(float), S(stream));
-  k_fanout_fwd<<<grid_for(per, 2), 256, 0, S(stream)>>>(gout, x, ds, dt, e2, sign_grad, loss2, weight / (float)per, per / 4);
-  return check_launch("twg_fanout_fwd");
+  const unsigned nb = grid_for(per, 2);
+  float* parts = partials(2 * (int64_t)nb, false, S(stream));
+  if (!parts) return fail(TWG_ERR_UNSUPPORTED, "twg_fanout_fwd: scratch");
+  k_fanout_fwd<<<nb, 256, 0, S(stream)>>>(gout, x, ds, dt, e2, sign_grad, parts, weight / (float)per, per / 4);
+  if (int rc = check_launch("twg_fanout_fwd")) return rc;
+  return add_partials(loss2, parts, (int)nb, 2, S(stream));
 }
 
 int twg_fanout_bwd(const float* gds, const float* gdt, const float* ge2, const float* sign_grad, const float* gl_s,
@@ -2106,8 +2151,11 @@ int twg_l1_groups(const float* a, const float* b, float weight, float* loss, flo
   if (!a || !b || !loss || !grad_a || groups <= 0 || per_group <= 0) return fail(TWG_ERR_INVALID, "twg_l1_groups: bad args");
   cudaMemsetAsync(loss, 0, groups * sizeof(float), S(stream));
   dim3 grid((unsigned)grid_for(per_group, 8), (unsigned)groups);
-  k_l1_groups<<<grid, 256, 0, S(stream)>>>(a, b, weight / (float)per_group, loss, grad_a, per_group);
-  return check_launch("twg_l1_groups");
+  float* parts = partials((int64_t)grid.x * groups, false, S(stream));
+  if (!parts) return fail(TWG_ERR_UNSUPPORTED, "twg_l1_groups: scratch");
+  k_l1_groups<<<grid, 256, 0, S(stream)>>>(a, b, weight / (float)per_group, parts, grad_a, per_group);
+  if (int rc = check_launch("twg_l1_groups")) return rc;
+  return add_partials(loss, parts, (int)grid.x, groups, S(stream));
 }
 
 int twg_scale_groups2(const float* grad, const float* gl0, const float* gl1, float sign, float* out, int64_t per_group,

@@ -27,7 +27,7 @@ FLAG_LRELU = 1
 FLAG_PIXNORM = 2
 NORM_NONE, NORM_INSTANCE, NORM_BATCH, NORM_RENORM = 0, 1, 2, 3
 
-# 1 = tcgen05 tensor-core convs where the library covers the shape, 0 = exact fp32 CUDA cores everywhere
+# 1 = wgmma tensor-core convs where the library covers the shape, 0 = exact fp32 CUDA cores everywhere
 _PREC = 1
 _TC_MIN_HW = 0   # layers with H < _TC_MIN_HW stay on the exact-fp32 CUDA-core path (precision policy knob)
 _TC_OK = {}          # (op, shape) -> bool, remembered capability of the tensor-core path
@@ -345,18 +345,9 @@ def _timed(fam, flops, fn):
   return out
 
 
-def _tc_family(H, W, kc, nc, k):
-  """Which tensor-core kernel the library dispatches for GEMM-K channels `kc`, GEMM-N channels `nc` (mirrors
-  halo_shape_ok in csrc/twg_conv_tc.cu); only used to label bench.py's per-kernel timing."""
-  small = (16, 32, 64)
-  if k == 3 and kc in small and nc in small and kc * nc <= 2048 and H >= 16 and W >= 16:
-    return 'tc_halo'
-  return 'tc_tap'
-
-
 def conv_fwd_planes(xp, wp, N, H, W, Cin, Cout, k, pad):
   y = torch.empty((N, H, W, Cout), device=xp.device, dtype=torch.float32)
-  _timed(_tc_family(H, W, Cin, Cout, k), (2.0 * N * H * W * Cin * Cout * k * k, 4.0 * N * H * W * (Cin + Cout)),
+  _timed('tc_fwd', (2.0 * N * H * W * Cin * Cout * k * k, 4.0 * N * H * W * (Cin + Cout)),
          lambda: lib().call('twg_conv_fwd_planes', _p(xp), _p(wp), _p(y), N, H, W, Cin, Cout, k, pad, _st()))
   return y
 
@@ -374,14 +365,14 @@ def conv_fwd_planes_stats(xp, wp, N, H, W, Cin, Cout, k, pad):
     return conv_fwd_planes(xp, wp, N, H, W, Cin, Cout, k, pad), None, 0
   y = torch.empty((N, H, W, Cout), device=xp.device, dtype=torch.float32)
   stats = torch.empty((N, slots, Cout, 4), device=xp.device, dtype=torch.float32)
-  _timed(_tc_family(H, W, Cin, Cout, k), (2.0 * N * H * W * Cin * Cout * k * k, 4.0 * N * H * W * (Cin + Cout)),
+  _timed('tc_fwd', (2.0 * N * H * W * Cin * Cout * k * k, 4.0 * N * H * W * (Cin + Cout)),
          lambda: L.call('twg_conv_fwd_planes_stats', _p(xp), _p(wp), _p(y), _p(stats), N, H, W, Cin, Cout, k, pad, _st()))
   return y, stats, slots
 
 
 def conv_dgrad_planes(gp, wp, N, H, W, Cin, Cout, k, pad):
   gx = torch.empty((N, H, W, Cin), device=gp.device, dtype=torch.float32)
-  _timed(_tc_family(H, W, Cout, Cin, k), (2.0 * N * H * W * Cin * Cout * k * k, 4.0 * N * H * W * (Cin + Cout)),
+  _timed('tc_fwd', (2.0 * N * H * W * Cin * Cout * k * k, 4.0 * N * H * W * (Cin + Cout)),
          lambda: lib().call('twg_conv_dgrad_planes', _p(gp), _p(wp), _p(gx), N, H, W, Cin, Cout, k, pad, _st()))
   return gx
 
@@ -545,11 +536,11 @@ class ConvBiasActFn(Function):
     if act and ACT_SIGN_MASK and L.cdll.twg_conv_has_act_mask(N, H, W_, Cin, Cout, k, pad):
       # the epilogue also writes the sign bits of z (one byte per 4 channels): all the first-order backward needs of z
       mask = torch.empty(z.numel() // 4, device=x.device, dtype=torch.uint8)
-      _timed(_tc_family(H, W_, Cin, Cout, k), (2.0 * N * H * W_ * Cin * Cout * k * k, 4.0 * N * H * W_ * (Cin + Cout)),
+      _timed('tc_fwd', (2.0 * N * H * W_ * Cin * Cout * k * k, 4.0 * N * H * W_ * (Cin + Cout)),
              lambda: L.call('twg_conv_bias_act_fwd_planes_mask', _p(xp), _p(weight_planes(w, False)), _p(_check(bias)),
                             _p(z), _p(zp), _p(mask), N, H, W_, Cin, Cout, k, pad, _st()))
     else:
-      _timed(_tc_family(H, W_, Cin, Cout, k), (2.0 * N * H * W_ * Cin * Cout * k * k, 4.0 * N * H * W_ * (Cin + Cout)),
+      _timed('tc_fwd', (2.0 * N * H * W_ * Cin * Cout * k * k, 4.0 * N * H * W_ * (Cin + Cout)),
              lambda: L.call('twg_conv_bias_act_fwd_planes', _p(xp), _p(weight_planes(w, False)), _p(_check(bias)),
                             int(act), _p(z), _p(zp), N, H, W_, Cin, Cout, k, pad, _st()))
     ctx.mask = mask
@@ -905,7 +896,7 @@ def norm_act_eval(y, gamma, beta, kind, flags, eps, moving_mean=None, moving_var
 
 
 def affine_epilogue_ok(N, H, W, Cin, Cout, k, pad) -> bool:
-  """Whether conv_affine_act_eval covers this shape (the halo kernel: a thread holds all Cout channels of its pixel)."""
+  """Whether conv_affine_act_eval covers this shape (one output-channel block: all Cout channels of a pixel are in one CTA)."""
   return bool(_PREC == 1 and tc_eligible(N, H, W, Cin, Cout, k, pad) and
               lib().cdll.twg_conv_has_act_mask(N, H, W, Cin, Cout, k, pad))
 
@@ -924,7 +915,7 @@ def conv_affine_act_eval(x, w, gamma, beta, moving_mean, moving_var, flags, eps,
   z = torch.empty((N, H, W_, Cout), device=x.device, dtype=torch.float32)
   planes_only = emit == 'planes'
   zp = _new_planes(z.shape, x.device) if emit in ('planes', 'both') else None
-  _timed(_tc_family(H, W_, Cin, Cout, 3), (2.0 * N * H * W_ * Cin * Cout * 9, 4.0 * N * H * W_ * (Cin + Cout)),
+  _timed('tc_fwd', (2.0 * N * H * W_ * Cin * Cout * 9, 4.0 * N * H * W_ * (Cin + Cout)),
          lambda: L.call('twg_conv_affine_act_fwd_planes', _p(xp), _p(weight_planes(w, False)), _p(ab[0]), _p(ab[1]), int(flags),
                         None if planes_only else _p(z), _p(zp), N, H, W_, Cin, Cout, 3, 1, _st()))
   if zp is not None:
