@@ -55,60 +55,56 @@ int64_t twg_launch_count(void);
  *      tf.gradients-generated Conv2DBackpropInput / Conv2DBackpropFilter -------------------------------
  * Stride 1.  x:[N,H,W,Cin]  w:[k,k,Cin,Cout]  y:[N,Ho,Wo,Cout], Ho = H + 2*pad - k + 1.
  * SAME for k=3 is pad=1, k=1 pad=0; VALID is pad=0.
- * `prec`: 0 = fp32 CUDA-core path (always available), 1 = wgmma tensor-core path with split-bf16
- * (3 MMAs per product, ~fp32 accuracy); the tensor-core path returns TWG_ERR_UNSUPPORTED for shapes it
- * does not cover and the caller picks prec=0 for those.                                              */
+ * Two kernel families: exact fp32 on fp32 operands (any shape), and wgmma tensor cores on split-bf16 planes (3 MMAs per
+ * product, ~fp32 accuracy) for the shapes twg_conv_path reports as TWG_CONV_TC.                                       */
+#define TWG_CONV_SIMT 0  /* exact fp32, CUDA cores */
+#define TWG_CONV_PW 1    /* exact fp32, the thin 1x1 layers (fromRGB / toRGB): twg_conv_fwd/dgrad/wgrad use it in any case */
+#define TWG_CONV_TC 2    /* tensor cores: 3x3 SAME / 1x1 with 16, 32, 64 or a multiple of 128 channels */
+/* which family covers this stride-1 conv shape (one of TWG_CONV_*) */
+int twg_conv_path(int N, int H, int W, int Cin, int Cout, int k, int pad);
+/* exact fp32: y = conv(x, w) */
 int twg_conv_fwd(const float* x, const float* w, float* y, int N, int H, int W, int Cin, int Cout, int k, int pad,
-                 int prec, void* workspace, int64_t workspace_bytes, twg_stream_t stream);
+                 twg_stream_t stream);
 /* gx:[N,H,W,Cin] = d/dx of sum(gy*y) */
 int twg_conv_dgrad(const float* gy, const float* w, float* gx, int N, int H, int W, int Cin, int Cout, int k, int pad,
-                   int prec, void* workspace, int64_t workspace_bytes, twg_stream_t stream);
+                   twg_stream_t stream);
 /* gw:[k,k,Cin,Cout] (+)= d/dw; accumulate!=0 adds into gw */
 int twg_conv_wgrad(const float* x, const float* gy, float* gw, int N, int H, int W, int Cin, int Cout, int k, int pad,
-                   int accumulate, int prec, void* workspace, int64_t workspace_bytes, twg_stream_t stream);
-/* bytes of scratch the three calls above need for this shape/precision (0 for prec=0) */
-int64_t twg_conv_workspace_bytes(int N, int H, int W, int Cin, int Cout, int k, int pad, int prec);
+                   int accumulate, twg_stream_t stream);
 
 /* ---- tensor-core convolution on pre-split operands ("split-bf16 planes": hi plane then lo plane, bf16, same
  *      NHWC element order as the fp32 tensor; x = hi + lo).  Lets the caller split an activation once and reuse
  *      it for forward + wgrad, a gradient once for dgrad + wgrad, and a weight once per optimiser step.        */
-/* 1 if the tensor-core path covers this stride-1 conv shape (3x3 SAME / 1x1, channels multiple of 16), else 0 */
-int twg_conv_tc_supported(int N, int H, int W, int Cin, int Cout, int k, int pad);
 /* planes: 2*n bf16 */
 int twg_split_act(const float* x, void* planes, int64_t n, twg_stream_t stream);
 /* planes: 2*k*k*Cin*Cout bf16; dgrad=0: [tap][Cout][Cin] (forward operand), dgrad=1: [flip(tap)][Cin][Cout] */
 int twg_split_weights(const float* w, void* planes, int k, int Cin, int Cout, int dgrad, twg_stream_t stream);
-int twg_conv_fwd_planes(const void* x_planes, const void* w_planes, float* y, int N, int H, int W, int Cin, int Cout,
-                        int k, int pad, twg_stream_t stream);
-/* Same with lrelu_on = 1, and the SIGN MASK of z as a by-product: act_mask[i] (one byte per 4 consecutive channels, bit j =
- * z[4i+j] > 0), which is all the first-order backward of tf.maximum(0.2x, x) needs (util_misc.py:86) -- the backward then
- * reads 0.25 B instead of 4 B per element (twg_lrelu_bwd_colsum_planes_pool_mask).  twg_conv_has_act_mask: 1 if the shape
- * runs on a kernel with this epilogue. */
-int twg_conv_has_act_mask(int N, int H, int W, int Cin, int Cout, int k, int pad);
-int twg_conv_bias_act_fwd_planes_mask(const void* x_planes, const void* w_planes, const float* bias, float* z, void* z_planes,
-                                      void* act_mask, int N, int H, int W, int Cin, int Cout, int k, int pad,
-                                      twg_stream_t stream);
+/* Fused epilogue of the forward conv (sign mask, statistics, evaluation-mode affine): the number of statistics records
+ * per image it writes for this shape, 0 when the shape has no fused epilogue (the small-channel high-resolution layers
+ * have one: a pixel's Cout channels sit in one CTA). */
+int twg_conv_epilogue_slots(int N, int H, int W, int Cin, int Cout, int k, int pad);
+/* y = lrelu?(conv(x, w) + bias): bias (nullable) and act = 1 (leaky-ReLU, needs bias) give the discriminator layer in one
+ * kernel (nets/pggan_utils.py:116-127), so the pre-activation never touches HBM.  Optional outputs (each nullable):
+ *  - z_planes: y also as split planes, for the next conv;
+ *  - act_mask (act = 1): the SIGN MASK of y, act_mask[i] one byte per 4 consecutive channels, bit j = y[4i+j] > 0, which
+ *    is all the first-order backward of tf.maximum(0.2x, x) needs (util_misc.py:86) -- the backward then reads 0.25 B
+ *    instead of 4 B per element (twg_lrelu_bwd_colsum);
+ *  - stats (no bias, no z_planes): the statistics tf.nn.moments would take over y (libs/instance_norm.py:131-135 after
+ *    nets/pggan.py:78-81), from the conv epilogue: stats[n][slot][c] = {count, pivot, sum (y - pivot), sum (y - pivot)^2}
+ *    (float4) over the pixels one epilogue warp drained, slot < twg_conv_epilogue_slots(...) per image -- no second pass
+ *    over y, no atomics.  N * slots * Cout float4, fully written by the call.
+ * act_mask and stats need twg_conv_epilogue_slots(...) > 0. */
+int twg_conv_fwd_planes(const void* x_planes, const void* w_planes, const float* bias, int act, float* y, void* z_planes,
+                        void* act_mask, float* stats, int N, int H, int W, int Cin, int Cout, int k, int pad,
+                        twg_stream_t stream);
 /* Inference-mode generator / encoder layer in ONE kernel (nets/pggan.py:78-81 with is_training=False:
  * libs/batch_norm.py:266-278 turns the normaliser into the per-channel affine a = gamma / sqrt(moving_var + eps),
  * b = beta - moving_mean * a, twg_norm_eval_affine):  z = pixel_norm?(lrelu?(a[c] * conv(x, w) + b[c])), flags =
  * TWG_FLAG_LRELU | TWG_FLAG_PIXNORM, written as fp32 z and / or split planes (either may be NULL, not both).  Covered
- * shapes: twg_conv_has_act_mask(...) == 1 (one output-channel block: a pixel's Cout channels sit in one CTA). */
+ * shapes: twg_conv_epilogue_slots(...) > 0. */
 int twg_conv_affine_act_fwd_planes(const void* x_planes, const void* w_planes, const float* a, const float* b, int flags,
                                    float* z, void* z_planes, int N, int H, int W, int Cin, int Cout, int k, int pad,
                                    twg_stream_t stream);
-/* Forward conv that also emits the statistics tf.nn.moments would take over y (libs/instance_norm.py:131-135 after
- * nets/pggan.py:78-81), from the conv epilogue: stats[n][slot][c] = {count, pivot, sum (y - pivot), sum (y - pivot)^2}
- * (float4) over the pixels one epilogue warp drained, slot < twg_conv_stats_slots(...) per image -- no second pass over
- * y, no atomics.  twg_conv_stats_slots returns 0 when the shape runs on a kernel without this epilogue (the caller then
- * uses twg_moments).  stats: N * slots * Cout float4, fully written by the call. */
-int twg_conv_stats_slots(int N, int H, int W, int Cin, int Cout, int k, int pad);
-int twg_conv_fwd_planes_stats(const void* x_planes, const void* w_planes, float* y, float* stats, int N, int H, int W,
-                              int Cin, int Cout, int k, int pad, twg_stream_t stream);
-/* discriminator layer in one kernel: z = lrelu?(conv(x, w) + bias)  (nets/pggan_utils.py:116-127), fused in the
- * conv epilogue so the pre-activation never touches HBM */
-int twg_conv_bias_act_fwd_planes(const void* x_planes, const void* w_planes, const float* bias, int lrelu_on, float* z,
-                                 void* z_planes /* nullable: also emit z as split planes for the next conv */, int N,
-                                 int H, int W, int Cin, int Cout, int k, int pad, twg_stream_t stream);
 int twg_conv_dgrad_planes(const void* gy_planes, const void* w_planes, float* gx, int N, int H, int W, int Cin,
                           int Cout, int k, int pad, twg_stream_t stream);
 int twg_conv_wgrad_planes(const void* x_planes, const void* gy_planes, float* gw, int N, int H, int W, int Cin,
@@ -138,7 +134,7 @@ int twg_norm_finalize(const float* sums, const float* y, const float* gamma0, co
                       const float* beta1, int dom_mask, int group_size, const float* renorm0, const float* renorm1,
                       int kind, float eps, const float* clip, float* a, float* b, float* mean, float* rstd, float* rd_out,
                       float* batch_stats, int N, int HW, int C, twg_stream_t stream);
-/* Instance-norm variant of twg_norm_finalize that merges the epilogue records of twg_conv_fwd_planes_stats (records
+/* Instance-norm variant of twg_norm_finalize that merges the epilogue statistics records of twg_conv_fwd_planes (records
  * re-based to one pivot drawn from the data: the accuracy of tf.nn.moments' two-pass form, libs/instance_norm.py:131-135) */
 int twg_norm_finalize_partials(const float* stats, int slots, const float* gamma0, const float* beta0, const float* gamma1,
                                const float* beta1, int dom_mask, int group_size, float eps, float* a, float* b, float* mean,
@@ -146,31 +142,26 @@ int twg_norm_finalize_partials(const float* stats, int slots, const float* gamma
 /* Evaluation-mode affine from moving statistics (libs/batch_norm.py:266-278): a,b:[N][C] broadcast */
 int twg_norm_eval_affine(const float* gamma, const float* beta, const float* moving_mean, const float* moving_var,
                          float eps, float* a, float* b, int N, int C, twg_stream_t stream);
-/* z = pixnorm?( lrelu?( a[n,c]*y + b[n,c] ) ) */
-int twg_norm_act_fwd(const float* y, const float* a, const float* b, float* z, int N, int HW, int C, int flags,
-                     twg_stream_t stream);
-/* same, additionally (or only, when z is null) writing the result as split-bf16 planes for the next tensor-core conv */
-int twg_norm_act_fwd_planes(const float* y, const float* a, const float* b, float* z, void* planes, int N, int HW, int C,
-                            int flags, twg_stream_t stream);
-/* first backward pass: gu = d/du of the activation/pixel-norm part, red[n][c] = {sum gu, sum gu*yhat} */
+/* z = pixnorm?( lrelu?( a[n,c]*y + b[n,c] ) ) as fp32 z and / or split-bf16 planes for the next tensor-core conv
+ * (either may be NULL, not both) */
+int twg_norm_act_fwd(const float* y, const float* a, const float* b, float* z, void* planes, int N, int HW, int C,
+                     int flags, twg_stream_t stream);
+/* first backward pass: gu = d/du of the activation/pixel-norm part, red[n][c] = {sum gu, sum gu*yhat}.  For a layer
+ * whose output also feeds a 2x2 average pool (nets/pggan.py:436,468), `gpool` [N,H/2,W/2,C] is the gradient w.r.t. the
+ * pooled tensor; its contribution 0.25*gpool[h/2][w/2] is added on the fly (the full-resolution pool gradient and
+ * autograd's accumulation with a UNet-skip gradient `gz` are never materialised).  gz or gpool may be NULL, not both.
+ * W = row length of the full-resolution tensor (read only with gpool). */
 int twg_norm_act_bwd_reduce(const float* y, const float* a, const float* b, const float* mean, const float* rstd,
-                            const float* gz, float* gu, float* red, int N, int HW, int C, int flags,
-                            twg_stream_t stream);
-/* Same, for a layer whose output also feeds a 2x2 average pool (nets/pggan.py:436,468): `gpool` [N,H/2,W/2,C] is the
- * gradient w.r.t. the pooled tensor; its contribution 0.25*gpool[h/2][w/2] is added on the fly (the full-resolution
- * pool gradient and autograd's accumulation with a UNet-skip gradient `gz` are never materialised).  gz or gpool may
- * be NULL, not both.  W = row length of the full-resolution tensor. */
-int twg_norm_act_bwd_reduce_pool(const float* y, const float* a, const float* b, const float* mean, const float* rstd,
-                                 const float* gz, const float* gpool, int W, float* gu, float* red, int N, int HW, int C,
-                                 int flags, twg_stream_t stream);
+                            const float* gz, const float* gpool, int W, float* gu, float* red, int N, int HW, int C,
+                            int flags, twg_stream_t stream);
 /* second pass: gy = a*(gu - S1/M - yhat*S2/M) with the reduction domain of `kind` (fp32 and/or split-bf16 planes, the
  * operand dgrad and wgrad consume); ggammaX[C], gbetaX[C] = parameter gradients of domain X over its groups (groups /
  * dom_mask as in twg_norm_finalize; += when accumulate, e.g. straight into the flat gradient buffer); rd:[groups][2][C]
  * (r,d; null => r=1,d=0) */
-int twg_norm_act_bwd_apply_planes(const float* y, const float* a, const float* mean, const float* rstd, const float* gu,
-                                  const float* red, const float* rd, float* gy, void* gy_planes, float* ggamma0,
-                                  float* gbeta0, float* ggamma1, float* gbeta1, int accumulate, int dom_mask,
-                                  int group_size, int kind, int N, int HW, int C, twg_stream_t stream);
+int twg_norm_act_bwd_apply(const float* y, const float* a, const float* mean, const float* rstd, const float* gu,
+                           const float* red, const float* rd, float* gy, void* gy_planes, float* ggamma0, float* gbeta0,
+                           float* ggamma1, float* gbeta1, int accumulate, int dom_mask, int group_size, int kind, int N,
+                           int HW, int C, twg_stream_t stream);
 /* EMA pushes (libs/batch_norm.py:295-319, 359-393); decay 0.99 for batch_renorm (nets/pggan_utils.py:165), 0.999 for
  * plain batch_norm (libs/batch_norm.py:44 default): state layout per (layer,domain):
  * moving_mean[C], moving_var[C], renorm_mean[C], renorm_stddev[C], renorm_mean_weight, renorm_stddev_weight */
@@ -178,40 +169,33 @@ int twg_norm_update_stats(float* state, const float* batch_stats, int kind, floa
                           twg_stream_t stream);
 
 /* ---- discriminator-style bias + leaky-ReLU (nets/pggan_utils.py:116-127) -------------------------- */
-int twg_bias_lrelu_fwd(const float* y, const float* bias, float* z, int64_t rows, int C, int lrelu, twg_stream_t stream);
-/* Same; z additionally as split-bf16 planes (for the tensor-core conv that consumes it) and / or as its sign mask (one byte
- * per 4 channels, bit j = z[4i+j] > 0, for twg_lrelu_bwd_colsum_planes_pool_mask); either may be NULL; C % 4 == 0 */
-int twg_bias_lrelu_fwd_planes_mask(const float* y, const float* bias, float* z, void* planes, void* mask, int64_t rows, int C,
-                                   int lrelu_on, twg_stream_t stream);
+/* z = lrelu?(y + bias); z additionally as split-bf16 planes (for the tensor-core conv that consumes it) and / or as its
+ * sign mask (one byte per 4 channels, bit j = z[4i+j] > 0, for twg_lrelu_bwd_colsum); either may be NULL, and needs
+ * C % 4 == 0 */
+int twg_bias_lrelu_fwd(const float* y, const float* bias, float* z, void* planes, void* mask, int64_t rows, int C,
+                       int lrelu_on, twg_stream_t stream);
 /* out = g * (ref>0 ? 1 : 0.2)   (gradient of tf.maximum(0.2x,x); ref may be the activation output) */
 int twg_lrelu_bwd(const float* g, const float* ref, float* out, int64_t n, twg_stream_t stream);
-/* fused: out = lrelu_on ? g*slope(ref) : g (not written when lrelu_on=0) and colsum[c] (+)= sum_rows out[row][c] */
-int twg_lrelu_bwd_colsum(const float* g, const float* ref, float* out, float* colsum, int64_t rows, int C, int lrelu_on,
-                         int accumulate, twg_stream_t stream);
-/* Same, `out` optionally (or only) as split planes, and with `g` optionally given as the gradient w.r.t. avg_pool2(z)
- * ([N,poolH/2,poolW/2,C]; poolW = 0: plain form). */
-int twg_lrelu_bwd_colsum_planes_pool(const float* g, const float* ref, float* out, void* planes, float* colsum,
-                                     int64_t rows, int C, int lrelu_on, int poolH, int poolW, int accumulate,
-                                     twg_stream_t stream);
-/* Same with the activation's sign taken from `mask` (twg_conv_bias_act_fwd_planes_mask) instead of `ref` when mask != NULL */
-int twg_lrelu_bwd_colsum_planes_pool_mask(const float* g, const float* ref, const void* mask, float* out, void* planes,
-                                          float* colsum, int64_t rows, int C, int lrelu_on, int poolH, int poolW,
-                                          int accumulate, twg_stream_t stream);
+/* fused: out = lrelu_on ? g*slope(ref) : g (not written when lrelu_on=0) and colsum[c] (+)= sum_rows out[row][c].
+ * `out` fp32 and / or (`planes`) split planes; the activation's sign from `mask` (twg_conv_fwd_planes, twg_bias_lrelu_fwd)
+ * instead of `ref` when mask != NULL; `g` optionally given as the gradient w.r.t. avg_pool2(z) ([N,poolH/2,poolW/2,C];
+ * poolW = 0: plain form). */
+int twg_lrelu_bwd_colsum(const float* g, const float* ref, const void* mask, float* out, void* planes, float* colsum,
+                         int64_t rows, int C, int lrelu_on, int poolH, int poolW, int accumulate, twg_stream_t stream);
 /* out[c] (+)= sum_rows g[row][c] */
 int twg_colsum(const float* g, float* out, int64_t rows, int C, int accumulate, twg_stream_t stream);
 
 /* ---- resampling (nets/pggan_utils.py:349-350; tf.nn.avg_pool nets/pggan.py:274,306,436,468) -------- */
-/* out[N,H/2,W/2,C] = scale * sum of the 2x2 block (scale .25 = avg-pool; 1 = gradient of nearest x2) */
-int twg_pool2(const float* x, float* out, int N, int H, int W, int C, float scale, twg_stream_t stream);
-int twg_pool2_planes(const float* x, float* out, void* planes, int N, int H, int W, int C, float scale,
-                     twg_stream_t stream);
+/* out[N,H/2,W/2,C] = scale * sum of the 2x2 block (scale .25 = avg-pool; 1 = gradient of nearest x2); `out` fp32 and / or
+ * split planes */
+int twg_pool2(const float* x, float* out, void* planes, int N, int H, int W, int C, float scale, twg_stream_t stream);
 /* out[N,2H,2W,C] = scale * x[i/2,j/2] (scale 1 = nearest x2; .25 = gradient of avg-pool) */
 int twg_upsample2(const float* x, float* out, int N, int H, int W, int C, float scale, twg_stream_t stream);
 /* UNet join (nets/pggan_utils.py:281-298 + :349): out[N,2H,2W,Ca+Cb] = concat(nearest2(a[N,H,W,Ca]), b[n % Nb]) with
  * b:[Nb,2H,2W,Cb] -- Nb < N when several generator passes that share one encoder pass run as one batch.  `out` fp32
  * and/or split planes. */
-int twg_upsample_concat_planes(const float* a, const float* b, float* out, void* planes, int N, int H, int W, int Ca,
-                               int Cb, int Nb, twg_stream_t stream);
+int twg_upsample_concat(const float* a, const float* b, float* out, void* planes, int N, int H, int W, int Ca, int Cb,
+                        int Nb, twg_stream_t stream);
 /* its gradient: ga[N,H,W,Ca] = sum2x2(gout[..., :Ca]); gb[m] = sum_j gout[m + j*Nb][..., Ca:] */
 int twg_upsample_concat_bwd(const float* gout, float* ga, float* gb, int N, int H, int W, int Ca, int Cb, int Nb,
                             twg_stream_t stream);
@@ -311,8 +295,6 @@ int twg_adam(float* p, const float* g, float* m, float* v, int64_t n, float lr_t
  * can be replayed while the Adam time step advances) */
 int twg_adam_dev_lr(float* p, const float* g, float* m, float* v, int64_t n, const float* lr_t_dev, float beta1,
                     float beta2, float eps, twg_stream_t stream);
-/* dst = 0 */
-int twg_zero(float* dst, int64_t n, twg_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -22,17 +22,48 @@ def test_library_loads_and_exports_every_header_symbol(built_lib):
   assert declared == set(protos), declared ^ set(protos)
 
 
-def test_host_side_argument_validation_without_gpu(built_lib):
+def test_conv_and_pool_entries_reject_bad_arguments_without_gpu(built_lib):
   L = built_lib
-  assert L.try_call('twg_conv_fwd', None, None, None, 1, 4, 4, 16, 16, 3, 1, 0, None, 0, None) == -1
+  assert L.try_call('twg_conv_fwd', None, None, None, 1, 4, 4, 16, 16, 3, 1, None) == -1
   assert 'null' in L.last_error()
-  assert L.try_call('twg_conv_fwd', 8, 8, 8, 1, 2, 2, 4, 4, 5, 0, 0, None, 0, None) == -1      # empty output
-  assert L.try_call('twg_conv_wgrad', 8, 8, 8, 0, 4, 4, 4, 4, 3, 1, 0, 0, None, 0, None) == -1  # N=0 (empty batch)
-  assert L.try_call('twg_pool2', 8, 8, 1, 3, 4, 1, 0.25, None) == -1                           # odd H
-  # workspace query is a pure host function
-  assert L.cdll.twg_conv_workspace_bytes(16, 256, 256, 16, 16, 3, 1, 0) == 0
-  assert L.cdll.twg_conv_workspace_bytes(16, 256, 256, 16, 16, 3, 1, 1) > 2 * 16 * 256 * 256 * 16 * 4
-  assert L.cdll.twg_conv_workspace_bytes(4, 4, 4, 257, 256, 3, 1, 1) == 0                      # not covered by tensor cores
+  assert L.try_call('twg_conv_fwd', 8, 8, 8, 1, 2, 2, 4, 4, 5, 0, None) == -1           # empty output
+  assert L.try_call('twg_conv_wgrad', 8, 8, 8, 0, 4, 4, 4, 4, 3, 1, 0, None) == -1      # N=0 (empty batch)
+  assert L.try_call('twg_pool2', 8, 8, None, 1, 3, 4, 1, 0.25, None) == -1              # odd H
+
+
+def test_every_library_call_matches_the_header_arity():
+  """Every call in the package that names a library function -- `lib().call('twg_...', ...)`, `.try_call(...)`, the conv
+  launcher `_conv_launch(family, shape, 'twg_...', ...)`, `.cdll.twg_...(...)` -- passes as many arguments as include/twg.h
+  declares.  (ctypes checks the count only when a call is made, and without a GPU no kernel call is.)"""
+  import ast
+  from twingan_b200 import _lib
+  protos = _lib.parse_header()
+  pkg = os.path.join(ROOT, 'twingan_b200')
+  seen = 0
+  for fn in sorted(os.listdir(pkg)):
+    if not fn.endswith('.py'):
+      continue
+    for node in ast.walk(ast.parse(open(os.path.join(pkg, fn)).read())):
+      if not isinstance(node, ast.Call):
+        continue
+      named = [i for i, a in enumerate(node.args) if isinstance(a, ast.Constant) and str(a.value).startswith('twg_')]
+      f = node.func
+      if named:
+        name, args = node.args[named[0]].value, node.args[named[0] + 1:]
+      elif isinstance(f, ast.Attribute) and f.attr.startswith('twg_') and isinstance(f.value, ast.Attribute) \
+          and f.value.attr == 'cdll':
+        name, args = f.attr, node.args
+      else:
+        continue
+      where = '%s:%d %s' % (fn, node.lineno, name)
+      assert name in protos, where
+      want = len(protos[name][1])
+      if any(isinstance(a, ast.Starred) for a in args):    # (..., *ptrs, ...): at least not too many
+        assert len([a for a in args if not isinstance(a, ast.Starred)]) < want, where
+      else:
+        assert len(args) == want, (where, len(args), want)
+      seen += 1
+  assert seen >= 60, seen
 
 
 def test_product_never_imports_the_oracle_and_fails_loudly_without_cuda():

@@ -215,15 +215,15 @@ def test_adam_tf_epsilon_placement(built_lib):
   assert rel_err(pd, rp) < 1e-6 and rel_err(md, rm) < 1e-6 and rel_err(vd, rv) < 1e-6
 
 
-def test_empty_and_invalid_arguments(built_lib):
+def test_conv_and_pool_entries_reject_bad_arguments_on_gpu(built_lib):
   """Error behaviour of the C-ABI: invalid geometry returns a negative status and a message, never aborts."""
   L = built_lib
   x = torch.zeros(16, device='cuda:0')
-  rc = L.try_call('twg_conv_fwd', x.data_ptr(), x.data_ptr(), x.data_ptr(), 1, 2, 2, 1, 1, 5, 0, 0, None, 0, None)
+  rc = L.try_call('twg_conv_fwd', x.data_ptr(), x.data_ptr(), x.data_ptr(), 1, 2, 2, 1, 1, 5, 0, None)
   assert rc == -1 and 'empty output' in L.last_error()
-  rc = L.try_call('twg_conv_fwd', None, x.data_ptr(), x.data_ptr(), 1, 2, 2, 1, 1, 1, 0, 0, None, 0, None)
+  rc = L.try_call('twg_conv_fwd', None, x.data_ptr(), x.data_ptr(), 1, 2, 2, 1, 1, 1, 0, None)
   assert rc == -1 and 'null' in L.last_error()
-  rc = L.try_call('twg_pool2', x.data_ptr(), x.data_ptr(), 1, 3, 3, 1, 0.25, None)
+  rc = L.try_call('twg_pool2', x.data_ptr(), x.data_ptr(), None, 1, 3, 3, 1, 0.25, None)
   assert rc == -1
 
 
@@ -584,8 +584,8 @@ STATS_SHAPES = [(3, 64, 64, 16, 16), (2, 24, 40, 16, 32), (2, 128, 128, 32, 32),
 
 @pytest.mark.parametrize('offset', [0.0, 40.0])
 @pytest.mark.parametrize('shape', STATS_SHAPES)
-def test_conv_epilogue_statistics(built_lib, shape, offset):
-  """Instance-norm statistics taken in the conv epilogue (twg_conv_fwd_planes_stats + twg_norm_finalize_partials) against
+def test_conv_fwd_planes_epilogue_statistics(built_lib, shape, offset):
+  """Instance-norm statistics taken in the conv epilogue (twg_conv_fwd_planes + twg_norm_finalize_partials) against
   tf.nn.moments' two-pass definition on the conv output, incl. |mean| >> std (a constant input offset makes every output
   channel's mean large): mean to 1e-6 of its scale, rstd to 1e-4 relative."""
   from twingan_b200 import ops
@@ -599,10 +599,12 @@ def test_conv_epilogue_statistics(built_lib, shape, offset):
   gamma1 = 1 + _rand((Cout,), 25, 0.2)
   beta1 = _rand((Cout,), 26, 0.1)
   xd, wd = _dev(x), _dev(w)
-  xp, wp = ops.split_act(xd), ops.weight_planes(wd, False)
-  y, stats, slots = ops.conv_fwd_planes_stats(xp, wp, N, H, W, Cin, Cout, 3, 1)
-  assert stats is not None and slots > 0, 'this shape must offer epilogue statistics'
-  y_plain = ops.conv_fwd_planes(xp, wp, N, H, W, Cin, Cout, 3, 1)
+  xp = ops.split_act(xd)
+  slots = ops._epilogue_slots(N, H, W, Cin, Cout, 3, 1)
+  assert slots > 0, 'this shape must offer epilogue statistics'
+  stats = torch.empty((N, slots, Cout, 4), device='cuda:0')
+  y, _ = ops._conv_fwd(None, wd, 3, 1, xp=xp, stats=stats)
+  y_plain, _ = ops._conv_fwd(None, wd, 3, 1, xp=xp)
   assert torch.equal(y, y_plain)                       # the statistics epilogue does not change y
   buf = torch.empty((4, N, Cout), device='cuda:0')
   dom_mask, gs = 0b10 if N % 2 == 0 else 0, (N // 2 if N % 2 == 0 else N)
@@ -658,7 +660,7 @@ def test_generator_layer_epilogue_statistics_match_moments_pass(built_lib):
                                    (1, 64, 64, 32, 32)])   # the last two are wide enough for the image-row backward kernel
 def test_discriminator_layer_sign_mask_backward_is_bit_identical(built_lib, shape, pool):
   """The discriminator layer's first-order backward reads the activation's sign from the byte mask the conv epilogue wrote
-  (twg_conv_bias_act_fwd_planes_mask -> twg_lrelu_bwd_colsum_planes_pool_mask) instead of z: same forward tensors and,
+  (twg_conv_fwd_planes -> twg_lrelu_bwd_colsum) instead of z: same forward tensors and,
   bit for bit, the same input / weight / bias gradients as the path that reads z (util_misc.py:86: the gradient of
   tf.maximum(0.2 x, x) depends on x only through its sign)."""
   from twingan_b200 import ops

@@ -682,18 +682,6 @@ static bool tc_shape_ok(int N, int H, int W, int Cin, int Cout, int k, int pad) 
   return true;
 }
 
-static inline int64_t align_up(int64_t v, int64_t a) { return (v + a - 1) / a * a; }
-
-bool conv_tc_supported(int N, int H, int W, int Cin, int Cout, int k, int pad);
-
-int64_t conv_tc_workspace(int N, int H, int W, int Cin, int Cout, int k, int pad) {
-  if (!conv_tc_supported(N, H, W, Cin, Cout, k, pad)) return 0;
-  const int64_t px = (int64_t)N * H * W;
-  const int64_t cmax = Cin > Cout ? Cin : Cout;
-  // two activation-sized split buffers (x and gy for wgrad) + weights
-  return 2 * align_up(px * cmax * 4, 1024) + align_up((int64_t)k * k * Cin * Cout * 4, 1024) + 4096;
-}
-
 template <int CC, int BN>
 static int launch_fwd(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl, float* y,
                       const TcGeom& g, const float* bias, int act, void* z_planes, float4* stats, uint8_t* act_mask,
@@ -739,16 +727,11 @@ bool conv_tc_supported(int N, int H, int W, int Cin, int Cout, int k, int pad) {
   return pick_tile(g);
 }
 
-// Records per image the forward kernel writes when asked for epilogue statistics (0: not offered for this shape): one
-// {count, pivot, S1, S2} per (16 x 8 tile, consumer warp, channel).
-int conv_fwd_stats_slots(int N, int H, int W, int Cin, int Cout, int k, int pad) {
+// Records per image the forward kernel writes when asked for epilogue statistics: one {count, pivot, S1, S2} per
+// (16 x 8 tile, consumer warp, channel).  0: the shape has no fused epilogue (no statistics, sign mask or affine).
+int conv_fwd_epilogue_slots(int N, int H, int W, int Cin, int Cout, int k, int pad) {
   if (!tc_shape_ok(N, H, W, Cin, Cout, k, pad) || !epi_shape_ok(H, W, Cin, Cout, k, pad)) return 0;
   return (int)(cdiv(H, 8) * cdiv(W, 16) * kConsumerWarps);
-}
-
-// whether the fused bias + leaky-ReLU epilogue of this forward shape can also write the activation's sign mask
-bool conv_fwd_has_act_mask(int N, int H, int W, int Cin, int Cout, int k, int pad) {
-  return tc_shape_ok(N, H, W, Cin, Cout, k, pad) && epi_shape_ok(H, W, Cin, Cout, k, pad);
 }
 
 // core: activation planes [2][N,H,W,Kc] (Kc = Cin for forward, Cout for dgrad), weight planes from split_weight_planes
@@ -757,12 +740,13 @@ int conv_fwd_tc_planes(const void* a_planes, const void* w_planes, float* y, int
                        void* z_planes = nullptr, float4* stats = nullptr, uint8_t* act_mask = nullptr,
                        const float* aff_a = nullptr) {
   if (!tc_shape_ok(N, H, W, Cin, Cout, k, pad)) return fail(TWG_ERR_UNSUPPORTED, "tensor-core conv: shape not covered");
-  if (aff_a && (dgrad || !bias || stats || act_mask || !conv_fwd_has_act_mask(N, H, W, Cin, Cout, k, pad)))
+  const bool fused = conv_fwd_epilogue_slots(N, H, W, Cin, Cout, k, pad) > 0;
+  if (aff_a && (dgrad || !bias || stats || act_mask || !fused))
     return fail(TWG_ERR_UNSUPPORTED, "tensor-core conv: no affine epilogue for this call");
   if (!y && !(aff_a && z_planes)) return fail(TWG_ERR_INVALID, "tensor-core conv: null output");
-  if (act_mask && (dgrad || !bias || !act || !conv_fwd_has_act_mask(N, H, W, Cin, Cout, k, pad)))
+  if (act_mask && (dgrad || !bias || !act || !fused))
     return fail(TWG_ERR_UNSUPPORTED, "tensor-core conv: no activation mask for this call");
-  if (stats && (dgrad || bias || z_planes || conv_fwd_stats_slots(N, H, W, Cin, Cout, k, pad) == 0))
+  if (stats && (dgrad || bias || z_planes || !fused))
     return fail(TWG_ERR_UNSUPPORTED, "tensor-core conv: no epilogue statistics for this call");
   TcGeom g{};
   g.N = N; g.H = H; g.W = W; g.k = k; g.pad = pad;
@@ -793,22 +777,6 @@ int conv_fwd_tc_planes(const void* a_planes, const void* w_planes, float* y, int
   TWG_FWD_CASE(64, 16) TWG_FWD_CASE(64, 32) TWG_FWD_CASE(64, 64) TWG_FWD_CASE(64, 128)
 #undef TWG_FWD_CASE
   return fail(TWG_ERR_UNSUPPORTED, "tensor-core conv: no kernel for CC=%d BN=%d", CC, BN);
-}
-
-// x: [N,H,W,Cin_x] fp32 (for dgrad: gy with Cin_x = Cout), w: HWIO; splits into the caller's workspace first
-int conv_fwd_tc(const float* x, const float* w, float* y, int N, int H, int W, int Cin, int Cout, int k, int pad,
-                bool dgrad, void* ws, int64_t ws_bytes, cudaStream_t st) {
-  if (!conv_tc_supported(N, H, W, Cin, Cout, k, pad)) return fail(TWG_ERR_UNSUPPORTED, "tensor-core conv: shape not covered");
-  if (!ws || ws_bytes < conv_tc_workspace(N, H, W, Cin, Cout, k, pad)) return fail(TWG_ERR_INVALID, "tensor-core conv: workspace too small");
-  const int64_t px = (int64_t)N * H * W;
-  const int64_t cmax = Cin > Cout ? Cin : Cout;
-  const int kc = dgrad ? Cout : Cin;
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(ws) + 1023) & ~uintptr_t(1023));
-  uint8_t* wbase = base + 2 * align_up(px * cmax * 4, 1024);
-  int rc = split_act_planes(x, base, px * kc, st);
-  if (rc) return rc;
-  if ((rc = split_weight_planes(w, wbase, k, Cin, Cout, dgrad ? 1 : 0, st))) return rc;
-  return conv_fwd_tc_planes(base, wbase, y, N, H, W, Cin, Cout, k, pad, dgrad, st);
 }
 
 template <int CN, int BNW>
@@ -868,20 +836,6 @@ int conv_wgrad_tc_planes(const void* x_planes, const void* g_planes, float* gw, 
   TWG_WG_CASE(64, 16) TWG_WG_CASE(64, 32)
 #undef TWG_WG_CASE
   return fail(TWG_ERR_UNSUPPORTED, "tensor-core wgrad: no kernel for CN=%d BNW=%d", CN, BNW);
-}
-
-int conv_wgrad_tc(const float* x, const float* gy, float* gw, int N, int H, int W, int Cin, int Cout, int k, int pad,
-                  int accumulate, void* ws, int64_t ws_bytes, cudaStream_t st) {
-  if (!conv_tc_supported(N, H, W, Cin, Cout, k, pad)) return fail(TWG_ERR_UNSUPPORTED, "tensor-core wgrad: shape not covered");
-  if (!ws || ws_bytes < conv_tc_workspace(N, H, W, Cin, Cout, k, pad)) return fail(TWG_ERR_INVALID, "tensor-core wgrad: workspace too small");
-  const int64_t px = (int64_t)N * H * W;
-  const int64_t cmax = Cin > Cout ? Cin : Cout;
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(ws) + 1023) & ~uintptr_t(1023));
-  uint8_t* gbase = base + align_up(px * cmax * 4, 1024);
-  int rc = split_act_planes(x, base, px * Cin, st);
-  if (rc) return rc;
-  if ((rc = split_act_planes(gy, gbase, px * Cout, st))) return rc;
-  return conv_wgrad_tc_planes(base, gbase, gw, N, H, W, Cin, Cout, k, pad, accumulate, st);
 }
 
 }  // namespace twg

@@ -1675,7 +1675,7 @@ using namespace twg;
 
 extern "C" {
 
-int twg_version(void) { return 100; }
+int twg_version(void) { return 101; }
 const char* twg_last_error(void) { return g_err; }
 int64_t twg_launch_count(void) { return g_launches.load(); }
 
@@ -1747,13 +1747,8 @@ int twg_norm_update_stats(float* state, const float* batch_stats, int kind, floa
   return check_launch("twg_norm_update_stats");
 }
 
-int twg_norm_act_fwd(const float* y, const float* a, const float* b, float* z, int N, int HW, int C, int flags,
-                     twg_stream_t stream) {
-  return twg_norm_act_fwd_planes(y, a, b, z, nullptr, N, HW, C, flags, stream);
-}
-
-int twg_norm_act_fwd_planes(const float* y, const float* a, const float* b, float* z, void* planes, int N, int HW, int C,
-                            int flags, twg_stream_t stream) {
+int twg_norm_act_fwd(const float* y, const float* a, const float* b, float* z, void* planes, int N, int HW, int C,
+                     int flags, twg_stream_t stream) {
   if (!y || !a || !b || (!z && !planes)) return fail(TWG_ERR_INVALID, "twg_norm_act_fwd: null");
   const int64_t total = (int64_t)N * HW;
   VecGeom g = vec_geom(C);
@@ -1772,18 +1767,11 @@ int twg_norm_act_fwd_planes(const float* y, const float* a, const float* b, floa
 }
 
 int twg_norm_act_bwd_reduce(const float* y, const float* a, const float* b, const float* mean, const float* rstd,
-                            const float* gz, float* gu, float* red, int N, int HW, int C, int flags,
-                            twg_stream_t stream) {
-  if (!gz) return fail(TWG_ERR_INVALID, "twg_norm_act_bwd_reduce: null");
-  return twg_norm_act_bwd_reduce_pool(y, a, b, mean, rstd, gz, nullptr, 0, gu, red, N, HW, C, flags, stream);
-}
-
-int twg_norm_act_bwd_reduce_pool(const float* y, const float* a, const float* b, const float* mean, const float* rstd,
-                                 const float* gz, const float* gpool, int W, float* gu, float* red, int N, int HW, int C,
-                                 int flags, twg_stream_t stream) {
+                            const float* gz, const float* gpool, int W, float* gu, float* red, int N, int HW, int C,
+                            int flags, twg_stream_t stream) {
   if (!y || !a || !b || !mean || !rstd || (!gz && !gpool) || !gu || !red) return fail(TWG_ERR_INVALID, "twg_norm_act_bwd_reduce: null");
   if (gpool && (W <= 0 || W % 2 || HW % W || (HW / W) % 2 || !vec_geom(C).ok))
-    return fail(TWG_ERR_UNSUPPORTED, "twg_norm_act_bwd_reduce_pool: needs even H, W and a vectorisable C");
+    return fail(TWG_ERR_UNSUPPORTED, "twg_norm_act_bwd_reduce: the pool gradient needs even H, W and a vectorisable C");
   cudaMemsetAsync(red, 0, sizeof(float) * 2 * N * C, S(stream));
   VecGeom g = vec_geom(C);
   if (g.ok) {
@@ -1802,10 +1790,10 @@ int twg_norm_act_bwd_reduce_pool(const float* y, const float* a, const float* b,
   return check_launch("twg_norm_act_bwd_reduce");
 }
 
-int twg_norm_act_bwd_apply_planes(const float* y, const float* a, const float* mean, const float* rstd, const float* gu,
-                                  const float* red, const float* rd, float* gy, void* gy_planes, float* ggamma0,
-                                  float* gbeta0, float* ggamma1, float* gbeta1, int accumulate, int dom_mask,
-                                  int group_size, int kind, int N, int HW, int C, twg_stream_t stream) {
+int twg_norm_act_bwd_apply(const float* y, const float* a, const float* mean, const float* rstd, const float* gu,
+                           const float* red, const float* rd, float* gy, void* gy_planes, float* ggamma0, float* gbeta0,
+                           float* ggamma1, float* gbeta1, int accumulate, int dom_mask, int group_size, int kind, int N,
+                           int HW, int C, twg_stream_t stream) {
   if (!y || !a || !mean || !rstd || !gu || !red || (!gy && !gy_planes)) return fail(TWG_ERR_INVALID, "twg_norm_act_bwd_apply: null");
   if (gy_planes && (C % 4)) return fail(TWG_ERR_UNSUPPORTED, "twg_norm_act_bwd_apply: split-plane output needs C % 4 == 0");
   if (group_size <= 0 || N % group_size || N / group_size > 32) return fail(TWG_ERR_INVALID, "twg_norm_act_bwd_apply: bad group size");
@@ -1840,12 +1828,8 @@ int twg_norm_act_bwd_apply_planes(const float* y, const float* a, const float* m
   return check_launch("twg_norm_act_bwd_apply");
 }
 
-int twg_bias_lrelu_fwd(const float* y, const float* bias, float* z, int64_t rows, int C, int lrelu_on, twg_stream_t stream) {
-  return twg_bias_lrelu_fwd_planes_mask(y, bias, z, nullptr, nullptr, rows, C, lrelu_on, stream);
-}
-
-int twg_bias_lrelu_fwd_planes_mask(const float* y, const float* bias, float* z, void* planes, void* mask, int64_t rows, int C,
-                                   int lrelu_on, twg_stream_t stream) {
+int twg_bias_lrelu_fwd(const float* y, const float* bias, float* z, void* planes, void* mask, int64_t rows, int C,
+                       int lrelu_on, twg_stream_t stream) {
   if (!y || !z) return fail(TWG_ERR_INVALID, "twg_bias_lrelu_fwd: null");
   if ((planes || mask) && C % 4) return fail(TWG_ERR_UNSUPPORTED, "twg_bias_lrelu_fwd: planes / mask need C % 4 == 0");
   const int64_t total = rows * C;
@@ -1876,26 +1860,13 @@ int twg_colsum(const float* g, float* out, int64_t rows, int C, int accumulate, 
   return rc ? rc : add_partials(out, parts, (int)blocks, C, S(stream));
 }
 
-int twg_lrelu_bwd_colsum(const float* g, const float* ref, float* out, float* colsum, int64_t rows, int C, int lrelu_on,
-                         int accumulate, twg_stream_t stream) {
-  return twg_lrelu_bwd_colsum_planes_pool(g, ref, out, nullptr, colsum, rows, C, lrelu_on, 0, 0, accumulate, stream);
-}
-
-int twg_lrelu_bwd_colsum_planes_pool(const float* g, const float* ref, float* out, void* planes, float* colsum,
-                                     int64_t rows, int C, int lrelu_on, int poolH, int poolW, int accumulate,
-                                     twg_stream_t stream) {
-  return twg_lrelu_bwd_colsum_planes_pool_mask(g, ref, nullptr, out, planes, colsum, rows, C, lrelu_on, poolH, poolW, accumulate,
-                                               stream);
-}
-
-int twg_lrelu_bwd_colsum_planes_pool_mask(const float* g, const float* ref, const void* mask, float* out, void* planes,
-                                          float* colsum, int64_t rows, int C, int lrelu_on, int poolH, int poolW,
-                                          int accumulate, twg_stream_t stream) {
+int twg_lrelu_bwd_colsum(const float* g, const float* ref, const void* mask, float* out, void* planes, float* colsum,
+                         int64_t rows, int C, int lrelu_on, int poolH, int poolW, int accumulate, twg_stream_t stream) {
   const uint8_t* mk = reinterpret_cast<const uint8_t*>(mask);
   if (mk && !vec_geom(C).ok) return fail(TWG_ERR_UNSUPPORTED, "twg_lrelu_bwd_colsum: the sign mask needs a vectorisable C");
   if (mk) ref = ref ? ref : reinterpret_cast<const float*>(mk);      // only tested for null below
   if (poolW > 0 && (poolH <= 0 || poolH % 2 || poolW % 2 || rows % ((int64_t)poolH * poolW) || !vec_geom(C).ok))
-    return fail(TWG_ERR_UNSUPPORTED, "twg_lrelu_bwd_colsum_planes_pool: needs even H, W and a vectorisable C");
+    return fail(TWG_ERR_UNSUPPORTED, "twg_lrelu_bwd_colsum: the pool gradient needs even H, W and a vectorisable C");
   if (!g || !colsum || (lrelu_on && (!ref || (!out && !planes)))) return fail(TWG_ERR_INVALID, "twg_lrelu_bwd_colsum: null");
   if (!accumulate) cudaMemsetAsync(colsum, 0, sizeof(float) * C, S(stream));
   VecGeom gm = vec_geom(C);
@@ -1942,12 +1913,7 @@ int twg_lrelu_bwd_colsum_planes_pool_mask(const float* g, const float* ref, cons
   return add_partials(colsum, parts, (int)blocks, C, S(stream));
 }
 
-int twg_pool2(const float* x, float* out, int N, int H, int W, int C, float scale, twg_stream_t stream) {
-  return twg_pool2_planes(x, out, nullptr, N, H, W, C, scale, stream);
-}
-
-int twg_pool2_planes(const float* x, float* out, void* planes, int N, int H, int W, int C, float scale,
-                     twg_stream_t stream) {
+int twg_pool2(const float* x, float* out, void* planes, int N, int H, int W, int C, float scale, twg_stream_t stream) {
   if (!x || (!out && !planes) || (H & 1) || (W & 1)) return fail(TWG_ERR_INVALID, "twg_pool2: bad args");
   const int64_t total = (int64_t)N * (H / 2) * (W / 2) * C;
   if (C % 4 == 0 && (int64_t)N * (H / 2) < (1ll << 31) && (int64_t)(W / 2) * (C / 4) >= 64)
@@ -1968,8 +1934,8 @@ int twg_upsample2(const float* x, float* out, int N, int H, int W, int C, float 
   return check_launch("twg_upsample2");
 }
 
-int twg_upsample_concat_planes(const float* a, const float* b, float* out, void* planes, int N, int H, int W, int Ca,
-                               int Cb, int Nb, twg_stream_t stream) {
+int twg_upsample_concat(const float* a, const float* b, float* out, void* planes, int N, int H, int W, int Ca, int Cb,
+                        int Nb, twg_stream_t stream) {
   if (!a || !b || (!out && !planes)) return fail(TWG_ERR_INVALID, "twg_upsample_concat: null");
   if (Nb <= 0 || N % Nb) return fail(TWG_ERR_INVALID, "twg_upsample_concat: skip batch %d does not divide %d", Nb, N);
   const int64_t total = (int64_t)N * H * W * 4 * (Ca + Cb);
@@ -2214,13 +2180,6 @@ int twg_split_weights_table(const float* flat, void* planes, const void* table, 
   k_split_weights_table<<<grid, 256, 0, S(stream)>>>(flat, reinterpret_cast<__nv_bfloat16*>(planes),
                                                      reinterpret_cast<const SplitRow*>(table));
   return check_launch("twg_split_weights_table");
-}
-
-int twg_zero(float* dst, int64_t n, twg_stream_t stream) {
-  if (!dst) return fail(TWG_ERR_INVALID, "twg_zero: null");
-  cudaError_t e = cudaMemsetAsync(dst, 0, sizeof(float) * n, S(stream));
-  if (e != cudaSuccess) return fail(TWG_ERR_CUDA, "twg_zero: %s", cudaGetErrorString(e));
-  return TWG_OK;
 }
 
 }  // extern "C"

@@ -29,10 +29,7 @@ NORM_NONE, NORM_INSTANCE, NORM_BATCH, NORM_RENORM = 0, 1, 2, 3
 
 # 1 = wgmma tensor-core convs where the library covers the shape, 0 = exact fp32 CUDA cores everywhere
 _PREC = 1
-_TC_MIN_HW = 0   # layers with H < _TC_MIN_HW stay on the exact-fp32 CUDA-core path (precision policy knob)
-_TC_OK = {}          # (op, shape) -> bool, remembered capability of the tensor-core path
 _SKIP_PARAM_GRADS = set()   # parameter groups whose wgrad / bias-grad is not wanted in the running backward
-_WORKSPACE = {}      # device -> uint8 tensor
 
 
 def set_precision(prec: int) -> None:
@@ -74,14 +71,6 @@ def _st():
   return torch.cuda.current_stream().cuda_stream
 
 
-def _workspace(nbytes: int, device) -> torch.Tensor:
-  ws = _WORKSPACE.get(device)
-  if ws is None or ws.numel() < nbytes:
-    ws = torch.empty(max(nbytes, 1 << 20), dtype=torch.uint8, device=device)
-    _WORKSPACE[device] = ws
-  return ws
-
-
 # ------------------------------------------------------------------------------------------------
 # convolution (bilinear => closed under differentiation)
 # ------------------------------------------------------------------------------------------------
@@ -107,7 +96,7 @@ def _trace(kind: str, t: torch.Tensor) -> None:
   ACTIVE_SET_TRACE[kind].append((TRACE_TAG, t.cpu()))
 
 
-_CONV_TIMING = None   # list of (family, flops, start event, end event) while bench.py's roofline pass runs
+_CONV_TIMING = None   # list of (family, flops, bytes, start event, end event) while bench.py's roofline pass runs
 
 
 def enable_conv_timing(on: bool) -> None:
@@ -116,93 +105,40 @@ def enable_conv_timing(on: bool) -> None:
 
 
 def collect_conv_timing():
-  """{'tc'|'simt': {'launches', 'ms', 'flops'}} -- CUDA-event time of every conv-family launch since enable."""
+  """{family: {'launches', 'ms', 'flops', 'bytes', 'tflops', 'algorithmic_gbs'}} -- CUDA-event time of every conv launch
+  since enable, by kernel family ('tc_fwd', 'tc_wgrad', 'tc_ws', 'fp32_cuda_core')."""
   out = {}
-  for fam, fl, e0, e1 in (_CONV_TIMING or []):
-    d = out.setdefault(fam, {'launches': 0, 'ms': 0.0, 'flops': 0.0})
+  for fam, fl, nb, e0, e1 in (_CONV_TIMING or []):
+    d = out.setdefault(fam, {'launches': 0, 'ms': 0.0, 'flops': 0.0, 'bytes': 0.0})
     d['launches'] += 1
     d['ms'] += e0.elapsed_time(e1)
-    d['flops'] += fl[0] if isinstance(fl, tuple) else fl
-    d['bytes'] = d.get('bytes', 0.0) + (fl[1] if isinstance(fl, tuple) else 0.0)
+    d['flops'] += fl
+    d['bytes'] += nb
   for d in out.values():
     d['ms'] = round(d['ms'], 4)
     d['tflops'] = round(d['flops'] / max(d['ms'], 1e-9) / 1e9, 3)
-    d['algorithmic_gbs'] = round(d.get('bytes', 0.0) / max(d['ms'], 1e-9) / 1e6, 1)
+    d['algorithmic_gbs'] = round(d['bytes'] / max(d['ms'], 1e-9) / 1e6, 1)
   return out
 
 
-def _conv_call(op: str, a, b, out, N, H, W, Cin, Cout, k, pad, accumulate=None):
-  if _CONV_TIMING is not None:
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    used = _conv_call_inner(op, a, b, out, N, H, W, Cin, Cout, k, pad, accumulate)
-    e1.record()
-    Ho, Wo = H + 2 * pad - k + 1, W + 2 * pad - k + 1
-    _CONV_TIMING.append(('tc_ws' if used else 'fp32_cuda_core', 2.0 * N * Ho * Wo * Cin * Cout * k * k, e0, e1))
-    return
-  _conv_call_inner(op, a, b, out, N, H, W, Cin, Cout, k, pad, accumulate)
-
-
-def _conv_call_inner(op: str, a, b, out, N, H, W, Cin, Cout, k, pad, accumulate=None):
-  L = lib()
-  key = (op, N, H, W, Cin, Cout, k, pad)
-  prec = _PREC if (_TC_OK.get(key, True) and H >= _TC_MIN_HW) else 0
-  while True:
-    nbytes = L.cdll.twg_conv_workspace_bytes(N, H, W, Cin, Cout, k, pad, prec) if prec else 0
-    ws = _workspace(nbytes, out.device) if nbytes else None
-    args = [_p(a), _p(b), _p(out), N, H, W, Cin, Cout, k, pad]
-    if accumulate is not None:
-      args.append(int(accumulate))
-    args += [prec, _p(ws), nbytes, _st()]
-    rc = L.try_call(op, *args)
-    if rc == 0:
-      return prec
-    if rc == -2 and prec == 1:
-      _TC_OK[key] = False
-      prec = 0
-      continue
-    raise TwgError('%s failed (%d): %s' % (op, rc, L.last_error()))
-
-
 def conv_fwd_raw(x, w, k, pad):
-  x, w = _check(x), _check(w)
-  N, H, W_, Cin = x.shape
-  Cout = w.shape[3]
-  y = torch.empty((N, H + 2 * pad - k + 1, W_ + 2 * pad - k + 1, Cout), device=x.device, dtype=torch.float32)
-  _conv_call('twg_conv_fwd', x, w, y, N, H, W_, Cin, Cout, k, pad)
-  return y
+  """y = conv2d(x, w) outside autograd: the tensor-core kernel where tc_eligible(), else the exact-fp32 one."""
+  return _conv_fwd(_check(x), _check(w), k, pad)[0]
 
 
 def conv_dgrad_raw(gy, w, x_shape, k, pad):
-  gy, w = _check(gy), _check(w)
-  N, H, W_, Cin = x_shape
-  Cout = w.shape[3]
-  gx = torch.empty(x_shape, device=gy.device, dtype=torch.float32)
-  _conv_call('twg_conv_dgrad', gy, w, gx, N, H, W_, Cin, Cout, k, pad)
-  return gx
+  return _conv_dgrad(_check(gy), _check(w), tuple(x_shape), k, pad)[0]
 
 
-def conv_wgrad_raw(x, gy, k, pad, out=None):
-  """`out`: accumulate (+=) into this fp32 buffer of k*k*Cin*Cout elements instead of returning a new tensor."""
-  x, gy = _check(x), _check(gy)
-  N, H, W_, Cin = x.shape
-  Cout = gy.shape[3]
-  gw = out if out is not None else torch.empty((k, k, Cin, Cout), device=x.device, dtype=torch.float32)
-  _conv_call('twg_conv_wgrad', x, gy, gw, N, H, W_, Cin, Cout, k, pad, accumulate=1 if out is not None else 0)
-  return gw
+def conv_wgrad_raw(x, gy, k, pad):
+  return _conv_wgrad(_check(x), _check(gy), k, pad)
 
 
 # ---- split-bf16 planes: split an activation ONCE (forward + wgrad), a gradient ONCE (dgrad + wgrad) and a
 # ---- registered weight once per optimiser step ----------------------------------------------------------------
 
-_TC_SHAPE = {}
 _WEIGHT_TABLES = {}      # data_ptr of a registered conv weight -> weak reference to its WeightPlaneTable
 _LIVE_TABLES = weakref.WeakSet()
-
-
-def _tc_channels_ok(c: int) -> bool:
-  """Channel counts the tensor-core kernels are built for (mirrors tc_shape_ok in csrc/twg_conv_tc.cu)."""
-  return c in (16, 32, 64) or (c >= 128 and c % 128 == 0)
 
 
 class WeightPlaneTable:
@@ -219,7 +155,7 @@ class WeightPlaneTable:
       if not name.endswith('/weights') or t.dim() != 4:
         continue
       k, _, cin, cout = (int(v) for v in t.shape)
-      if k not in (1, 3) or not _tc_channels_ok(cin) or not _tc_channels_ok(cout):
+      if conv_path(1, 1, 1, cin, cout, k, (k - 1) // 2) != CONV_TC:    # (the path does not depend on N, H, W)
         continue
       n = k * k * cin * cout
       for dgrad in (0, 1):
@@ -255,20 +191,29 @@ def invalidate_weight_cache() -> None:
     t.dirty = True
 
 
-def set_tc_min_hw(h: int) -> None:
-  global _TC_MIN_HW
-  _TC_MIN_HW = int(h)
+CONV_SIMT, CONV_PW, CONV_TC = 0, 1, 2     # kernel families of twg_conv_path
+_CONV_PATHS = {}
+
+
+def conv_path(N, H, W, Cin, Cout, k, pad) -> int:
+  """Which kernel family the library has for this conv shape: CONV_SIMT, CONV_PW (exact fp32) or CONV_TC (tensor cores)."""
+  key = (N, H, W, Cin, Cout, k, pad)
+  v = _CONV_PATHS.get(key)
+  if v is None:
+    v = _CONV_PATHS[key] = int(lib().cdll.twg_conv_path(N, H, W, Cin, Cout, k, pad))
+  return v
 
 
 def tc_eligible(N, H, W, Cin, Cout, k, pad) -> bool:
-  if _PREC != 1 or H < _TC_MIN_HW:
-    return False
-  key = (N, H, W, Cin, Cout, k, pad)
-  v = _TC_SHAPE.get(key)
-  if v is None:
-    v = bool(lib().cdll.twg_conv_tc_supported(N, H, W, Cin, Cout, k, pad))
-    _TC_SHAPE[key] = v
-  return v
+  return _PREC == 1 and conv_path(N, H, W, Cin, Cout, k, pad) == CONV_TC
+
+
+def _epilogue_slots(N, H, W, Cin, Cout, k, pad) -> int:
+  """Statistics records per image of the forward conv's fused epilogue; 0: this conv has no fused epilogue (no statistics,
+  sign mask or evaluation-mode affine)."""
+  if not tc_eligible(N, H, W, Cin, Cout, k, pad):
+    return 0
+  return int(lib().cdll.twg_conv_epilogue_slots(N, H, W, Cin, Cout, k, pad))
 
 
 def split_act(x: torch.Tensor) -> torch.Tensor:
@@ -334,59 +279,98 @@ def weight_planes(w: torch.Tensor, dgrad: bool) -> torch.Tensor:
   return planes
 
 
-def _timed(fam, flops, fn):
-  if _CONV_TIMING is None:
-    return fn()
-  e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  e0.record()
-  out = fn()
-  e1.record()
-  _CONV_TIMING.append((fam, flops, e0, e1))
-  return out
-
-
-def conv_fwd_planes(xp, wp, N, H, W, Cin, Cout, k, pad):
-  y = torch.empty((N, H, W, Cout), device=xp.device, dtype=torch.float32)
-  _timed('tc_fwd', (2.0 * N * H * W * Cin * Cout * k * k, 4.0 * N * H * W * (Cin + Cout)),
-         lambda: lib().call('twg_conv_fwd_planes', _p(xp), _p(wp), _p(y), N, H, W, Cin, Cout, k, pad, _st()))
-  return y
-
-
 EPILOGUE_STATS = True    # A/B switch: instance-norm statistics from the conv epilogue instead of a twg_moments pass
 ACT_SIGN_MASK = True     # A/B switch: discriminator conv epilogues write z's sign mask; the activation backward reads it, not z
 
 
-def conv_fwd_planes_stats(xp, wp, N, H, W, Cin, Cout, k, pad):
-  """Forward conv whose epilogue also emits the normaliser statistics of y.  Returns (y, stats, slots); stats is None
-  when the shape runs on a kernel without that epilogue."""
-  L = lib()
-  slots = L.cdll.twg_conv_stats_slots(N, H, W, Cin, Cout, k, pad) if EPILOGUE_STATS else 0
-  if slots <= 0:
-    return conv_fwd_planes(xp, wp, N, H, W, Cin, Cout, k, pad), None, 0
-  y = torch.empty((N, H, W, Cout), device=xp.device, dtype=torch.float32)
-  stats = torch.empty((N, slots, Cout, 4), device=xp.device, dtype=torch.float32)
-  _timed('tc_fwd', (2.0 * N * H * W * Cin * Cout * k * k, 4.0 * N * H * W * (Cin + Cout)),
-         lambda: L.call('twg_conv_fwd_planes_stats', _p(xp), _p(wp), _p(y), _p(stats), N, H, W, Cin, Cout, k, pad, _st()))
-  return y, stats, slots
+# ---- conv dispatch: every conv launch goes through _conv_fwd / _conv_dgrad / _conv_wgrad.  Each takes its activation
+# ---- operands as fp32 and / or split planes, runs the tensor-core kernel on planes when tc_eligible() and the exact-fp32
+# ---- kernel on fp32 otherwise, and records the launch while conv timing is on.
+
+def _nhwc(t, planes):
+  return tuple(int(d) for d in (t.shape if t is not None else planes.shape[1:]))
 
 
-def conv_dgrad_planes(gp, wp, N, H, W, Cin, Cout, k, pad):
-  gx = torch.empty((N, H, W, Cin), device=gp.device, dtype=torch.float32)
-  _timed('tc_fwd', (2.0 * N * H * W * Cin * Cout * k * k, 4.0 * N * H * W * (Cin + Cout)),
-         lambda: lib().call('twg_conv_dgrad_planes', _p(gp), _p(wp), _p(gx), N, H, W, Cin, Cout, k, pad, _st()))
-  return gx
+def _conv_launch(fam, shape, name, *args):
+  """lib().call(name, *args) for a conv of `shape` = (N, H, W, Cin, Cout, k, pad), timed under `fam` while conv timing is
+  on.  The tensor-core families also count the bytes of their fp32-sized input and output."""
+  if _CONV_TIMING is None:
+    lib().call(name, *args)
+    return
+  e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+  e0.record()
+  lib().call(name, *args)
+  e1.record()
+  N, H, W, Cin, Cout, k, pad = shape
+  Ho, Wo = H + 2 * pad - k + 1, W + 2 * pad - k + 1
+  nbytes = 4.0 * N * H * W * (Cin + Cout) if fam in ('tc_fwd', 'tc_wgrad') else 0.0
+  _CONV_TIMING.append((fam, 2.0 * N * Ho * Wo * Cin * Cout * k * k, nbytes, e0, e1))
 
 
-def conv_wgrad_planes(xp, gp, N, H, W, Cin, Cout, k, pad, out=None):
-  gw = out if out is not None else torch.empty((k, k, Cin, Cout), device=xp.device, dtype=torch.float32)
+def _exact_family(shape) -> str:
+  # bench.py reports the pointwise fromRGB / toRGB kernels apart from the SIMT ones at precision 1 only
+  return 'tc_ws' if (_PREC == 1 and conv_path(*shape) == CONV_PW) else 'fp32_cuda_core'
+
+
+def _conv_fwd(x, w, k, pad, xp=None, bias=None, act=False, zp=None, mask=None, stats=None):
+  """y = lrelu?(conv2d(x, w) + bias), x given as fp32 and / or its planes `xp` (taken from the producer or split here when
+  missing).  The epilogue outputs -- y's planes `zp`, its sign `mask`, instance-norm `stats` (N x _epilogue_slots x Cout
+  float4) -- need the tensor-core path.  Returns (y, x's planes on the tensor-core path, else None)."""
+  N, H, W_, Cin = _nhwc(x, xp)
+  Cout = int(w.shape[3])
+  shape = (N, H, W_, Cin, Cout, k, pad)
+  y = torch.empty((N, H + 2 * pad - k + 1, W_ + 2 * pad - k + 1, Cout), device=w.device, dtype=torch.float32)
+  if not tc_eligible(*shape):
+    if bias is not None or zp is not None or mask is not None or stats is not None:
+      raise TwgError('fused conv epilogues need the tensor-core path')
+    _conv_launch(_exact_family(shape), shape, 'twg_conv_fwd', _p(_check(x)), _p(_check(w)), _p(y), N, H, W_, Cin, Cout, k,
+                 pad, _st())
+    return y, None
+  xp = xp if xp is not None else planes_of(x)
+  _conv_launch('tc_fwd', shape, 'twg_conv_fwd_planes', _p(xp), _p(weight_planes(w, False)), _p(bias), int(act), _p(y),
+               _p(zp), _p(mask), _p(stats), N, H, W_, Cin, Cout, k, pad, _st())
+  return y, xp
+
+
+def _conv_dgrad(gy, w, x_shape, k, pad, gp=None):
+  """gx = conv2d_backprop_input(gy, w), gy given as fp32 and / or its planes `gp`.  Returns (gx, gy's planes on the
+  tensor-core path, else None)."""
+  N, H, W_, Cin = x_shape
+  Cout = int(w.shape[3])
+  shape = (N, H, W_, Cin, Cout, k, pad)
+  gx = torch.empty(x_shape, device=w.device, dtype=torch.float32)
+  if not tc_eligible(*shape):
+    _conv_launch(_exact_family(shape), shape, 'twg_conv_dgrad', _p(_check(gy)), _p(_check(w)), _p(gx), N, H, W_, Cin, Cout,
+                 k, pad, _st())
+    return gx, None
+  gp = gp if gp is not None else split_act(gy)
+  _conv_launch('tc_fwd', shape, 'twg_conv_dgrad_planes', _p(gp), _p(weight_planes(w, True)), _p(gx), N, H, W_, Cin, Cout, k,
+               pad, _st())
+  return gx, gp
+
+
+def _conv_wgrad(x, gy, k, pad, xp=None, gp=None, out=None):
+  """gw = conv2d_backprop_filter(x, gy), each operand given as fp32 and / or planes.  `out`: add (+=) into this fp32
+  buffer of k*k*Cin*Cout elements (a gradient sink) instead of returning a new tensor."""
+  N, H, W_, Cin = _nhwc(x, xp)
+  Cout = _nhwc(gy, gp)[3]
+  shape = (N, H, W_, Cin, Cout, k, pad)
   acc = 1 if out is not None else 0
-  _timed('tc_wgrad', (2.0 * N * H * W * Cin * Cout * k * k, 4.0 * N * H * W * (Cin + Cout)),
-         lambda: lib().call('twg_conv_wgrad_planes', _p(xp), _p(gp), _p(gw), N, H, W, Cin, Cout, k, pad, acc, _st()))
+  gw = out if out is not None else torch.empty((k, k, Cin, Cout), device=(x if x is not None else xp).device,
+                                               dtype=torch.float32)
+  if not tc_eligible(*shape):
+    _conv_launch(_exact_family(shape), shape, 'twg_conv_wgrad', _p(_check(x)), _p(_check(gy)), _p(gw), N, H, W_, Cin, Cout,
+                 k, pad, acc, _st())
+    return gw
+  xp = xp if xp is not None else split_act(x)
+  gp = gp if gp is not None else split_act(gy)
+  _conv_launch('tc_wgrad', shape, 'twg_conv_wgrad_planes', _p(xp), _p(gp), _p(gw), N, H, W_, Cin, Cout, k, pad, acc, _st())
   return gw
 
 
-# ---- gradient sinks: weight gradients accumulate straight into the flat gradient buffer (one += per use of a shared
-# ---- variable inside the wgrad kernel's own atomics) instead of autograd summing per-use tensors and a later packing
+# ---- gradient sinks: weight gradients accumulate straight into the flat gradient buffer (each use of a shared variable
+# ---- adds its gradient there with accumulate=1, after the kernel has summed its own partials in a fixed order) instead
+# ---- of autograd summing per-use tensors and a later packing
 _GRAD_SINKS = {}     # weight data_ptr -> fp32 view of the flat gradient buffer
 
 
@@ -395,15 +379,16 @@ def register_grad_sinks(mapping) -> None:
   _GRAD_SINKS.update({int(k): v for k, v in mapping.items()})
 
 
-def _wgrad_into_sink(sink, x, gy, x_planes, gy_planes, x_shape, k, pad):
-  N, H, W_, Cin = x_shape
-  Cout = int(gy.shape[3]) if gy is not None else int(gy_planes.shape[4])
-  if tc_eligible(N, H, W_, Cin, Cout, k, pad):
-    xp = x_planes if x_planes is not None else split_act(x)
-    gp = gy_planes if gy_planes is not None else split_act(gy)
-    conv_wgrad_planes(xp, gp, N, H, W_, Cin, Cout, k, pad, out=sink)
-  else:
-    conv_wgrad_raw(x, gy, k, pad, out=sink)
+def _weight_grad(ctx, w, x, gy, xp=None, gp=None):
+  """The weight gradient of the conv node `ctx` (inputs [x-like, w, ...]) from its operands: added into w's gradient sink
+  when one is registered, else returned for autograd; None when not wanted or sunk."""
+  if not (ctx.needs_input_grad[1] and ctx.group not in _SKIP_PARAM_GRADS):
+    return None
+  sink = _sink(w)
+  if sink is not None:
+    _conv_wgrad(x, gy, ctx.k, ctx.pad, xp, gp, out=sink)
+    return None
+  return ConvWgradFn.apply(x, gy, ctx.k, ctx.pad, ctx.group, xp, gp)
 
 
 class ConvFn(Function):
@@ -412,35 +397,17 @@ class ConvFn(Function):
 
   @staticmethod
   def forward(ctx, x, w, k, pad, group):
-    N, H, W_, Cin = x.shape
-    Cout = w.shape[3]
-    ctx.k, ctx.pad, ctx.group = k, pad, group
-    ctx.xshape = tuple(x.shape)
-    ctx.tc = tc_eligible(N, H, W_, Cin, Cout, k, pad)
-    if ctx.tc:
-      xp = planes_of(x)
-      ctx.save_for_backward(xp, w)
-      return conv_fwd_planes(xp, weight_planes(w, False), N, H, W_, Cin, Cout, k, pad)
-    ctx.save_for_backward(x, w)
-    return conv_fwd_raw(x, w, k, pad)
+    ctx.k, ctx.pad, ctx.group, ctx.xshape = k, pad, group, tuple(x.shape)
+    y, xp = _conv_fwd(x, w, k, pad)
+    ctx.save_for_backward(x if xp is None else None, xp, w)
+    return y
 
   @staticmethod
   def backward(ctx, gy):
-    x, w = ctx.saved_tensors      # x is the planes tensor on the tensor-core path
-    gx = gw = None
-    want_w = ctx.needs_input_grad[1] and ctx.group not in _SKIP_PARAM_GRADS
-    gp = planes_of(gy) if ctx.tc else None
-    if ctx.needs_input_grad[0]:
-      gx = ConvDgradFn.apply(gy, w, ctx.xshape, ctx.k, ctx.pad, ctx.group, gp)
-    if want_w:
-      sink = _sink(w)
-      if sink is not None:
-        _wgrad_into_sink(sink, None if ctx.tc else x, gy, x if ctx.tc else None, gp, ctx.xshape, ctx.k, ctx.pad)
-      elif ctx.tc:
-        gw = ConvWgradFn.apply(None, gy, ctx.k, ctx.pad, ctx.group, x, gp, ctx.xshape)
-      else:
-        gw = ConvWgradFn.apply(x, gy, ctx.k, ctx.pad, ctx.group, None, None, ctx.xshape)
-    return gx, gw, None, None, None
+    x, xp, w = ctx.saved_tensors     # x on the exact path, its planes on the tensor-core path
+    gp = planes_of(gy) if xp is not None else None
+    gx = ConvDgradFn.apply(gy, w, ctx.xshape, ctx.k, ctx.pad, ctx.group, gp) if ctx.needs_input_grad[0] else None
+    return gx, _weight_grad(ctx, w, x, gy, xp, gp), None, None, None
 
 
 class ConvDgradFn(Function):
@@ -448,70 +415,45 @@ class ConvDgradFn(Function):
 
   @staticmethod
   def forward(ctx, gy, w, x_shape, k, pad, group, gy_planes=None):
-    N, H, W_, Cin = x_shape
-    Cout = w.shape[3]
-    ctx.k, ctx.pad, ctx.group, ctx.xshape = k, pad, group, tuple(x_shape)
-    ctx.tc = tc_eligible(N, H, W_, Cin, Cout, k, pad)
-    if ctx.tc:
-      gp = gy_planes if gy_planes is not None else split_act(gy)
-      ctx.save_for_backward(gp, w)
-      return conv_dgrad_planes(gp, weight_planes(w, True), N, H, W_, Cin, Cout, k, pad)
-    ctx.save_for_backward(gy, w)
-    return conv_dgrad_raw(gy, w, x_shape, k, pad)
+    ctx.k, ctx.pad, ctx.group = k, pad, group
+    gx, gp = _conv_dgrad(gy, w, tuple(x_shape), k, pad, gy_planes)
+    ctx.save_for_backward(gy if gp is None else None, gp, w)
+    return gx
 
   @staticmethod
   def backward(ctx, ggx):
-    gy, w = ctx.saved_tensors     # gy is the planes tensor on the tensor-core path
-    d_gy = d_w = None
+    gy, gp, w = ctx.saved_tensors    # gy on the exact path, its planes on the tensor-core path
     ggx_planes = None
-    if ctx.tc:
+    if gp is not None:
       # ggx feeds a conv (d_gy) and a weight gradient: split it ONCE and hand the planes to both
       ggx_planes = planes_of(ggx)
       _put_planes(ggx, ggx_planes)
-    if ctx.needs_input_grad[0]:
-      d_gy = ConvFn.apply(ggx, w, ctx.k, ctx.pad, ctx.group)
+    d_gy = ConvFn.apply(ggx, w, ctx.k, ctx.pad, ctx.group) if ctx.needs_input_grad[0] else None
     _take_planes(ggx)
-    if ctx.needs_input_grad[1] and ctx.group not in _SKIP_PARAM_GRADS:
-      sink = _sink(w)
-      if sink is not None:
-        _wgrad_into_sink(sink, ggx, None if ctx.tc else gy, ggx_planes, gy if ctx.tc else None, ctx.xshape, ctx.k, ctx.pad)
-      elif ctx.tc:
-        d_w = ConvWgradFn.apply(ggx, None, ctx.k, ctx.pad, ctx.group, None, gy, ctx.xshape)
-      else:
-        d_w = ConvWgradFn.apply(ggx, gy, ctx.k, ctx.pad, ctx.group, None, None, ctx.xshape)
-    return d_gy, d_w, None, None, None, None, None
+    return d_gy, _weight_grad(ctx, w, ggx, gy, ggx_planes, gp), None, None, None, None, None
 
 
 class ConvWgradFn(Function):
-  """gw = conv2d_backprop_filter(x, gy).  Either operand may be given as fp32 (x / gy) or as split planes."""
+  """gw = conv2d_backprop_filter(x, gy).  Either operand may be given as fp32 (x / gy) and / or as split planes."""
 
   @staticmethod
-  def forward(ctx, x, gy, k, pad, group, x_planes, gy_planes, x_shape):
-    N, H, W_, Cin = x_shape
-    Cout = int(gy.shape[3]) if gy is not None else int(gy_planes.shape[4])
-    ctx.k, ctx.pad, ctx.group, ctx.xshape = k, pad, group, tuple(x_shape)
-    if tc_eligible(N, H, W_, Cin, Cout, k, pad):
-      xp = x_planes if x_planes is not None else split_act(x)
-      gp = gy_planes if gy_planes is not None else split_act(gy)
-      ctx.planes = True
-      ctx.save_for_backward(xp, gp)
-      return conv_wgrad_planes(xp, gp, N, H, W_, Cin, Cout, k, pad)
-    ctx.planes = False
+  def forward(ctx, x, gy, k, pad, group, x_planes=None, gy_planes=None):
+    ctx.k, ctx.pad, ctx.group, ctx.xshape = k, pad, group, _nhwc(x, x_planes)
     ctx.save_for_backward(x, gy)
-    return conv_wgrad_raw(x, gy, k, pad)
+    return _conv_wgrad(x, gy, k, pad, x_planes, gy_planes)
 
   @staticmethod
   def backward(ctx, ggw):
     # third-order term: never needed by the TwinGAN step (the penalty is differentiated once more, not twice)
-    if ctx.planes:
-      raise TwgError('ConvWgradFn backward on split planes is not implemented (no third-order path in the step)')
     x, gy = ctx.saved_tensors
+    if x is None or gy is None:
+      raise TwgError('ConvWgradFn backward needs fp32 operands (no third-order path in the step)')
     d_x = d_gy = None
     if ctx.needs_input_grad[0]:
       d_x = ConvDgradFn.apply(gy, ggw, ctx.xshape, ctx.k, ctx.pad, ctx.group, None)
     if ctx.needs_input_grad[1]:
       d_gy = ConvFn.apply(x, ggw, ctx.k, ctx.pad, ctx.group)
-    return d_x, d_gy, None, None, None, None, None, None
+    return d_x, d_gy, None, None, None, None, None
 
 
 class ConvBiasActFn(Function):
@@ -528,21 +470,12 @@ class ConvBiasActFn(Function):
     ctx.set_materialize_grads(False)
     ctx.k, ctx.pad, ctx.group, ctx.act = k, pad, group, act
     ctx.xshape = tuple(x.shape)
-    xp = planes_of(x)
-    z = torch.empty((N, H, W_, Cout), device=x.device, dtype=torch.float32)
-    zp = _new_planes(z.shape, x.device) if emit_planes else None
-    L = lib()
+    zp = _new_planes((N, H, W_, Cout), x.device) if emit_planes else None
     mask = None
-    if act and ACT_SIGN_MASK and L.cdll.twg_conv_has_act_mask(N, H, W_, Cin, Cout, k, pad):
+    if act and ACT_SIGN_MASK and _epilogue_slots(N, H, W_, Cin, Cout, k, pad):
       # the epilogue also writes the sign bits of z (one byte per 4 channels): all the first-order backward needs of z
-      mask = torch.empty(z.numel() // 4, device=x.device, dtype=torch.uint8)
-      _timed('tc_fwd', (2.0 * N * H * W_ * Cin * Cout * k * k, 4.0 * N * H * W_ * (Cin + Cout)),
-             lambda: L.call('twg_conv_bias_act_fwd_planes_mask', _p(xp), _p(weight_planes(w, False)), _p(_check(bias)),
-                            _p(z), _p(zp), _p(mask), N, H, W_, Cin, Cout, k, pad, _st()))
-    else:
-      _timed('tc_fwd', (2.0 * N * H * W_ * Cin * Cout * k * k, 4.0 * N * H * W_ * (Cin + Cout)),
-             lambda: L.call('twg_conv_bias_act_fwd_planes', _p(xp), _p(weight_planes(w, False)), _p(_check(bias)),
-                            int(act), _p(z), _p(zp), N, H, W_, Cin, Cout, k, pad, _st()))
+      mask = torch.empty(N * H * W_ * Cout // 4, device=x.device, dtype=torch.uint8)
+    z, xp = _conv_fwd(x, w, k, pad, bias=_check(bias), act=act, zp=zp, mask=mask)
     ctx.mask = mask
     if mask is not None:
       _MASKS[id(z)] = (weakref.ref(z), mask)
@@ -555,7 +488,7 @@ class ConvBiasActFn(Function):
       return z
     pooled = torch.empty((N, H // 2, W_ // 2, Cout), device=x.device, dtype=torch.float32)
     pp = _new_planes(pooled.shape, x.device) if pool == 'planes' else None
-    lib().call('twg_pool2_planes', _p(z), _p(pooled), _p(pp), N, H, W_, Cout, 0.25, _st())
+    lib().call('twg_pool2', _p(z), _p(pooled), _p(pp), N, H, W_, Cout, 0.25, _st())
     if pp is not None:
       _put_planes(pooled, pp)
     return z, pooled
@@ -584,7 +517,7 @@ class ConvBiasActFn(Function):
       bsink = _sink(bias) if (want_p and ctx.needs_input_grad[2]) else None
       gb = bsink if bsink is not None else torch.empty(C, device=z.device, dtype=torch.float32)
       H, W_ = int(z.shape[1]), int(z.shape[2])
-      lib().call('twg_lrelu_bwd_colsum_planes_pool_mask', _p(src), _p(z), _p(ctx.mask), None, _p(gp), _p(gb), z.numel() // C, C,
+      lib().call('twg_lrelu_bwd_colsum', _p(src), _p(z), _p(ctx.mask), None, _p(gp), _p(gb), z.numel() // C, C,
                  int(ctx.act), H if pooled_only else 0, W_ if pooled_only else 0, 1 if bsink is not None else 0, _st())
       if bsink is not None or not (want_p and ctx.needs_input_grad[2]):
         gb = None
@@ -593,16 +526,8 @@ class ConvBiasActFn(Function):
       if want_p and ctx.needs_input_grad[2]:
         gb = ColsumFn.apply(gy)
       gp = planes_of(gy)           # written by LreluBwdFn's own pass when it ran
-    gx = gw = None
-    if ctx.needs_input_grad[0]:
-      gx = ConvDgradFn.apply(gy, w, ctx.xshape, ctx.k, ctx.pad, ctx.group, gp)
-    if ctx.needs_input_grad[1] and want_p:
-      sink = _sink(w)
-      if sink is not None:
-        _wgrad_into_sink(sink, None, gy, xp, gp, ctx.xshape, ctx.k, ctx.pad)
-      else:
-        gw = ConvWgradFn.apply(None, gy, ctx.k, ctx.pad, ctx.group, xp, gp, ctx.xshape)
-    return gx, gw, gb, None, None, None, None, None, None
+    gx = ConvDgradFn.apply(gy, w, ctx.xshape, ctx.k, ctx.pad, ctx.group, gp) if ctx.needs_input_grad[0] else None
+    return gx, _weight_grad(ctx, w, None, gy, xp, gp), gb, None, None, None, None, None, None
 
 
 def vec_ok(C: int) -> bool:
@@ -619,8 +544,9 @@ def conv_bias_act(x, w, bias, pad, act=True, group='D', emit_planes=False, pool=
   k = int(w.shape[0])
   N, H, W_, Cin = x.shape
   Cout = int(w.shape[3])
-  # low-resolution wide layers run split-K (fp32 atomics), which excludes the fused epilogue; there the separate
-  # bias+activation pass is over a tiny tensor anyway
+  # Below 16384 output pixels the layer runs as conv + a separate bias / activation pass, which is then over a small
+  # tensor.  The bound dates from kernels that split K on those layers; it stays because moving it changes which kernels
+  # run, and its effect on the step time has not been measured since.
   if tc_eligible(N, H, W_, Cin, Cout, k, int(pad)) and N * H * W_ >= 16384:
     if pool is not None and vec_ok(Cout) and H % 2 == 0 and W_ % 2 == 0:
       return ConvBiasActFn.apply(x, w, bias, k, int(pad), bool(act), group, bool(emit_planes), pool)
@@ -727,7 +653,7 @@ class NormActFn(Function):
       clip = torch.tensor([float(v) for v in clip], device=y.device, dtype=torch.float32)
     buf, rd = _norm_forward(L, y, gamma, beta, None, None, kind, eps, clip, state_snapshot, None, batch_stats_out, N, 0)
     z = torch.empty_like(y)
-    L.call('twg_norm_act_fwd', _p(y), _p(buf[0]), _p(buf[1]), _p(z), N, H * W_, C, flags, _st())
+    L.call('twg_norm_act_fwd', _p(y), _p(buf[0]), _p(buf[1]), _p(z), None, N, H * W_, C, flags, _st())
     if ACTIVE_SET_TRACE is not None and (flags & FLAG_LRELU):
       _trace('lrelu', z > 0)
     ctx.save_for_backward(y, buf, rd)
@@ -745,14 +671,14 @@ class NormActFn(Function):
     a, b, mean, rstd = buf[0], buf[1], buf[2], buf[3]
     gu = torch.empty_like(y)
     red = torch.empty((N, C, 2), device=y.device, dtype=torch.float32)
-    L.call('twg_norm_act_bwd_reduce', _p(y), _p(a), _p(b), _p(mean), _p(rstd), _p(gz), _p(gu), _p(red), N, HW, C,
+    L.call('twg_norm_act_bwd_reduce', _p(y), _p(a), _p(b), _p(mean), _p(rstd), _p(gz), None, 0, _p(gu), _p(red), N, HW, C,
            ctx.flags, _st())
     want_p = ctx.group not in _SKIP_PARAM_GRADS
     ggamma = torch.empty(C, device=y.device, dtype=torch.float32) if (ctx.has_gamma and want_p) else None
     gbeta = torch.empty(C, device=y.device, dtype=torch.float32) if want_p else None
     gy = torch.empty_like(y) if ctx.kind != NORM_NONE else gu
     if ctx.kind != NORM_NONE:
-      L.call('twg_norm_act_bwd_apply_planes', _p(y), _p(a), _p(mean), _p(rstd), _p(gu), _p(red), _p(rd), _p(gy), None,
+      L.call('twg_norm_act_bwd_apply', _p(y), _p(a), _p(mean), _p(rstd), _p(gu), _p(red), _p(rd), _p(gy), None,
              _p(ggamma), _p(gbeta), None, None, 0, 0, N, ctx.kind, N, HW, C, _st())
     elif want_p:
       L.call('twg_colsum', _p(gu), _p(gbeta), N * HW, C, 0, _st())
@@ -783,17 +709,9 @@ class GenLayerFn(Function):
     L = lib()
     gs = int(group_size) if group_size else N
     ctx.set_materialize_grads(False)
-    ctx.tc = tc_eligible(N, H, W_, Cin, Cout, k, pad)
-    epi_stats, epi_slots = None, 0
-    if ctx.tc:
-      xs = planes_of(x)
-      if kind == NORM_INSTANCE:
-        y, epi_stats, epi_slots = conv_fwd_planes_stats(xs, weight_planes(w, False), N, H, W_, Cin, Cout, k, pad)
-      else:
-        y = conv_fwd_planes(xs, weight_planes(w, False), N, H, W_, Cin, Cout, k, pad)
-    else:
-      xs = _check(x)
-      y = conv_fwd_raw(xs, w, k, pad)
+    epi_slots = _epilogue_slots(N, H, W_, Cin, Cout, k, pad) if (kind == NORM_INSTANCE and EPILOGUE_STATS) else 0
+    epi_stats = torch.empty((N, epi_slots, Cout, 4), device=x.device, dtype=torch.float32) if epi_slots else None
+    y, xp = _conv_fwd(x, w, k, pad, stats=epi_stats)
     Ho, Wo = int(y.shape[1]), int(y.shape[2])
     HW = Ho * Wo
     dev = y.device
@@ -804,13 +722,13 @@ class GenLayerFn(Function):
     want_planes = emit in ('planes', 'both') and Cout % 4 == 0
     want_fp32 = (emit != 'planes') or (not want_planes) or tracing or pool is not None
     zp = _new_planes(y.shape, dev) if want_planes else None
-    L.call('twg_norm_act_fwd_planes', _p(y), _p(buf[0]), _p(buf[1]), _p(z) if want_fp32 else None, _p(zp), N, HW, Cout,
-           flags, _st())
+    L.call('twg_norm_act_fwd', _p(y), _p(buf[0]), _p(buf[1]), _p(z) if want_fp32 else None, _p(zp), N, HW, Cout, flags,
+           _st())
     if zp is not None:
       _put_planes(z, zp)
     if tracing:
       _trace('lrelu', z > 0)
-    ctx.save_for_backward(xs, w, y, buf, rd, gamma0, beta0, gamma1, beta1)
+    ctx.save_for_backward(x if xp is None else None, xp, w, y, buf, rd, gamma0, beta0, gamma1, beta1)
     ctx.k, ctx.pad, ctx.kind, ctx.flags, ctx.group = k, pad, kind, flags, group
     ctx.gs, ctx.dom_mask = gs, int(dom_mask)
     ctx.xshape = (N, H, W_, Cin)
@@ -819,14 +737,15 @@ class GenLayerFn(Function):
       return z
     pooled = torch.empty((N, Ho // 2, Wo // 2, Cout), device=dev, dtype=torch.float32)
     pp = _new_planes(pooled.shape, dev) if pool == 'planes' else None
-    L.call('twg_pool2_planes', _p(z), _p(pooled), _p(pp), N, Ho, Wo, Cout, 0.25, _st())
+    L.call('twg_pool2', _p(z), _p(pooled), _p(pp), N, Ho, Wo, Cout, 0.25, _st())
     if pp is not None:
       _put_planes(pooled, pp)
     return z, pooled
 
   @staticmethod
   def backward(ctx, gz, gpool=None):
-    xs, w, y, buf, rd, gamma0, beta0, gamma1, beta1 = ctx.saved_tensors
+    # x on the exact path, its planes on the tensor-core path
+    x, xp, w, y, buf, rd, gamma0, beta0, gamma1, beta1 = ctx.saved_tensors
     gz = _check(gz) if gz is not None else None
     gpool = _check(gpool) if gpool is not None else None
     N, Ho, Wo, C = y.shape
@@ -834,44 +753,29 @@ class GenLayerFn(Function):
       return (None,) * 20
     HW = Ho * Wo
     L = lib()
-    k, pad = ctx.k, ctx.pad
-    _, H, W_, Cin = ctx.xshape
     a, b, mean, rstd = buf[0], buf[1], buf[2], buf[3]
     gu = torch.empty_like(y)
     red = torch.empty((N, C, 2), device=y.device, dtype=torch.float32)
-    L.call('twg_norm_act_bwd_reduce_pool', _p(y), _p(a), _p(b), _p(mean), _p(rstd), _p(gz), _p(gpool), Wo, _p(gu), _p(red),
+    L.call('twg_norm_act_bwd_reduce', _p(y), _p(a), _p(b), _p(mean), _p(rstd), _p(gz), _p(gpool), Wo, _p(gu), _p(red),
            N, HW, C, ctx.flags, _st())
     want_p = ctx.group not in _SKIP_PARAM_GRADS
     ptrs, acc, ret = _norm_param_grads(C, y.device, want_p, gamma0, beta0, gamma1, beta1)
     gy = gp = None
     if ctx.kind != NORM_NONE:
-      if ctx.tc:
+      if xp is not None:
         gp = _new_planes(y.shape, y.device)        # gy exists only as the split planes dgrad/wgrad consume
       else:
         gy = torch.empty_like(y)
-      L.call('twg_norm_act_bwd_apply_planes', _p(y), _p(a), _p(mean), _p(rstd), _p(gu), _p(red), _p(rd), _p(gy), _p(gp),
+      L.call('twg_norm_act_bwd_apply', _p(y), _p(a), _p(mean), _p(rstd), _p(gu), _p(red), _p(rd), _p(gy), _p(gp),
              ptrs[0], ptrs[1], ptrs[2], ptrs[3], acc, ctx.dom_mask, ctx.gs, ctx.kind, N, HW, C, _st())
     else:
       gy = gu
       if want_p:
         L.call('twg_colsum', _p(gu), ptrs[1], N * HW, C, acc, _st())
-      if ctx.tc:
+      if xp is not None:
         gp = split_act(gu)
-    gx = gw = None
-    want_w = ctx.needs_input_grad[1] and want_p
-    sink = _sink(w) if want_w else None
-    if ctx.tc:
-      if ctx.needs_input_grad[0]:
-        gx = conv_dgrad_planes(gp, weight_planes(w, True), N, H, W_, Cin, C, k, pad)
-      if want_w:
-        gw = conv_wgrad_planes(xs, gp, N, H, W_, Cin, C, k, pad, out=sink)
-    else:
-      if ctx.needs_input_grad[0]:
-        gx = conv_dgrad_raw(gy, w, ctx.xshape, k, pad)
-      if want_w:
-        gw = conv_wgrad_raw(xs, gy, k, pad, out=sink)
-    if sink is not None:
-      gw = None
+    gx = _conv_dgrad(gy, w, ctx.xshape, ctx.k, ctx.pad, gp)[0] if ctx.needs_input_grad[0] else None
+    gw = _weight_grad(ctx, w, x, gy, xp, gp)
     return (gx, gw, ret[0], ret[1], ret[2], ret[3]) + (None,) * 14
 
 
@@ -889,7 +793,7 @@ def norm_act_eval(y, gamma, beta, kind, flags, eps, moving_mean=None, moving_var
     buf, _ = _norm_forward(L, y, gamma, beta, None, None, kind, eps, None, None, None, None, N, 0)
   z = torch.empty_like(y)
   zp = _new_planes(y.shape, y.device) if (emit == 'planes' and vec_ok(C)) else None
-  L.call('twg_norm_act_fwd_planes', _p(y), _p(buf[0]), _p(buf[1]), _p(z), _p(zp), N, H * W_, C, flags, _st())
+  L.call('twg_norm_act_fwd', _p(y), _p(buf[0]), _p(buf[1]), _p(z), _p(zp), N, H * W_, C, flags, _st())
   if zp is not None:
     _put_planes(z, zp)
   return z
@@ -897,8 +801,7 @@ def norm_act_eval(y, gamma, beta, kind, flags, eps, moving_mean=None, moving_var
 
 def affine_epilogue_ok(N, H, W, Cin, Cout, k, pad) -> bool:
   """Whether conv_affine_act_eval covers this shape (one output-channel block: all Cout channels of a pixel are in one CTA)."""
-  return bool(_PREC == 1 and tc_eligible(N, H, W, Cin, Cout, k, pad) and
-              lib().cdll.twg_conv_has_act_mask(N, H, W, Cin, Cout, k, pad))
+  return _epilogue_slots(N, H, W, Cin, Cout, k, pad) > 0
 
 
 def conv_affine_act_eval(x, w, gamma, beta, moving_mean, moving_var, flags, eps, emit='fp32'):
@@ -915,9 +818,8 @@ def conv_affine_act_eval(x, w, gamma, beta, moving_mean, moving_var, flags, eps,
   z = torch.empty((N, H, W_, Cout), device=x.device, dtype=torch.float32)
   planes_only = emit == 'planes'
   zp = _new_planes(z.shape, x.device) if emit in ('planes', 'both') else None
-  _timed('tc_fwd', (2.0 * N * H * W_ * Cin * Cout * 9, 4.0 * N * H * W_ * (Cin + Cout)),
-         lambda: L.call('twg_conv_affine_act_fwd_planes', _p(xp), _p(weight_planes(w, False)), _p(ab[0]), _p(ab[1]), int(flags),
-                        None if planes_only else _p(z), _p(zp), N, H, W_, Cin, Cout, 3, 1, _st()))
+  _conv_launch('tc_fwd', (N, H, W_, Cin, Cout, 3, 1), 'twg_conv_affine_act_fwd_planes', _p(xp), _p(weight_planes(w, False)),
+               _p(ab[0]), _p(ab[1]), int(flags), None if planes_only else _p(z), _p(zp), N, H, W_, Cin, Cout, 3, 1, _st())
   if zp is not None:
     _put_planes(z, zp)
   return z
@@ -944,8 +846,8 @@ def _dummy_colsum(device, C):
 
 class LreluBwdFn(Function):
   """out = g * slope(ref) -- the gradient of tf.maximum(0.2x, x); linear in g.  `emit_planes`: the caller consumes the
-  result as split-bf16 planes right away (ConvBiasActFn's differentiable backward), so the same pass writes them too
-  (side table, see planes_of) instead of a later split pass.  (Emitting them unconditionally was measured slower: the
+  result as split-bf16 planes right away (the differentiable backward of ConvBiasActFn, a tensor-core layer), so the same
+  pass writes them too (side table, see planes_of) instead of a later split pass.  (Emitting them unconditionally was measured slower: the
   other consumers receive the tensor through the autograd engine, where the side table cannot follow it.)"""
 
   @staticmethod
@@ -960,13 +862,13 @@ class LreluBwdFn(Function):
     if not (C and vec_ok(C)):
       mask = None
     ctx.mask = mask
-    if emit_planes and _PREC == 1 and C and _tc_channels_ok(C) and g.numel() >= (1 << 16):
+    if emit_planes and C and g.numel() >= (1 << 16):
       planes = _new_planes(g.shape, g.device)
-      lib().call('twg_lrelu_bwd_colsum_planes_pool_mask', _p(g), _p(ref), _p(mask), _p(out), _p(planes),
+      lib().call('twg_lrelu_bwd_colsum', _p(g), _p(ref), _p(mask), _p(out), _p(planes),
                  _p(_dummy_colsum(g.device, C)), g.numel() // C, C, 1, 0, 0, 1, _st())
       _put_planes(out, planes)
     elif mask is not None:
-      lib().call('twg_lrelu_bwd_colsum_planes_pool_mask', _p(g), _p(ref), _p(mask), _p(out), None,
+      lib().call('twg_lrelu_bwd_colsum', _p(g), _p(ref), _p(mask), _p(out), None,
                  _p(_dummy_colsum(g.device, C)), g.numel() // C, C, 1, 0, 0, 1, _st())
     else:
       lib().call('twg_lrelu_bwd', _p(g), _p(ref), _p(out), g.numel(), _st())
@@ -993,7 +895,8 @@ class ColsumFn(Function):
 
 
 class BiasActFn(Function):
-  """z = lrelu?(y + bias)  (pggan_discriminator_arg_scope: bias because no normalizer)."""
+  """z = lrelu?(y + bias)  (pggan_discriminator_arg_scope: bias because no normalizer).  `emit_planes`: z also feeds a
+  tensor-core conv (the caller has checked tc_eligible for it), so the same pass writes its split planes."""
 
   @staticmethod
   def forward(ctx, y, bias, act, group, emit_planes=False):
@@ -1001,9 +904,9 @@ class BiasActFn(Function):
     C = y.shape[-1]
     z = torch.empty_like(y)
     vec = y.dim() == 4 and vec_ok(C) and y.numel() >= (1 << 16)
-    planes = _new_planes(y.shape, y.device) if (emit_planes and vec and _PREC == 1 and _tc_channels_ok(C)) else None
+    planes = _new_planes(y.shape, y.device) if (emit_planes and vec) else None
     mask = torch.empty(y.numel() // 4, device=y.device, dtype=torch.uint8) if (act and vec and ACT_SIGN_MASK) else None
-    lib().call('twg_bias_lrelu_fwd_planes_mask', _p(y), _p(bias), _p(z), _p(planes), _p(mask), y.numel() // C, C, int(act), _st())
+    lib().call('twg_bias_lrelu_fwd', _p(y), _p(bias), _p(z), _p(planes), _p(mask), y.numel() // C, C, int(act), _st())
     if planes is not None:
       _put_planes(z, planes)
     if ACTIVE_SET_TRACE is not None and act:
@@ -1023,7 +926,7 @@ class BiasActFn(Function):
       gy = torch.empty_like(gz) if ctx.act else gz
       bsink = _sink(bias)
       gb = bsink if bsink is not None else torch.empty(C, device=gz.device, dtype=torch.float32)
-      lib().call('twg_lrelu_bwd_colsum_planes_pool_mask', _p(gz), _p(z), _p(ctx.mask), _p(gy) if ctx.act else None, None, _p(gb),
+      lib().call('twg_lrelu_bwd_colsum', _p(gz), _p(z), _p(ctx.mask), _p(gy) if ctx.act else None, None, _p(gb),
                  gz.numel() // C, C, int(ctx.act), 0, 0, 1 if bsink is not None else 0, _st())
       return gy, (None if bsink is not None else gb), None, None, None
     gy = LreluBwdFn.apply(gz, z, False, ctx.mask) if ctx.act else gz
@@ -1047,7 +950,7 @@ class Pool2Fn(Function):
     ctx.scale = scale
     out = torch.empty((N, H // 2, W_ // 2, C), device=x.device, dtype=torch.float32)
     planes = _new_planes(out.shape, x.device) if (emit_planes and C % 4 == 0) else None
-    lib().call('twg_pool2_planes', _p(x), _p(out), _p(planes), N, H, W_, C, float(scale), _st())
+    lib().call('twg_pool2', _p(x), _p(out), _p(planes), N, H, W_, C, float(scale), _st())
     if planes is not None:
       _put_planes(out, planes)
     return out
@@ -1097,10 +1000,10 @@ class UpsampleConcatFn(Function):
     if planes_only and Ca % 4 == 0 and Cb % 4 == 0:
       # the joined tensor only feeds the block's first (tensor-core) conv: write it as split planes, never as fp32
       planes = _new_planes(out.shape, a.device)
-      lib().call('twg_upsample_concat_planes', _p(a), _p(b), None, _p(planes), N, H, W_, Ca, Cb, Nb, _st())
+      lib().call('twg_upsample_concat', _p(a), _p(b), None, _p(planes), N, H, W_, Ca, Cb, Nb, _st())
       _put_planes(out, planes)
     else:
-      lib().call('twg_upsample_concat_planes', _p(a), _p(b), _p(out), None, N, H, W_, Ca, Cb, Nb, _st())
+      lib().call('twg_upsample_concat', _p(a), _p(b), _p(out), None, N, H, W_, Ca, Cb, Nb, _st())
     ctx.dims = (N, H, W_, Ca, Cb, Nb)
     return out
 
