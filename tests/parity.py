@@ -27,6 +27,41 @@ def rel_err(a: torch.Tensor, b: torch.Tensor) -> float:
   return (a - b).abs().max().item() / denom
 
 
+def conv_error_ratio(dev: torch.Tensor, ref: torch.Tensor, S: torch.Tensor, c, tiny: float = 1e-30) -> float:
+  """max over elements of |dev - ref| / (c * S + tiny): the check |dev - ref| <= c * S + tiny holds iff this is <= 1.
+
+  S is the operation applied to the operands' absolute values (conv(|x|, |w|) for a forward), i.e. the sum of |products|
+  each output element adds up.  Rounding errors of a sum are bounded relative to S, not to the output itself or to the
+  largest output, so this holds every element to its own condition: border pixels, taps that read only padding (S = 0
+  demands an exact 0) and small weight-gradient entries.  `c`: a number or a per-element tensor (tc_elem_c,
+  exact_elem_c).  Compared in fp64 on `ref`'s device."""
+  ref = ref.detach().double()
+  dev = dev.detach().to(ref.device, torch.float64)
+  S = S.detach().to(ref.device, torch.float64)
+  if torch.is_tensor(c):
+    c = c.detach().to(ref.device, torch.float64)
+  return float(((dev - ref).abs() / (c * S + tiny)).max())
+
+
+# Per-element bound c of conv_error_ratio on the tensor-core path, for an output that adds K >= 256 products.  Split-bf16
+# operands (a = hi + lo, three MMAs per product) leave each product off by at most 3 * 2^-16 ~ 4.6e-5 relative, typically
+# ~2^-18 and of either sign, so a long sum stays within ~5e-6 of S; a kernel that drops a cross term is off by > 1e-4 of S.
+TC_ELEM_C = 2e-5
+
+
+def tc_elem_c(K: torch.Tensor) -> torch.Tensor:
+  """Per-element c of the tensor-core path for outputs that each add K products (K = the operation on all-ones operands).
+  A short sum averages its products' rounding less: c grows like 1/sqrt(K) below K = 256, to 16 * TC_ELEM_C = 3.2e-4 at
+  K = 1, 7x the worst split-bf16 error of a single product."""
+  return TC_ELEM_C * torch.sqrt(256.0 / K.clamp(min=1.0)).clamp(min=1.0)
+
+
+def exact_elem_c(K) -> torch.Tensor:
+  """Per-element c of an exact-fp32 conv for outputs that each add K products: 4x the 2 u of rounding the fp64 operands to
+  fp32, and 4x the sqrt(K) u statistical growth of K rounded additions, u = 2^-24."""
+  return (8.0 + 4.0 * torch.as_tensor(K, dtype=torch.float64).sqrt()) * 2.0 ** -24
+
+
 def _log_result(rec):
   try:
     import json

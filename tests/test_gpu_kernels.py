@@ -6,7 +6,7 @@ import math
 import pytest
 import torch
 
-from tests.parity import rel_err, REL_TOL
+from tests.parity import rel_err, REL_TOL, conv_error_ratio, exact_elem_c, tc_elem_c, _log_result
 
 pytestmark = pytest.mark.gpu
 
@@ -45,28 +45,109 @@ CONV_SHAPES = [
     (2, 24, 40, 64, 16, 3, 1),    # row-shift weight gradient, two M groups (64-channel chunk)
     (2, 20, 36, 64, 32, 3, 1),
 ]
+# tensor-core geometries the network runs and the shapes above do not reach (tests/test_cpu_conv_error_model.py
+# calibrates the per-element bound on these)
+TC_EDGE_SHAPES = [
+    # the discriminator's 4x4 VALID head as ops.conv2d runs it: a 1x1 tensor-core conv over the flattened 4x4x256 input
+    # (one 128-image tile of 1x1 pixels, 64 K chunks); 130 images = two batch tiles, the last one ragged
+    (5, 1, 1, 4096, 256, 1, 0),
+    (130, 1, 1, 4096, 256, 1, 0),
+    (6, 4, 4, 384, 256, 3, 1),    # the minibatch-stddev conv as run: 257 input channels zero-padded to 384 (tc_channel_pad)
+    (2, 16, 16, 16, 128, 3, 1),   # forward kernels <16, 128> and <32, 128>, and the dgrads that select them
+    (2, 16, 16, 128, 16, 3, 1),
+    (2, 12, 20, 32, 128, 3, 1),
+    (2, 12, 20, 128, 32, 3, 1),
+    (2, 8, 8, 128, 256, 1, 0),    # 1x1 tensor-core conv over an image
+    (9, 3, 5, 64, 64, 3, 1),      # several images per tile (TN > 1), ragged batch, odd image
+    (3, 2, 2, 128, 128, 3, 1),    # 2x2 images: only some taps of each pixel are inside
+    (5, 1, 1, 64, 64, 3, 1),      # 1x1 images: only the centre tap is inside
+]
+CONV_SHAPES += TC_EDGE_SHAPES
+# every other conv geometry of the training step and of inference at 4x4 .. 256x256 (fromRGB / toRGB, 3x3 layers, 1x1
+# residual shortcuts; test_gpu_conv_conformance.py checks that this list and the rest of the suite cover them all)
+STEP_SHAPES = [
+    (2, 4, 4, 3, 256, 1, 0), (2, 4, 4, 256, 3, 1, 0), (2, 4, 4, 256, 256, 3, 1), (2, 8, 8, 3, 256, 1, 0),
+    (2, 8, 8, 256, 3, 1, 0), (2, 8, 8, 256, 256, 3, 1), (2, 8, 8, 512, 256, 1, 0), (2, 8, 8, 512, 256, 3, 1),
+    (2, 16, 16, 3, 256, 1, 0), (2, 16, 16, 256, 3, 1, 0), (2, 16, 16, 256, 256, 3, 1), (2, 16, 16, 512, 256, 1, 0),
+    (2, 32, 32, 3, 128, 1, 0), (2, 32, 32, 128, 3, 1, 0), (2, 32, 32, 128, 256, 1, 0), (2, 32, 32, 128, 256, 3, 1),
+    (2, 32, 32, 512, 128, 1, 0), (2, 32, 32, 512, 128, 3, 1), (2, 64, 64, 3, 64, 1, 0), (2, 64, 64, 64, 3, 1, 0),
+    (2, 64, 64, 64, 128, 1, 0), (2, 64, 64, 64, 128, 3, 1), (2, 64, 64, 256, 64, 1, 0), (2, 64, 64, 256, 64, 3, 1),
+    (1, 128, 128, 3, 32, 1, 0), (1, 128, 128, 32, 3, 1, 0), (1, 128, 128, 32, 32, 3, 1), (1, 128, 128, 32, 64, 1, 0),
+    (1, 128, 128, 32, 64, 3, 1), (1, 128, 128, 128, 32, 1, 0), (1, 128, 128, 128, 32, 3, 1), (1, 256, 256, 3, 16, 1, 0),
+    (1, 256, 256, 16, 3, 1, 0), (1, 256, 256, 16, 16, 3, 1), (1, 256, 256, 16, 32, 1, 0), (1, 256, 256, 16, 32, 3, 1),
+    (1, 256, 256, 64, 16, 1, 0), (1, 256, 256, 64, 16, 3, 1),
+]
+CONV_SHAPES += STEP_SHAPES
+
+_CPU_REF_MACS = 2e8     # fp64 references above this many multiply-adds run on the GPU (F.conv2d), below it on the CPU
+
+
+def conv_refs(x, w, gy, k, pad, device):
+  """fp64 references of the three directions on `device`, the same operations on absolute values (the S of
+  parity.conv_error_ratio) and on all-ones operands (the number of products each output element adds):
+  (y, gx, gw), (S_y, S_gx, S_gw), (K_y, K_gx, K_gw)."""
+  pad_s = 'SAME' if pad else 'VALID'
+  out = []
+  for a, b, g in ((x, w, gy), (x.abs(), w.abs(), gy.abs()), (torch.ones_like(x), torch.ones_like(w), torch.ones_like(gy))):
+    a = a.detach().to(device).requires_grad_(True)
+    b = b.detach().to(device).requires_grad_(True)
+    y = O.conv2d_nhwc(a, b, pad_s)
+    ga, gb = torch.autograd.grad(y, (a, b), g.to(device))
+    out.append((y.detach(), ga, gb))
+  return out
 
 
 @pytest.mark.parametrize('prec', [0, 1])
 @pytest.mark.parametrize('shape', CONV_SHAPES)
 def test_conv_fwd_dgrad_wgrad(built_lib, shape, prec):
+  """Each direction against fp64, on the whole tensor (rel_err) and per element: |dev - ref| <= c * S with S the same
+  operation on absolute values (parity.conv_error_ratio).  Also the weight gradient's accumulate mode."""
   from twingan_b200 import ops
   ops.set_precision(prec)
+  try:
+    N, H, W, Cin, Cout, k, pad = shape
+    Ho, Wo = H + 2 * pad - k + 1, W + 2 * pad - k + 1
+    x = _rand((N, H, W, Cin), 1)
+    w = _rand((k, k, Cin, Cout), 2, 0.05)
+    gy = _rand((N, Ho, Wo, Cout), 3)
+    macs = N * Ho * Wo * Cin * Cout * k * k
+    refs, sums, counts = conv_refs(x, w, gy, k, pad, 'cpu' if macs < _CPU_REF_MACS else 'cuda:0')
+    yd = ops.conv_fwd_raw(_dev(x), _dev(w), k, pad)
+    gxd = ops.conv_dgrad_raw(_dev(gy), _dev(w), (N, H, W, Cin), k, pad)
+    gwd = ops.conv_wgrad_raw(_dev(x), _dev(gy), k, pad)
+    torch.cuda.synchronize()
+    tol = 2e-5 if prec == 0 else 1e-4   # << 1e-3 north_star tolerance
+    for got, ref in zip((yd, gxd, gwd), refs):
+      assert rel_err(got, ref) < tol
+    tc = ops.tc_eligible(*shape)
+    rec = {'test': 'conv_elem', 'shape': list(shape), 'prec': prec, 'family': 'tc' if tc else 'exact'}
+    for d, got, ref, S, K in zip(('fwd', 'dgrad', 'wgrad'), (yd, gxd, gwd), refs, sums, counts):
+      c = tc_elem_c(K) if tc else exact_elem_c(K)
+      r = conv_error_ratio(got, ref, S, c)
+      # the worst |err| / S over the elements with the family's plain constant (K >= 128), for the record
+      rec[d] = {'ratio_to_bound': r, 'max_err_over_S': conv_error_ratio(got, ref, S, 1.0)}
+    _log_result(rec)
+    for d in ('fwd', 'dgrad', 'wgrad'):
+      assert rec[d]['ratio_to_bound'] <= 1.0, rec
+    # accumulate = 1: the weight gradient is added to what the buffer holds
+    buf = _dev(_rand((k, k, Cin, Cout), 4))
+    before = buf.clone()
+    out = ops._conv_wgrad(_dev(x), _dev(gy), k, pad, out=buf)
+    torch.cuda.synchronize()
+    assert out is buf
+    assert torch.equal(buf, before + gwd)
+  finally:
+    ops.set_precision(1)
+
+
+def test_conv_reference_on_the_gpu_matches_the_cpu_oracle(built_lib):
+  """The large cases above take their fp64 reference from F.conv2d on the GPU: it agrees with the CPU oracle."""
+  shape = (3, 8, 8, 64, 32, 3, 1)
   N, H, W, Cin, Cout, k, pad = shape
-  x = _rand((N, H, W, Cin), 1).requires_grad_(True)
-  w = _rand((k, k, Cin, Cout), 2, 0.05).requires_grad_(True)
-  y = O.conv2d_nhwc(x, w, 'SAME' if pad else 'VALID')
-  gy = _rand(tuple(y.shape), 3)
-  gx, gw = torch.autograd.grad(y, (x, w), gy)
-  yd = ops.conv_fwd_raw(_dev(x), _dev(w), k, pad)
-  gxd = ops.conv_dgrad_raw(_dev(gy), _dev(w), (N, H, W, Cin), k, pad)
-  gwd = ops.conv_wgrad_raw(_dev(x), _dev(gy), k, pad)
-  torch.cuda.synchronize()
-  tol = 2e-5 if prec == 0 else 1e-4   # << 1e-3 north_star tolerance
-  assert rel_err(yd, y) < tol
-  assert rel_err(gxd, gx) < tol
-  assert rel_err(gwd, gw) < tol
-  ops.set_precision(1)
+  x, w, gy = _rand((N, H, W, Cin), 1), _rand((k, k, Cin, Cout), 2, 0.05), _rand((N, H, W, Cout), 3)
+  cpu, gpu = conv_refs(x, w, gy, k, pad, 'cpu'), conv_refs(x, w, gy, k, pad, 'cuda:0')
+  for a, b, s in zip(gpu[0], cpu[0], cpu[1]):
+    assert conv_error_ratio(a, b.to('cuda:0'), s, 1e-13) <= 1.0
 
 
 @pytest.mark.parametrize('kind', ['instance_norm', 'batch_norm', 'batch_renorm', 'none'])
@@ -701,7 +782,9 @@ def test_discriminator_layer_sign_mask_backward_is_bit_identical(built_lib, shap
 
 
 @pytest.mark.parametrize('flags_pix', [True, False])
-@pytest.mark.parametrize('shape', [(3, 64, 64, 16, 16), (2, 24, 40, 16, 32), (2, 32, 32, 64, 32), (2, 128, 128, 32, 32)])
+@pytest.mark.parametrize('shape', [(3, 64, 64, 16, 16), (2, 24, 40, 16, 32), (2, 32, 32, 64, 32), (2, 128, 128, 32, 32),
+                                   # the other fused instantiations <Cin chunk, Cout>: <16, 64>, <32, 16>, <32, 64>, <64, 16>
+                                   (2, 16, 32, 16, 64), (2, 32, 16, 32, 16), (2, 16, 16, 32, 64), (2, 16, 16, 64, 16)])
 def test_inference_layer_in_one_kernel(built_lib, shape, flags_pix):
   """twg_conv_affine_act_fwd_planes: conv -> evaluation-mode normaliser (moving statistics = per-channel affine,
   libs/batch_norm.py:266-278) -> leaky-ReLU -> pixel norm in the conv epilogue, against the fp64 oracle primitives and
