@@ -2,6 +2,7 @@
 compare.  Used by tests/test_gpu_*.py and __graft_entry__.smoke().  The oracle is the checker only."""
 from __future__ import annotations
 
+import math
 import os
 import sys
 
@@ -60,6 +61,48 @@ def exact_elem_c(K) -> torch.Tensor:
   """Per-element c of an exact-fp32 conv for outputs that each add K products: 4x the 2 u of rounding the fp64 operands to
   fp32, and 4x the sqrt(K) u statistical growth of K rounded additions, u = 2^-24."""
   return (8.0 + 4.0 * torch.as_tensor(K, dtype=torch.float64).sqrt()) * 2.0 ** -24
+
+
+U32 = 2.0 ** -24   # unit roundoff of fp32
+
+
+def serial_run(L, C) -> float:
+  """Terms one thread of the normaliser's statistics / reduce kernels adds serially in a sum of L terms over C channels:
+  256 threads per block, G = min(C / 4, 32) of them share a pixel (vec_geom), one thread per pixel on the scalar route
+  (C % 4 != 0)."""
+  G = min(C // 4, 32) if C % 4 == 0 else 1
+  return max(1.0, L * G / 256.0)
+
+
+def norm_sum_c(R, samples=1) -> float:
+  """c of conv_error_ratio for an fp32 reduction whose threads each add R terms serially (serial_run), followed by a tree,
+  and for the batch kinds by a serial sum of the `samples` per-sample sums of a group.  A serial run of same-sign terms is
+  off by ~sqrt(R) u / 2 of its S at worst over the channels (the emulation in tests/test_cpu_norm_error_model.py);
+  c = (16 + 2 sqrt(R) + 2 sqrt(samples)) u keeps that 4x inside at every audited geometry, while a pixel left out of a
+  sum of 65536 terms (~1/65536 of S, more in the channel where that pixel is large) exceeds it 4x."""
+  return (16.0 + 2.0 * math.sqrt(R) + 2.0 * math.sqrt(samples)) * U32
+
+
+def mean_bound(R, abs_dev_mean, mean, samples=1):
+  """Per-element bound on |mean_dev - mean_ref| for a mean taken from shifted sums with serial runs of R terms: the sum's
+  bound on E|y - pivot| (`abs_dev_mean`), plus 4x the final rounding of pivot + E[y - pivot] (<= u |mean|)."""
+  return norm_sum_c(R, samples) * abs_dev_mean + 4.0 * U32 * abs(mean)
+
+
+def rstd_rel_bound(R, kappa, var, eps, samples=1):
+  """Per-element bound on |rstd_dev - rstd_ref| / rstd_ref, rstd = 1 / sqrt(var + eps), var from shifted sums with serial
+  runs of R terms (over `samples` samples).  The variance E[(y - p)^2] - E[y - p]^2 loses accuracy with the condition
+  kappa = 1 + (mean - p)^2 / var of the pivot p: relative error <= 3 (norm_sum_c + u) kappa; rsqrt halves it and adds
+  its own few ulp.  The single-pass unshifted form (p = 0) has kappa = 1 + mean^2 / var, 4e4 at mean 10, std 0.05, and
+  breaks this bound; a pivot drawn from the data keeps kappa = O(1)."""
+  return 1.5 * (norm_sum_c(R, samples) + U32) * kappa * var / (var + eps) + 4.0 * U32
+
+
+def ema_c(pushes) -> float:
+  """c of the EMA state after `pushes` pushes of k_norm_update_stats, relative to the running magnitudes of the state and
+  the pushed statistics: each push rounds a handful of fp32 operations (renorm: a quotient and its square, ~8 u), and the
+  errors add over the pushes; 16 u per push."""
+  return 16.0 * U32 * pushes
 
 
 def _log_result(rec):

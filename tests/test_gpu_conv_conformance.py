@@ -10,6 +10,7 @@ import pytest
 import torch
 
 from tests.parity import _log_result, conv_error_ratio, tc_elem_c
+from tests.product_launches import harvest_product_launches
 from tests.test_gpu_kernels import CONV_SHAPES, conv_refs, _dev, _rand
 
 pytestmark = pytest.mark.gpu
@@ -296,40 +297,9 @@ def suite_keys():
   return keys
 
 
-def harvest_product_convs(monkeypatch):
-  """Every conv launch of one eager training step per image size (4..256, 16 pairs; growing at alpha 0.5 from 8 up; instance
-  norm, batch renorm, residual blocks) and of inference on 64 images."""
-  from twingan_b200 import ops, twingan
-  from twingan_b200._lib import lib
-  L = lib()
-  seen = set()
-  call = L.call
-
-  def spy(name, *args):
-    if name in _GEOM_AT:
-      seen.add(conv_key(name, args))
-    return call(name, *args)
-
-  monkeypatch.setattr(L, 'call', spy)
-  gen = torch.Generator(device=DEV).manual_seed(0)
-  ops.set_precision(1)
-  for hw in (4, 8, 16, 32, 64, 128, 256):
-    for growing in ((False, True) if hw >= 8 else (False,)):
-      for norm, res in (('instance_norm', False), ('batch_renorm', False), ('instance_norm', True)):
-        flags = twingan.Flags(train_image_size=hw, is_growing=growing, alpha_grow=0.5 if growing else 0.0,
-                              generator_norm_type=norm, use_res_block=res)
-        model = twingan.GanModel(flags, device=DEV)
-        s = torch.rand((16, hw, hw, 3), device=DEV, generator=gen)
-        t = torch.rand((16, hw, hw, 3), device=DEV, generator=gen)
-        model.compute_gradients(s, t, twingan.make_dragan_rand(16, hw, DEV, gen))
-        del model
-  for norm in ('instance_norm', 'batch_renorm'):
-    model = twingan.GanModel(twingan.Flags(train_image_size=256, generator_norm_type=norm), device=DEV)
-    model.infer(torch.rand((64, 256, 256, 3), device=DEV, generator=gen))
-    del model
-  torch.cuda.synchronize()
-  monkeypatch.undo()
-  return seen
+def harvest_product_convs():
+  """The keys of every conv launch in the shared harvest of the product (tests/product_launches.py)."""
+  return {conv_key(name, args) for name, args in harvest_product_launches() if name in _GEOM_AT}
 
 
 # The conv launches of the product, harvested by harvest_product_convs.  A change that adds, removes or re-dispatches a conv
@@ -399,8 +369,8 @@ PRODUCT_CONVS = {
 PRODUCT_CONV_KEYS = {(entry,) + key for entry, keys in PRODUCT_CONVS.items() for key in keys}
 
 
-def test_every_product_conv_is_a_kernel_suite_case(built_lib, monkeypatch):
-  seen = harvest_product_convs(monkeypatch)
+def test_every_product_conv_is_a_kernel_suite_case(built_lib):
+  seen = harvest_product_convs()
   _log_result({'test': 'conv_coverage', 'harvested': len(seen), 'keys': sorted(seen)})
   assert seen == PRODUCT_CONV_KEYS, ('new', sorted(seen - PRODUCT_CONV_KEYS), 'gone', sorted(PRODUCT_CONV_KEYS - seen))
   missing = sorted(seen - suite_keys())

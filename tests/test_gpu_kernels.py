@@ -150,56 +150,6 @@ def test_conv_reference_on_the_gpu_matches_the_cpu_oracle(built_lib):
     assert conv_error_ratio(a, b.to('cuda:0'), s, 1e-13) <= 1.0
 
 
-@pytest.mark.parametrize('kind', ['instance_norm', 'batch_norm', 'batch_renorm', 'none'])
-@pytest.mark.parametrize('C,pix', [(16, True), (64, True), (256, True), (3, False), (32, False)])
-def test_norm_act_fwd_bwd(built_lib, kind, C, pix):
-  """The fused conv-epilogue family of BASELINE config 2 (normaliser + leaky-ReLU + pixel-norm, fwd+bwd)."""
-  from twingan_b200 import ops
-  from twingan_b200 import pggan_utils as pu
-  N, H, W = 4, 8, 8
-  y = (_rand((N, H, W, C), 5) * 0.7 + 0.3).requires_grad_(True)
-  gamma = (1 + _rand((C,), 6, 0.2)).requires_grad_(True)
-  beta = _rand((C,), 7, 0.1).requires_grad_(True)
-  gz = _rand((N, H, W, C), 8)
-  clip = {'rmin': 0.9, 'rmax': 1.1, 'dmax': 0.1}
-  stats = {'renorm_mean': _rand((C,), 9, 0.02) * 0.6, 'renorm_stddev': (0.3 + 0.1 * _rand((C,), 10).abs()) * 0.6,
-           'renorm_mean_weight': torch.tensor(0.6, dtype=torch.float64),
-           'renorm_stddev_weight': torch.tensor(0.6, dtype=torch.float64)}
-  if kind == 'instance_norm':
-    u = O.instance_norm(y, gamma, beta)
-  elif kind == 'batch_norm':
-    u = O.batch_norm_train(y, gamma, beta, None, False, None)
-  elif kind == 'batch_renorm':
-    u = O.batch_norm_train(y, gamma, beta, stats, True, clip)
-  else:
-    u = y + beta
-  z = O.leaky_relu(u)
-  if pix:
-    z = O.pixel_norm(z)
-  gy_ref, gg_ref, gb_ref = torch.autograd.grad(z, (y, gamma, beta), gz, allow_unused=True)
-
-  yd = _dev(y.detach()).requires_grad_(True)
-  gd = _dev(gamma.detach()).requires_grad_(True)
-  bd = _dev(beta.detach()).requires_grad_(True)
-  kid = pu._KIND[kind]
-  flags = ops.FLAG_LRELU | (ops.FLAG_PIXNORM if pix else 0)
-  snap = torch.zeros(4 * C + 2, device='cuda:0')
-  snap[2 * C:3 * C] = _dev(stats['renorm_mean'])
-  snap[3 * C:4 * C] = _dev(stats['renorm_stddev'])
-  snap[4 * C] = 0.6
-  snap[4 * C + 1] = 0.6
-  bs = torch.empty((2, C), device='cuda:0')
-  zd = ops.NormActFn.apply(yd, gd if kid != ops.NORM_NONE else None, bd, kid, flags, pu._EPS[kid], (0.9, 1.1, 0.1),
-                           snap, bs if kid in (ops.NORM_BATCH, ops.NORM_RENORM) else None, 'G')
-  grads = torch.autograd.grad(zd, (yd, gd, bd) if kid != ops.NORM_NONE else (yd, bd), _dev(gz))
-  torch.cuda.synchronize()
-  assert rel_err(zd, z) < REL_TOL * 0.1
-  assert rel_err(grads[0], gy_ref) < REL_TOL * 0.2
-  if kid != ops.NORM_NONE:
-    assert rel_err(grads[1], gg_ref) < REL_TOL * 0.2
-  assert rel_err(grads[-1], gb_ref) < REL_TOL * 0.2
-
-
 def test_bias_lrelu_pool_upsample_lerp_double_backward(built_lib):
   """Discriminator-side operators are twice differentiable: check d/dtheta of ||d out/dx||^2."""
   from twingan_b200 import ops
