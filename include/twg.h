@@ -119,7 +119,8 @@ int64_t twg_crc32c(const void* data, int64_t n, int64_t crc);
  *      and _pixel_norm (nets/pggan_utils.py:330-331) and their gradients --------------------------------- */
 /* Shifted sums (tf.nn.moments is two-pass; raw single-pass sums cancel once |mean| >> std):
  * sums[n][c] = {sum_hw (y - p), sum_hw (y - p)^2}, p = y[first sample of n's pivot group][pixel 0][c]
- * (pivot_group = 1 for instance norm, = the statistics group size for the batch kinds).  Zeroed by the call. */
+ * (pivot_group = 1 for instance norm, = the statistics group size for the batch kinds).  2*N*C floats, fully written
+ * by the call. */
 int twg_moments(const float* y, float* sums, int N, int HW, int C, int pivot_group, twg_stream_t stream);
 /* Turn the sums into the per-(n,c) affine z = a*y + b of the chosen normaliser (training mode) plus
  * mean/rstd for the backward.  The batch is N/group_size groups of group_size samples -- one group per original

@@ -1,7 +1,7 @@
 """Calibration of the normaliser bounds (tests/parity.py norm_sum_c, mean_bound, rstd_rel_bound) on the CPU.
 
 The statistics kernels add in a fixed order: within one block per sample, the thread of pixel group `grp` adds the pixels
-grp, grp + 256/G, grp + 2 * 256/G, ... serially in fp32 (G = lanes per pixel, vec_geom(C) in twg_elementwise.cu), the
+grp, grp + 256/G, grp + 2 * 256/G, ... serially in fp32 (G = lanes per pixel, vec_geom(C) in twg_common.cuh), the
 squares with one rounding (fma); a shared-memory tree then halves the 256/G partials.  The batch kinds add the per-sample
 sums serially over the group; the conv-epilogue route merges per-warp records {count, pivot, sum (y - pivot),
 sum (y - pivot)^2} as k_norm_finalize_inst_partials does, 32 lanes each striding over the slots, then a butterfly.  This

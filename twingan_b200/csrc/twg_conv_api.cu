@@ -1,7 +1,6 @@
 // C-ABI entry points of the convolution family: the exact-fp32 kernels on fp32 operands (pointwise for the thin 1x1
 // layers, twg_conv_pw.cu; SIMT otherwise, twg_conv_simt.cu) and the wgmma tensor-core kernels on split-bf16 planes
 // (twg_conv_tc.cu).
-#include <string.h>
 #include "twg_common.cuh"
 
 namespace twg {
@@ -11,6 +10,7 @@ int conv_wgrad_simt(const float*, const float*, float*, int, int, int, int, int,
 bool conv_tc_supported(int, int, int, int, int, int, int);
 int split_act_planes(const float*, void*, int64_t, cudaStream_t);
 int split_weight_planes(const float*, void*, int, int, int, int, cudaStream_t);
+int split_weight_table(const float*, void*, const void*, int, int64_t, cudaStream_t);
 int conv_fwd_tc_planes(const void*, const void*, float*, int, int, int, int, int, int, int, bool, cudaStream_t,
                        const float* bias = nullptr, int act = 0, void* z_planes = nullptr, float4* stats = nullptr,
                        uint8_t* act_mask = nullptr, const float* aff_a = nullptr);
@@ -75,6 +75,12 @@ int twg_split_weights(const float* w, void* planes, int k, int Cin, int Cout, in
   return split_weight_planes(w, planes, k, Cin, Cout, dgrad, S(stream));
 }
 
+int twg_split_weights_table(const float* flat, void* planes, const void* table, int rows, int64_t max_elems,
+                            twg_stream_t stream) {
+  if (!flat || !planes || !table || rows <= 0) return fail(TWG_ERR_INVALID, "twg_split_weights_table: bad args");
+  return split_weight_table(flat, planes, table, rows, max_elems, S(stream));
+}
+
 int twg_conv_epilogue_slots(int N, int H, int W, int Cin, int Cout, int k, int pad) {
   if (N <= 0 || H <= 0 || W <= 0 || Cin <= 0 || Cout <= 0) return 0;
   return conv_fwd_epilogue_slots(N, H, W, Cin, Cout, k, pad);
@@ -114,33 +120,6 @@ int twg_conv_wgrad_planes(const void* x_planes, const void* gy_planes, float* gw
   int rc = check_geom("twg_conv_wgrad_planes", x_planes, gy_planes, gw, N, H, W, Cin, Cout, k, pad);
   if (rc) return rc;
   return conv_wgrad_tc_planes(x_planes, gy_planes, gw, N, H, W, Cin, Cout, k, pad, accumulate, S(stream));
-}
-
-int64_t twg_crc32c(const void* data, int64_t n, int64_t crc) {
-  static uint32_t table[8][256];
-  static bool init = false;
-  if (!init) {
-    for (uint32_t i = 0; i < 256; ++i) {
-      uint32_t c = i;
-      for (int k = 0; k < 8; ++k) c = (c & 1) ? (c >> 1) ^ 0x82F63B78u : c >> 1;
-      table[0][i] = c;
-    }
-    for (uint32_t i = 0; i < 256; ++i)
-      for (int t = 1; t < 8; ++t) table[t][i] = (table[t - 1][i] >> 8) ^ table[0][table[t - 1][i] & 0xFF];
-    init = true;
-  }
-  const uint8_t* p = static_cast<const uint8_t*>(data);
-  uint32_t c = (uint32_t)crc ^ 0xFFFFFFFFu;
-  while (n >= 8) {                       // slicing-by-8
-    uint32_t lo, hi;
-    memcpy(&lo, p, 4); memcpy(&hi, p + 4, 4);
-    lo ^= c;
-    c = table[7][lo & 0xFF] ^ table[6][(lo >> 8) & 0xFF] ^ table[5][(lo >> 16) & 0xFF] ^ table[4][lo >> 24] ^
-        table[3][hi & 0xFF] ^ table[2][(hi >> 8) & 0xFF] ^ table[1][(hi >> 16) & 0xFF] ^ table[0][hi >> 24];
-    p += 8; n -= 8;
-  }
-  while (n-- > 0) c = table[0][(c ^ *p++) & 0xFF] ^ (c >> 8);
-  return (int64_t)(c ^ 0xFFFFFFFFu);
 }
 
 }  // extern "C"

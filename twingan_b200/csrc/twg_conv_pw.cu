@@ -159,16 +159,10 @@ __global__ void __launch_bounds__(256) k_pw_wgrad(const float* __restrict__ smal
   for (int s = 0; s < S; ++s) {
 #pragma unroll
     for (int j = 0; j < 4 * V; ++j) {
-      __syncthreads();
-      sm[threadIdx.x] = acc[s][j];
-      __syncthreads();
-      for (int st = 128; st >= G; st >>= 1) {
-        if (threadIdx.x < st) sm[threadIdx.x] += sm[threadIdx.x + st];
-        __syncthreads();
-      }
+      const float sum = block_tree_sum(acc[s][j], G, sm);
       if (threadIdx.x < G) {
         const int l = (lg + (j / 4) * 32) * 4 + (j & 3);
-        gw[(int64_t)blockIdx.x * S * L + s * ws_s + l * ws_l] = sm[threadIdx.x];   // this block's partial (add_partials)
+        gw[(int64_t)blockIdx.x * S * L + s * ws_s + l * ws_l] = sum;   // this block's partial (add_partials)
       }
     }
   }

@@ -149,60 +149,47 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes
 __device__ __forceinline__ uint64_t desc_add(uint64_t d, uint32_t byte_off) { return d + (uint64_t)(byte_off >> 4); }
 __host__ __device__ constexpr uint32_t swizzle_layout_for(int cc) { return cc == 64 ? 1u : (cc == 32 ? 2u : 3u); }
 
-// write 2 consecutive fp32 values as split-bf16 planes (hi plane [n], lo plane [n]); e = even element index
-__device__ __forceinline__ void st_planes2(void* planes, int64_t n_total, int64_t e, float a, float b) {
-  const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-  const float2 f = __bfloat1622float2(h);
-  const __nv_bfloat162 l = __floats2bfloat162_rn(a - f.x, b - f.y);
-  __nv_bfloat16* hi = reinterpret_cast<__nv_bfloat16*>(planes);
-  *reinterpret_cast<__nv_bfloat162*>(hi + e) = h;
-  *reinterpret_cast<__nv_bfloat162*>(hi + n_total + e) = l;
-}
-
 // ----------------------------------------------------------------------------------------------------
 // split kernels: fp32 -> bf16 hi/lo planes
 // ----------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void split1(float x, __nv_bfloat16& hi, __nv_bfloat16& lo) {
-  hi = __float2bfloat16_rn(x);
-  lo = __float2bfloat16_rn(x - __bfloat162float(hi));
+__global__ void __launch_bounds__(256) k_split_act(const float* __restrict__ x, void* __restrict__ planes, int64_t n4) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x)
+    st_split4(planes, n4 * 4, i, reinterpret_cast<const float4*>(x)[i]);
 }
 
-__global__ void __launch_bounds__(256) k_split_act(const float* __restrict__ x, __nv_bfloat16* __restrict__ hi,
-                                                   __nv_bfloat16* __restrict__ lo, int64_t n4) {
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
-    float4 v = reinterpret_cast<const float4*>(x)[i];
-    __nv_bfloat16 h[4], l[4];
-    split1(v.x, h[0], l[0]); split1(v.y, h[1], l[1]); split1(v.z, h[2], l[2]); split1(v.w, h[3], l[3]);
-    reinterpret_cast<uint2*>(hi)[i] = *reinterpret_cast<uint2*>(h);
-    reinterpret_cast<uint2*>(lo)[i] = *reinterpret_cast<uint2*>(l);
-  }
-}
-
+// One conv weight w[taps][Cin][Cout] (HWIO, at flat + src) -> planes at planes + dst, in the layout the weight TMA maps read:
 // forward: out[tap][co][ci] = w[tap][ci][co]           (K = Cin contiguous)
 // dgrad  : out[tap][ci][co] = w[flip(tap)][ci][co]     (K = Cout contiguous)
-__global__ void __launch_bounds__(256) k_split_weights(const float* __restrict__ w, __nv_bfloat16* __restrict__ hi,
-                                                       __nv_bfloat16* __restrict__ lo, int taps, int Cin, int Cout,
-                                                       int dgrad) {
-  const int64_t total = (int64_t)taps * Cin * Cout;
+struct SplitRow { long long src, dst; int taps, cin, cout, dgrad; };
+__device__ __forceinline__ void split_weight_row(const float* __restrict__ flat, __nv_bfloat16* __restrict__ planes,
+                                                 const SplitRow& r) {
+  const float* w = flat + r.src;
+  const int64_t total = (int64_t)r.taps * r.cin * r.cout;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     int64_t t = i;
     float v;
-    if (!dgrad) {
-      const int ci = (int)(t % Cin); t /= Cin;
-      const int co = (int)(t % Cout);
-      const int tap = (int)(t / Cout);
-      v = w[((int64_t)tap * Cin + ci) * Cout + co];
+    if (!r.dgrad) {
+      const int ci = (int)(t % r.cin); t /= r.cin;
+      const int co = (int)(t % r.cout);
+      const int tap = (int)(t / r.cout);
+      v = w[((int64_t)tap * r.cin + ci) * r.cout + co];
     } else {
-      const int co = (int)(t % Cout); t /= Cout;
-      const int ci = (int)(t % Cin);
-      const int tap = (int)(t / Cin);
-      v = w[((int64_t)(taps - 1 - tap) * Cin + ci) * Cout + co];
+      const int co = (int)(t % r.cout); t /= r.cout;
+      const int ci = (int)(t % r.cin);
+      const int tap = (int)(t / r.cin);
+      v = w[((int64_t)(r.taps - 1 - tap) * r.cin + ci) * r.cout + co];
     }
-    __nv_bfloat16 h, l;
-    split1(v, h, l);
-    hi[i] = h;
-    lo[i] = l;
+    st_split1(planes + r.dst, total, i, v);
   }
+}
+__global__ void __launch_bounds__(256) k_split_weights(const float* __restrict__ w, __nv_bfloat16* __restrict__ planes,
+                                                       SplitRow r) {
+  split_weight_row(w, planes, r);
+}
+// every conv weight of the model in one launch: blockIdx.y = table row
+__global__ void __launch_bounds__(256) k_split_weights_table(const float* __restrict__ flat, __nv_bfloat16* __restrict__ planes,
+                                                             const SplitRow* __restrict__ table) {
+  split_weight_row(flat, planes, table[blockIdx.y]);
 }
 
 // ----------------------------------------------------------------------------------------------------
@@ -705,19 +692,27 @@ static unsigned split_blocks(int64_t n4) {
   return (unsigned)blocks;
 }
 
-// planes layout: hi plane [n] bf16 followed by lo plane [n] bf16
 int split_act_planes(const float* x, void* planes, int64_t n, cudaStream_t st) {
   if (n % 4) return fail(TWG_ERR_INVALID, "twg_split_act: element count must be a multiple of 4");
-  __nv_bfloat16* hi = reinterpret_cast<__nv_bfloat16*>(planes);
-  k_split_act<<<split_blocks(n / 4), 256, 0, st>>>(x, hi, hi + n, n / 4);
+  k_split_act<<<split_blocks(n / 4), 256, 0, st>>>(x, planes, n / 4);
   return check_launch("twg_split_act");
 }
 
 int split_weight_planes(const float* w, void* planes, int k, int Cin, int Cout, int dgrad, cudaStream_t st) {
-  const int64_t total = (int64_t)k * k * Cin * Cout;
-  __nv_bfloat16* hi = reinterpret_cast<__nv_bfloat16*>(planes);
-  k_split_weights<<<(unsigned)cdiv(total, 256), 256, 0, st>>>(w, hi, hi + total, k * k, Cin, Cout, dgrad ? 1 : 0);
+  const SplitRow r{0, 0, k * k, Cin, Cout, dgrad ? 1 : 0};
+  k_split_weights<<<(unsigned)cdiv((int64_t)r.taps * Cin * Cout, 256), 256, 0, st>>>(
+      w, reinterpret_cast<__nv_bfloat16*>(planes), r);
   return check_launch("twg_split_weights");
+}
+
+int split_weight_table(const float* flat, void* planes, const void* table, int rows, int64_t max_elems, cudaStream_t st) {
+  int64_t bx = cdiv(max_elems, 256 * 4);
+  if (bx > 64) bx = 64;
+  if (bx < 1) bx = 1;
+  dim3 grid((unsigned)bx, (unsigned)rows);
+  k_split_weights_table<<<grid, 256, 0, st>>>(flat, reinterpret_cast<__nv_bfloat16*>(planes),
+                                              reinterpret_cast<const SplitRow*>(table));
+  return check_launch("twg_split_weights_table");
 }
 
 bool conv_tc_supported(int N, int H, int W, int Cin, int Cout, int k, int pad) {

@@ -531,7 +531,7 @@ class ConvBiasActFn(Function):
 
 
 def vec_ok(C: int) -> bool:
-  """Channel counts the vectorised elementwise kernels cover (mirrors vec_geom in csrc/twg_elementwise.cu)."""
+  """Channel counts the vectorised elementwise kernels cover (mirrors vec_geom in csrc/twg_common.cuh)."""
   if C % 4:
     return False
   q = C // 4
