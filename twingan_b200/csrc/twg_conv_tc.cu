@@ -221,112 +221,25 @@ struct FwdSmem {
   static_assert(kBytes <= 227 * 1024, "forward conv exceeds shared memory");
 };
 
-// Epilogue options (all null / 0 = plain fp32 store):
+// Forward epilogue of one 128-pixel tile from a consumer warp's accumulator fragment.  Options (all null / 0 = plain fp32
+// store):
 //   bias, act & 1      : + bias[c], leaky-ReLU                       (discriminator layers)
 //   z_planes           : also store the result as split-bf16 planes  (input of the next conv)
 //   act_mask           : sign of the (activated) result, 4 bits per 4 channels (the activation backward reads these)
 //   stats              : {count, pivot, S1, S2} per (image, tile, consumer warp, channel) for the instance-norm statistics
 //   aff_a              : z = pixel_norm?(lrelu?(aff_a[c] * conv + bias[c])), act bit 1 = pixel norm (Cout == BN: a row of
 //                        the accumulator fragment is spread over 4 lanes, so the pixel's mean square is a 4-lane sum)
-template <int CC, int BN>
-__global__ void __launch_bounds__(kThreads, 1) k_conv_fwd_wgmma(const __grid_constant__ CUtensorMap tm_a_hi,
-                                                                const __grid_constant__ CUtensorMap tm_a_lo,
-                                                                const __grid_constant__ CUtensorMap tm_b_hi,
-                                                                const __grid_constant__ CUtensorMap tm_b_lo,
-                                                                float* __restrict__ y, TcGeom g,
-                                                                const float* __restrict__ bias, int act,
-                                                                void* __restrict__ z_planes, float4* __restrict__ stats,
-                                                                uint8_t* __restrict__ act_mask, const float* __restrict__ aff_a) {
-  using SM = FwdSmem<CC, BN>;
-  constexpr int kStages = SM::kStages;
+// The thread holds rows r0 = 16 (warp % 4) + lane / 4 (+ 8) of warpgroup warp / 4's half and columns 8 j + 2 (lane % 4) (+ 1).
+template <int BN>
+__device__ __forceinline__ void fwd_epilogue(float (&acc)[BN / 2], float* __restrict__ y, const TcGeom& g, int tw_i,
+                                             int th_i, int n0, int co0, int warp, int lane, const float* __restrict__ bias,
+                                             int act, void* __restrict__ z_planes, float4* __restrict__ stats,
+                                             uint8_t* __restrict__ act_mask, const float* __restrict__ aff_a) {
   // the statistics, sign-mask and pixel-norm epilogues exist for the single-block shapes only (Cout <= 64; the host
-  // never asks for them otherwise), which keeps the BN = 128 instantiation within its registers
+  // never asks for them otherwise), which keeps the BN = 128 instantiations within their registers
   constexpr bool kFused = BN <= 64;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + kStages * SM::kStage);   // [kStages]
-  uint64_t* empty = full + kStages;                                           // [kStages]
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  int mt = blockIdx.x;
-  const int tw_i = mt % g.tiles_w; mt /= g.tiles_w;
-  const int th_i = mt % g.tiles_h;
-  const int tn_i = mt / g.tiles_h;
-  const int w0 = tw_i * g.TW, h0 = th_i * g.TH, n0 = tn_i * g.TN;
-  const int co0 = blockIdx.y * BN;
-  const int cchunks = g.Cin / CC;
-  const int kb_begin = 0, kb_end = g.k * g.k * cchunks;
-
-  if (warp == kConsumerWarps && lane == 0) {
-    prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_a_lo); prefetch_tmap(&tm_b_hi); prefetch_tmap(&tm_b_lo);
-    for (int s = 0; s < kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kConsumerWarps); }
-    fence_barrier_init();
-  }
-  __syncthreads();
-
-  if (warp == kConsumerWarps) {
-    if (lane == 0) {
-      int stage = 0; uint32_t phase = 0;
-      for (int kb = kb_begin; kb < kb_end; ++kb) {
-        mbar_wait(&empty[stage], phase ^ 1);
-        const int tap = kb / cchunks, cc = kb - tap * cchunks;
-        const int kh = tap / g.k, kw = tap - kh * g.k;
-        uint8_t* sa = smem + stage * SM::kStage;
-        mbar_expect_tx(&full[stage], 2 * SM::kATile + 2 * SM::kBTileRaw);
-        tma_load_4d(&tm_a_hi, &full[stage], sa, cc * CC, w0 + kw - g.pad, h0 + kh - g.pad, n0);
-        tma_load_4d(&tm_a_lo, &full[stage], sa + SM::kATile, cc * CC, w0 + kw - g.pad, h0 + kh - g.pad, n0);
-        tma_load_2d(&tm_b_hi, &full[stage], sa + 2 * SM::kATile, cc * CC, tap * g.Cout + co0);
-        tma_load_2d(&tm_b_lo, &full[stage], sa + 2 * SM::kATile + SM::kBTile, cc * CC, tap * g.Cout + co0);
-        if (++stage == kStages) { stage = 0; phase ^= 1; }
-      }
-    }
-    return;
-  }
-
-  // ---- consumers: warpgroup wg owns accumulator rows [64 wg, 64 wg + 64) of the 128-pixel tile ----
   const int wg = warp >> 2;
-  // The MMAs of kFlush consecutive stages accumulate into a fresh fragment `part`, which is then added to `acc` with fp32
-  // adds: one tensor-core accumulation chain over the whole K = 9 * Cin (up to ~14 k products) loses ~1e-5 relative.
-  constexpr int kFlush = 4;
-  float acc[BN / 2], part[BN / 2];
-#pragma unroll
-  for (int i = 0; i < BN / 2; ++i) { acc[i] = 0.f; part[i] = 0.f; }
-  {
-    constexpr uint32_t layout = swizzle_layout_for(CC);
-    constexpr uint32_t sbo = 8 * CC * 2;   // 8 rows of CC bf16
-    int stage = 0, prev = -1, chained = 0; uint32_t phase = 0;
-    for (int kb = kb_begin; kb < kb_end; ++kb) {
-      mbar_wait(&full[stage], phase);
-      const uint32_t sa = smem_u32(smem + stage * SM::kStage);
-      const uint32_t a_hi = sa + wg * (64 * CC * 2), a_lo = a_hi + SM::kATile;
-      const uint32_t b_hi = sa + 2 * SM::kATile, b_lo = b_hi + SM::kBTile;
-      const uint64_t dah = make_desc(a_hi, 16, sbo, layout), dal = make_desc(a_lo, 16, sbo, layout);
-      const uint64_t dbh = make_desc(b_hi, 16, sbo, layout), dbl = make_desc(b_lo, 16, sbo, layout);
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < CC / 16; ++ks) {
-        const uint32_t off = ks * 32;   // 16 bf16 along K inside the swizzle atom
-        Wgmma<BN>::template mma<0, 0>(part, desc_add(dal, off), desc_add(dbh, off));
-        Wgmma<BN>::template mma<0, 0>(part, desc_add(dah, off), desc_add(dbl, off));
-        Wgmma<BN>::template mma<0, 0>(part, desc_add(dah, off), desc_add(dbh, off));
-      }
-      wgmma_commit();
-      wgmma_wait<1>();                  // the previous stage's MMAs have read their operands: hand that stage back
-      if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev]); }
-      prev = stage;
-      if (++stage == kStages) { stage = 0; phase ^= 1; }
-      if (++chained == kFlush || kb + 1 == kb_end) {
-        wgmma_wait<0>();
-        fence_acc(part);
-#pragma unroll
-        for (int i = 0; i < BN / 2; ++i) { acc[i] += part[i]; part[i] = 0.f; }
-        fence_acc(part);
-        chained = 0;
-      }
-    }
-  }
-
-  // ---- epilogue: thread holds rows r0 = 16 (warp % 4) + lane / 4 (+ 8) and columns 8 j + 2 (lane % 4) (+ 1) ----
+  const int w0 = tw_i * g.TW, h0 = th_i * g.TH;
   const int quad = lane & 3;
   int64_t e_row[2];
   bool ok[2];
@@ -419,6 +332,245 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_fwd_wgmma(const __grid_con
         }
       }
     }
+  }
+}
+
+// General forward / dgrad: one CTA per (128-pixel tile, output-channel block), one pipeline stage per (tap, channel chunk)
+// holding that tap's shifted A tile and its weight tile.  Epilogue options: fwd_epilogue.
+template <int CC, int BN>
+__global__ void __launch_bounds__(kThreads, 1) k_conv_fwd_wgmma(const __grid_constant__ CUtensorMap tm_a_hi,
+                                                                const __grid_constant__ CUtensorMap tm_a_lo,
+                                                                const __grid_constant__ CUtensorMap tm_b_hi,
+                                                                const __grid_constant__ CUtensorMap tm_b_lo,
+                                                                float* __restrict__ y, TcGeom g,
+                                                                const float* __restrict__ bias, int act,
+                                                                void* __restrict__ z_planes, float4* __restrict__ stats,
+                                                                uint8_t* __restrict__ act_mask, const float* __restrict__ aff_a) {
+  using SM = FwdSmem<CC, BN>;
+  constexpr int kStages = SM::kStages;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + kStages * SM::kStage);   // [kStages]
+  uint64_t* empty = full + kStages;                                           // [kStages]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  int mt = blockIdx.x;
+  const int tw_i = mt % g.tiles_w; mt /= g.tiles_w;
+  const int th_i = mt % g.tiles_h;
+  const int tn_i = mt / g.tiles_h;
+  const int w0 = tw_i * g.TW, h0 = th_i * g.TH, n0 = tn_i * g.TN;
+  const int co0 = blockIdx.y * BN;
+  const int cchunks = g.Cin / CC;
+  const int kb_begin = 0, kb_end = g.k * g.k * cchunks;
+
+  if (warp == kConsumerWarps && lane == 0) {
+    prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_a_lo); prefetch_tmap(&tm_b_hi); prefetch_tmap(&tm_b_lo);
+    for (int s = 0; s < kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kConsumerWarps); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp == kConsumerWarps) {
+    if (lane == 0) {
+      int stage = 0; uint32_t phase = 0;
+      for (int kb = kb_begin; kb < kb_end; ++kb) {
+        mbar_wait(&empty[stage], phase ^ 1);
+        const int tap = kb / cchunks, cc = kb - tap * cchunks;
+        const int kh = tap / g.k, kw = tap - kh * g.k;
+        uint8_t* sa = smem + stage * SM::kStage;
+        mbar_expect_tx(&full[stage], 2 * SM::kATile + 2 * SM::kBTileRaw);
+        tma_load_4d(&tm_a_hi, &full[stage], sa, cc * CC, w0 + kw - g.pad, h0 + kh - g.pad, n0);
+        tma_load_4d(&tm_a_lo, &full[stage], sa + SM::kATile, cc * CC, w0 + kw - g.pad, h0 + kh - g.pad, n0);
+        tma_load_2d(&tm_b_hi, &full[stage], sa + 2 * SM::kATile, cc * CC, tap * g.Cout + co0);
+        tma_load_2d(&tm_b_lo, &full[stage], sa + 2 * SM::kATile + SM::kBTile, cc * CC, tap * g.Cout + co0);
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+      }
+    }
+    return;
+  }
+
+  // ---- consumers: warpgroup wg owns accumulator rows [64 wg, 64 wg + 64) of the 128-pixel tile ----
+  const int wg = warp >> 2;
+  // The MMAs of kFlush consecutive stages accumulate into a fresh fragment `part`, which is then added to `acc` with fp32
+  // adds: one tensor-core accumulation chain over the whole K = 9 * Cin (up to ~14 k products) loses ~1e-5 relative.
+  constexpr int kFlush = 4;
+  float acc[BN / 2], part[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) { acc[i] = 0.f; part[i] = 0.f; }
+  {
+    constexpr uint32_t layout = swizzle_layout_for(CC);
+    constexpr uint32_t sbo = 8 * CC * 2;   // 8 rows of CC bf16
+    int stage = 0, prev = -1, chained = 0; uint32_t phase = 0;
+    for (int kb = kb_begin; kb < kb_end; ++kb) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * SM::kStage);
+      const uint32_t a_hi = sa + wg * (64 * CC * 2), a_lo = a_hi + SM::kATile;
+      const uint32_t b_hi = sa + 2 * SM::kATile, b_lo = b_hi + SM::kBTile;
+      const uint64_t dah = make_desc(a_hi, 16, sbo, layout), dal = make_desc(a_lo, 16, sbo, layout);
+      const uint64_t dbh = make_desc(b_hi, 16, sbo, layout), dbl = make_desc(b_lo, 16, sbo, layout);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < CC / 16; ++ks) {
+        const uint32_t off = ks * 32;   // 16 bf16 along K inside the swizzle atom
+        Wgmma<BN>::template mma<0, 0>(part, desc_add(dal, off), desc_add(dbh, off));
+        Wgmma<BN>::template mma<0, 0>(part, desc_add(dah, off), desc_add(dbl, off));
+        Wgmma<BN>::template mma<0, 0>(part, desc_add(dah, off), desc_add(dbh, off));
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                  // the previous stage's MMAs have read their operands: hand that stage back
+      if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev]); }
+      prev = stage;
+      if (++stage == kStages) { stage = 0; phase ^= 1; }
+      if (++chained == kFlush || kb + 1 == kb_end) {
+        wgmma_wait<0>();
+        fence_acc(part);
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) { acc[i] += part[i]; part[i] = 0.f; }
+        fence_acc(part);
+        chained = 0;
+      }
+    }
+  }
+
+  fwd_epilogue<BN>(acc, y, g, tw_i, th_i, n0, co0, warp, lane, bias, act, z_planes, stats, act_mask, aff_a);
+}
+
+// ---- column-box forward / dgrad: 3x3 SAME, one channel chunk (GEMM K == CC <= 64), 16 x 8 pixel tiles inside one image.
+// Per tile the A operand is three boxes {CC, 16, 10, 1} per plane, one per kw, loaded at (w0 + kw - 1, h0 - 1): box kw's
+// pixel row r holds input pixel (w0 + kw - 1 + r % 16, h0 - 1 + r / 16), so tap (kh, kw)'s 128-pixel A tile is box kw from
+// pixel row 16 kh on, and warpgroup wg's 64-row half starts at row 16 (kh + 4 wg).  16 rows are a whole number of swizzle
+// atoms, so each tap view is an ordinary swizzled K-major operand at a different start address.  Every input pixel crosses
+// into shared memory 3 times instead of 9, with the same hardware zero fill at the borders; the consumer issues the same MMAs
+// in the same order (tap-major, lo.hi, hi.lo, hi.hi, flushed every kFlush taps) as k_conv_fwd_wgmma on the same operand
+// values, so the results are bit-identical to it.
+// The CTAs are persistent: CTA b computes work items b, b + gridDim.x, ... (item = tile + tiles * output-channel block),
+// each exactly once; the A boxes are double-buffered where they fit (CC <= 32), so the next tile's boxes load while the
+// current one computes, and weight tiles stream through their own per-tap ring.
+template <int CC, int BN>
+struct ColSmem {
+  static constexpr int kBox = 160 * CC * 2;                         // one box, one plane
+  static constexpr int kABuf = 6 * kBox;                            // [hi: kw 0, 1, 2][lo: kw 0, 1, 2]
+  static constexpr int kABufs = CC == 64 ? 1 : 2;                   // 2 x 120 KB would not fit at CC = 64
+  static constexpr int kBTileRaw = BN * CC * 2;
+  static constexpr int kBTile = (kBTileRaw + 1023) / 1024 * 1024;
+  static constexpr int kWStage = 2 * kBTile;
+  static constexpr int kWStagesRaw = (220 * 1024 - kABufs * kABuf) / kWStage;
+  static constexpr int kWStages = kWStagesRaw > 9 ? 9 : kWStagesRaw;
+  static constexpr int kBytes = kABufs * kABuf + kWStages * kWStage + 1024 /*align*/ + 256 /*barriers*/;
+  static_assert(kWStages >= 2, "column-box conv: weight ring too short");
+  static_assert(kBytes <= 227 * 1024, "column-box conv exceeds shared memory");
+};
+
+template <int CC, int BN>
+__global__ void __launch_bounds__(kThreads, 1) k_conv_fwd_cols_wgmma(const __grid_constant__ CUtensorMap tm_a_hi,
+                                                                     const __grid_constant__ CUtensorMap tm_a_lo,
+                                                                     const __grid_constant__ CUtensorMap tm_b_hi,
+                                                                     const __grid_constant__ CUtensorMap tm_b_lo,
+                                                                     float* __restrict__ y, TcGeom g,
+                                                                     const float* __restrict__ bias, int act,
+                                                                     void* __restrict__ z_planes, float4* __restrict__ stats,
+                                                                     uint8_t* __restrict__ act_mask,
+                                                                     const float* __restrict__ aff_a) {
+  using SM = ColSmem<CC, BN>;
+  constexpr int kABufs = SM::kABufs, kWStages = SM::kWStages;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sw = smem + kABufs * SM::kABuf;                                     // weight ring [kWStages][hi][lo]
+  uint64_t* afull = reinterpret_cast<uint64_t*>(sw + kWStages * SM::kWStage);  // [kABufs]
+  uint64_t* aempty = afull + kABufs;                                           // [kABufs]
+  uint64_t* wfull = aempty + kABufs;                                           // [kWStages]
+  uint64_t* wempty = wfull + kWStages;                                         // [kWStages]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tiles = g.tiles_w * g.tiles_h * g.tiles_n;
+  const int work = tiles * (g.Cout / BN);
+
+  if (warp == kConsumerWarps && lane == 0) {
+    prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_a_lo); prefetch_tmap(&tm_b_hi); prefetch_tmap(&tm_b_lo);
+    for (int s = 0; s < kABufs; ++s) { mbar_init(&afull[s], 1); mbar_init(&aempty[s], kConsumerWarps); }
+    for (int s = 0; s < kWStages; ++s) { mbar_init(&wfull[s], 1); mbar_init(&wempty[s], kConsumerWarps); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp == kConsumerWarps) {
+    if (lane == 0) {
+      int ab = 0, ws = 0; uint32_t aph = 0, wph = 0;
+      for (int u = blockIdx.x; u < work; u += gridDim.x) {
+        const int mt = u % tiles, co0 = (u / tiles) * BN;
+        const int tw_i = mt % g.tiles_w, th_i = (mt / g.tiles_w) % g.tiles_h, n0 = mt / (g.tiles_w * g.tiles_h);
+        const int w0 = tw_i * 16, h0 = th_i * 8;
+        mbar_wait(&aempty[ab], aph ^ 1);
+        mbar_expect_tx(&afull[ab], SM::kABuf);
+        uint8_t* sa = smem + ab * SM::kABuf;
+        for (int kw = 0; kw < 3; ++kw) {
+          tma_load_4d(&tm_a_hi, &afull[ab], sa + kw * SM::kBox, 0, w0 + kw - 1, h0 - 1, n0);
+          tma_load_4d(&tm_a_lo, &afull[ab], sa + (3 + kw) * SM::kBox, 0, w0 + kw - 1, h0 - 1, n0);
+        }
+        if (++ab == kABufs) { ab = 0; aph ^= 1; }
+        for (int tap = 0; tap < 9; ++tap) {
+          mbar_wait(&wempty[ws], wph ^ 1);
+          uint8_t* sb = sw + ws * SM::kWStage;
+          mbar_expect_tx(&wfull[ws], 2 * SM::kBTileRaw);
+          tma_load_2d(&tm_b_hi, &wfull[ws], sb, 0, tap * g.Cout + co0);
+          tma_load_2d(&tm_b_lo, &wfull[ws], sb + SM::kBTile, 0, tap * g.Cout + co0);
+          if (++ws == kWStages) { ws = 0; wph ^= 1; }
+        }
+      }
+    }
+    return;
+  }
+
+  const int wg = warp >> 2;
+  constexpr int kFlush = 4;                // as k_conv_fwd_wgmma (one stage there == one tap here)
+  constexpr uint32_t layout = swizzle_layout_for(CC);
+  constexpr uint32_t sbo = 8 * CC * 2;     // 8 rows of CC bf16
+  int ab = 0, ws = 0; uint32_t aph = 0, wph = 0;
+  for (int u = blockIdx.x; u < work; u += gridDim.x) {
+    const int mt = u % tiles, co0 = (u / tiles) * BN;
+    const int tw_i = mt % g.tiles_w, th_i = (mt / g.tiles_w) % g.tiles_h, n0 = mt / (g.tiles_w * g.tiles_h);
+    float acc[BN / 2], part[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) { acc[i] = 0.f; part[i] = 0.f; }
+    mbar_wait(&afull[ab], aph);
+    const uint32_t sa = smem_u32(smem + ab * SM::kABuf);
+    int prev = -1, chained = 0;
+#pragma unroll 1
+    for (int tap = 0; tap < 9; ++tap) {
+      const int kh = tap / 3, kw = tap - kh * 3;
+      mbar_wait(&wfull[ws], wph);
+      const uint32_t a_hi = sa + kw * SM::kBox + (kh + 4 * wg) * (16 * CC * 2), a_lo = a_hi + 3 * SM::kBox;
+      const uint32_t b_hi = smem_u32(sw + ws * SM::kWStage), b_lo = b_hi + SM::kBTile;
+      const uint64_t dah = make_desc(a_hi, 16, sbo, layout), dal = make_desc(a_lo, 16, sbo, layout);
+      const uint64_t dbh = make_desc(b_hi, 16, sbo, layout), dbl = make_desc(b_lo, 16, sbo, layout);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < CC / 16; ++ks) {
+        const uint32_t off = ks * 32;   // 16 bf16 along K inside the swizzle atom
+        Wgmma<BN>::template mma<0, 0>(part, desc_add(dal, off), desc_add(dbh, off));
+        Wgmma<BN>::template mma<0, 0>(part, desc_add(dah, off), desc_add(dbl, off));
+        Wgmma<BN>::template mma<0, 0>(part, desc_add(dah, off), desc_add(dbh, off));
+      }
+      wgmma_commit();
+      wgmma_wait<1>();                  // the previous tap's MMAs have read their weights: hand that stage back
+      if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&wempty[prev]); }
+      prev = ws;
+      if (++ws == kWStages) { ws = 0; wph ^= 1; }
+      if (++chained == kFlush || tap == 8) {
+        wgmma_wait<0>();
+        fence_acc(part);
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) { acc[i] += part[i]; part[i] = 0.f; }
+        fence_acc(part);
+        chained = 0;
+      }
+    }
+    // every MMA of the tile has completed: the last weight stage and the A buffer go back to the producer, which loads the
+    // next tile's boxes while this one runs its epilogue
+    __syncwarp();
+    if (lane == 0) { mbar_arrive(&wempty[prev]); mbar_arrive(&aempty[ab]); }
+    if (++ab == kABufs) { ab = 0; aph ^= 1; }
+    fwd_epilogue<BN>(acc, y, g, tw_i, th_i, n0, co0, warp, lane, bias, act, z_planes, stats, act_mask, aff_a);
   }
 }
 
@@ -685,6 +837,29 @@ static int launch_fwd(const CUtensorMap& ah, const CUtensorMap& al, const CUtens
   return check_launch("twg_conv tc");
 }
 
+// ah / al: activation maps with the column box {CC, 16, 10, 1}
+template <int CC, int BN>
+static int launch_fwd_cols(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
+                           float* y, const TcGeom& g, const float* bias, int act, void* z_planes, float4* stats,
+                           uint8_t* act_mask, const float* aff_a, cudaStream_t st) {
+  using SM = ColSmem<CC, BN>;
+  auto kern = k_conv_fwd_cols_wgmma<CC, BN>;
+  static std::once_flag once;                 // one-time attribute set-up, safe from several host threads
+  static cudaError_t attr_err = cudaSuccess;
+  static int per_sm = 1;
+  std::call_once(once, [&] {
+    attr_err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::kBytes);
+    if (attr_err == cudaSuccess)
+      attr_err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, SM::kBytes);
+    if (per_sm < 1) per_sm = 1;
+  });
+  if (attr_err != cudaSuccess) return fail(TWG_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(attr_err));
+  const int64_t work = (int64_t)g.tiles_w * g.tiles_h * g.tiles_n * (g.Cout / BN);
+  const int64_t ctas = work < (int64_t)kNumSMs * per_sm ? work : (int64_t)kNumSMs * per_sm;
+  kern<<<(unsigned)ctas, kThreads, SM::kBytes, st>>>(ah, al, bh, bl, y, g, bias, act, z_planes, stats, act_mask, aff_a);
+  return check_launch("twg_conv tc cols");
+}
+
 static unsigned split_blocks(int64_t n4) {
   int64_t blocks = cdiv(n4, 256 * 4);
   if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
@@ -758,12 +933,24 @@ int conv_fwd_tc_planes(const void* a_planes, const void* w_planes, float* y, int
   // No split-K: its fp32 atomics would add the partial tiles in a different order on every run.  The tile shape depends on
   // the layer only, never on the batch, so a sample's output is the same whichever batch it is computed in.
   const int BN = g.Cout >= 128 ? 128 : g.Cout;
+  // 3x3 SAME convs with one channel chunk on 16 x 8 tiles take the column-box kernel (same results, a third of the A traffic)
+  const bool cols = k == 3 && pad == 1 && g.Cin == CC && g.TW == 16 && g.TH == 8 && g.TN == 1 && H >= 10;
   CUtensorMap ah, al, bh, bl;
   int rc;
-  if ((rc = make_act_map(&ah, a_hi, N, H, W, g.Cin, CC, g.TW, g.TH, g.TN))) return rc;
-  if ((rc = make_act_map(&al, a_lo, N, H, W, g.Cin, CC, g.TW, g.TH, g.TN))) return rc;
+  if ((rc = make_act_map(&ah, a_hi, N, H, W, g.Cin, CC, g.TW, cols ? 10 : g.TH, g.TN))) return rc;
+  if ((rc = make_act_map(&al, a_lo, N, H, W, g.Cin, CC, g.TW, cols ? 10 : g.TH, g.TN))) return rc;
   if ((rc = make_w_map(&bh, w_hi, taps * g.Cout, g.Cin, CC, BN))) return rc;
   if ((rc = make_w_map(&bl, w_lo, taps * g.Cout, g.Cin, CC, BN))) return rc;
+#define TWG_COLS_CASE(cc, bn) \
+  if (CC == cc && BN == bn)   \
+    return launch_fwd_cols<cc, bn>(ah, al, bh, bl, y, g, bias, act, z_planes, stats, act_mask, aff_a, st);
+  if (cols) {
+    TWG_COLS_CASE(16, 16) TWG_COLS_CASE(16, 32) TWG_COLS_CASE(16, 64) TWG_COLS_CASE(16, 128)
+    TWG_COLS_CASE(32, 16) TWG_COLS_CASE(32, 32) TWG_COLS_CASE(32, 64) TWG_COLS_CASE(32, 128)
+    TWG_COLS_CASE(64, 16) TWG_COLS_CASE(64, 32) TWG_COLS_CASE(64, 64) TWG_COLS_CASE(64, 128)
+    return fail(TWG_ERR_UNSUPPORTED, "tensor-core conv: no column-box kernel for CC=%d BN=%d", CC, BN);
+  }
+#undef TWG_COLS_CASE
 #define TWG_FWD_CASE(cc, bn) \
   if (CC == cc && BN == bn)  \
     return launch_fwd<cc, bn>(ah, al, bh, bl, y, g, bias, act, z_planes, stats, act_mask, aff_a, st);
