@@ -33,6 +33,13 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// one arrive per warp, from lane 0, as a predicated instruction rather than a branch: between the MMAs of a chain a branch
+// costs registers (k_conv_fwd_cols_wgmma<16, 128> spills with `if (lane == 0) mbar_arrive(bar)`)
+__device__ __forceinline__ void mbar_arrive_lane0(uint64_t* bar, int lane) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.eq.s32 p, %1, 0;\n@p mbarrier.arrive.shared::cta.b64 _, [%0];\n}\n"
+      ::"r"(smem_u32(bar)), "r"(lane) : "memory");
+}
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   // try_wait suspends for a bounded time per attempt; a pipeline bug must surface as a trap, never as a hung GPU
   uint32_t done = 0;
@@ -335,6 +342,46 @@ __device__ __forceinline__ void fwd_epilogue(float (&acc)[BN / 2], float* __rest
   }
 }
 
+// One accumulation chain of the forward / dgrad consumer.  The MMAs of NST consecutive pipeline stages go into a fresh
+// fragment `part`, which is then added to `acc` with fp32 adds and cleared: one tensor-core accumulation chain over the whole
+// K = 9 * Cin (up to ~14 k products) would lose ~1e-5 relative.  NST is a compile-time constant and the loop is fully
+// unrolled, so no data-dependent branch touches `part` between a wgmma's issue and its wait; with one, ptxas serialises every
+// wgmma of the kernel (warning C7518) and the commit / wait_group pipelining below does nothing.
+// The ring `full` / `empty` has KST stages.  A stage goes back to the producer once the next stage's MMAs are issued and its
+// own have completed (wait_group 1); the chain's last stage once all of its MMAs have completed.
+// operands(J0 + j, stage, dah, dal, dbh, dbl) gives the A hi / lo and B hi / lo descriptors of the chain's stage j.
+template <int BN, int CC, int KST, int J0, int NST, class Operands>
+__device__ __forceinline__ void mma_chain(float (&acc)[BN / 2], float (&part)[BN / 2], uint64_t* full, uint64_t* empty,
+                                          int& stage, uint32_t& phase, int lane, const Operands& operands) {
+  int prev = 0;
+#pragma unroll
+  for (int j = 0; j < NST; ++j) {
+    mbar_wait(&full[stage], phase);
+    uint64_t dah, dal, dbh, dbl;
+    operands(J0 + j, stage, dah, dal, dbh, dbl);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < CC / 16; ++ks) {
+      const uint32_t off = ks * 32;   // 16 bf16 along K inside the swizzle atom
+      Wgmma<BN>::template mma<0, 0>(part, desc_add(dal, off), desc_add(dbh, off));
+      Wgmma<BN>::template mma<0, 0>(part, desc_add(dah, off), desc_add(dbl, off));
+      Wgmma<BN>::template mma<0, 0>(part, desc_add(dah, off), desc_add(dbh, off));
+    }
+    wgmma_commit();
+    wgmma_wait<1>();                  // the previous stage's MMAs have read their operands: hand that stage back
+    if (j > 0) { __syncwarp(); mbar_arrive_lane0(&empty[prev], lane); }
+    prev = stage;
+    if (++stage == KST) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  __syncwarp();
+  mbar_arrive_lane0(&empty[prev], lane);
+  fence_acc(part);
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) { acc[i] += part[i]; part[i] = 0.f; }
+  fence_acc(part);
+}
+
 // General forward / dgrad: one CTA per (128-pixel tile, output-channel block), one pipeline stage per (tap, channel chunk)
 // holding that tap's shifted A tile and its weight tile.  Epilogue options: fwd_epilogue.
 template <int CC, int BN>
@@ -391,45 +438,32 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_fwd_wgmma(const __grid_con
 
   // ---- consumers: warpgroup wg owns accumulator rows [64 wg, 64 wg + 64) of the 128-pixel tile ----
   const int wg = warp >> 2;
-  // The MMAs of kFlush consecutive stages accumulate into a fresh fragment `part`, which is then added to `acc` with fp32
-  // adds: one tensor-core accumulation chain over the whole K = 9 * Cin (up to ~14 k products) loses ~1e-5 relative.
-  constexpr int kFlush = 4;
+  constexpr int kFlush = 4;   // stages per accumulation chain (mma_chain)
   float acc[BN / 2], part[BN / 2];
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) { acc[i] = 0.f; part[i] = 0.f; }
   {
     constexpr uint32_t layout = swizzle_layout_for(CC);
     constexpr uint32_t sbo = 8 * CC * 2;   // 8 rows of CC bf16
-    int stage = 0, prev = -1, chained = 0; uint32_t phase = 0;
-    for (int kb = kb_begin; kb < kb_end; ++kb) {
-      mbar_wait(&full[stage], phase);
-      const uint32_t sa = smem_u32(smem + stage * SM::kStage);
-      const uint32_t a_hi = sa + wg * (64 * CC * 2), a_lo = a_hi + SM::kATile;
-      const uint32_t b_hi = sa + 2 * SM::kATile, b_lo = b_hi + SM::kBTile;
-      const uint64_t dah = make_desc(a_hi, 16, sbo, layout), dal = make_desc(a_lo, 16, sbo, layout);
-      const uint64_t dbh = make_desc(b_hi, 16, sbo, layout), dbl = make_desc(b_lo, 16, sbo, layout);
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < CC / 16; ++ks) {
-        const uint32_t off = ks * 32;   // 16 bf16 along K inside the swizzle atom
-        Wgmma<BN>::template mma<0, 0>(part, desc_add(dal, off), desc_add(dbh, off));
-        Wgmma<BN>::template mma<0, 0>(part, desc_add(dah, off), desc_add(dbl, off));
-        Wgmma<BN>::template mma<0, 0>(part, desc_add(dah, off), desc_add(dbh, off));
-      }
-      wgmma_commit();
-      wgmma_wait<1>();                  // the previous stage's MMAs have read their operands: hand that stage back
-      if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev]); }
-      prev = stage;
-      if (++stage == kStages) { stage = 0; phase ^= 1; }
-      if (++chained == kFlush || kb + 1 == kb_end) {
-        wgmma_wait<0>();
-        fence_acc(part);
-#pragma unroll
-        for (int i = 0; i < BN / 2; ++i) { acc[i] += part[i]; part[i] = 0.f; }
-        fence_acc(part);
-        chained = 0;
-      }
+    // stage 0's descriptors; stage s is SM::kStage * s bytes further
+    const uint32_t a_hi = smem_u32(smem) + wg * (64 * CC * 2), b_hi = smem_u32(smem) + 2 * SM::kATile;
+    const uint64_t dah0 = make_desc(a_hi, 16, sbo, layout), dbh0 = make_desc(b_hi, 16, sbo, layout);
+    const auto operands = [&](int, int s, uint64_t& dah, uint64_t& dal, uint64_t& dbh, uint64_t& dbl) {
+      dah = desc_add(dah0, s * SM::kStage); dal = desc_add(dah, SM::kATile);
+      dbh = desc_add(dbh0, s * SM::kStage); dbl = desc_add(dbh, SM::kBTile);
+    };
+    int stage = 0; uint32_t phase = 0;
+    int kb = kb_begin;
+#pragma unroll 1
+    for (; kb + kFlush <= kb_end; kb += kFlush)
+      mma_chain<BN, CC, kStages, 0, kFlush>(acc, part, full, empty, stage, phase, lane, operands);
+    switch (kb_end - kb) {   // the last, shorter chain
+      case 1: mma_chain<BN, CC, kStages, 0, 1>(acc, part, full, empty, stage, phase, lane, operands); break;
+      case 2: mma_chain<BN, CC, kStages, 0, 2>(acc, part, full, empty, stage, phase, lane, operands); break;
+      case 3: mma_chain<BN, CC, kStages, 0, 3>(acc, part, full, empty, stage, phase, lane, operands); break;
+      default: break;
     }
+    static_assert(kFlush == 4, "the tail chains above cover 1 .. kFlush - 1 stages");
   }
 
   fwd_epilogue<BN>(acc, y, g, tw_i, th_i, n0, co0, warp, lane, bias, act, z_planes, stats, act_mask, aff_a);
@@ -441,8 +475,8 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_fwd_wgmma(const __grid_con
 // pixel row 16 kh on, and warpgroup wg's 64-row half starts at row 16 (kh + 4 wg).  16 rows are a whole number of swizzle
 // atoms, so each tap view is an ordinary swizzled K-major operand at a different start address.  Every input pixel crosses
 // into shared memory 3 times instead of 9, with the same hardware zero fill at the borders; the consumer issues the same MMAs
-// in the same order (tap-major, lo.hi, hi.lo, hi.hi, flushed every kFlush taps) as k_conv_fwd_wgmma on the same operand
-// values, so the results are bit-identical to it.
+// in the same order (tap-major, lo.hi, hi.lo, hi.hi, in chains of taps 0-3, 4-7 and 8) as k_conv_fwd_wgmma on the same
+// operand values, so the results are bit-identical to it.
 // The CTAs are persistent: CTA b computes work items b, b + gridDim.x, ... (item = tile + tiles * output-channel block),
 // each exactly once; the A boxes are double-buffered where they fit (CC <= 32), so the next tile's boxes load while the
 // current one computes, and weight tiles stream through their own per-tap ring.
@@ -522,9 +556,10 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_fwd_cols_wgmma(const __gri
   }
 
   const int wg = warp >> 2;
-  constexpr int kFlush = 4;                // as k_conv_fwd_wgmma (one stage there == one tap here)
   constexpr uint32_t layout = swizzle_layout_for(CC);
   constexpr uint32_t sbo = 8 * CC * 2;     // 8 rows of CC bf16
+  // weight stage 0's descriptor; stage s is SM::kWStage * s bytes further
+  const uint64_t dbh0 = make_desc(smem_u32(sw), 16, sbo, layout);
   int ab = 0, ws = 0; uint32_t aph = 0, wph = 0;
   for (int u = blockIdx.x; u < work; u += gridDim.x) {
     const int mt = u % tiles, co0 = (u / tiles) * BN;
@@ -533,42 +568,21 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_fwd_cols_wgmma(const __gri
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) { acc[i] = 0.f; part[i] = 0.f; }
     mbar_wait(&afull[ab], aph);
-    const uint32_t sa = smem_u32(smem + ab * SM::kABuf);
-    int prev = -1, chained = 0;
-#pragma unroll 1
-    for (int tap = 0; tap < 9; ++tap) {
+    // hi box 0 from warpgroup wg's first pixel row; tap (kh, kw) starts kw boxes and 16 kh pixel rows further
+    const uint64_t dah0 = make_desc(smem_u32(smem + ab * SM::kABuf) + 4 * wg * (16 * CC * 2), 16, sbo, layout);
+    const auto operands = [&](int tap, int s, uint64_t& dah, uint64_t& dal, uint64_t& dbh, uint64_t& dbl) {
       const int kh = tap / 3, kw = tap - kh * 3;
-      mbar_wait(&wfull[ws], wph);
-      const uint32_t a_hi = sa + kw * SM::kBox + (kh + 4 * wg) * (16 * CC * 2), a_lo = a_hi + 3 * SM::kBox;
-      const uint32_t b_hi = smem_u32(sw + ws * SM::kWStage), b_lo = b_hi + SM::kBTile;
-      const uint64_t dah = make_desc(a_hi, 16, sbo, layout), dal = make_desc(a_lo, 16, sbo, layout);
-      const uint64_t dbh = make_desc(b_hi, 16, sbo, layout), dbl = make_desc(b_lo, 16, sbo, layout);
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < CC / 16; ++ks) {
-        const uint32_t off = ks * 32;   // 16 bf16 along K inside the swizzle atom
-        Wgmma<BN>::template mma<0, 0>(part, desc_add(dal, off), desc_add(dbh, off));
-        Wgmma<BN>::template mma<0, 0>(part, desc_add(dah, off), desc_add(dbl, off));
-        Wgmma<BN>::template mma<0, 0>(part, desc_add(dah, off), desc_add(dbh, off));
-      }
-      wgmma_commit();
-      wgmma_wait<1>();                  // the previous tap's MMAs have read their weights: hand that stage back
-      if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&wempty[prev]); }
-      prev = ws;
-      if (++ws == kWStages) { ws = 0; wph ^= 1; }
-      if (++chained == kFlush || tap == 8) {
-        wgmma_wait<0>();
-        fence_acc(part);
-#pragma unroll
-        for (int i = 0; i < BN / 2; ++i) { acc[i] += part[i]; part[i] = 0.f; }
-        fence_acc(part);
-        chained = 0;
-      }
-    }
-    // every MMA of the tile has completed: the last weight stage and the A buffer go back to the producer, which loads the
-    // next tile's boxes while this one runs its epilogue
+      dah = desc_add(dah0, kw * SM::kBox + kh * (16 * CC * 2)); dal = desc_add(dah, 3 * SM::kBox);
+      dbh = desc_add(dbh0, s * SM::kWStage); dbl = desc_add(dbh, SM::kBTile);
+    };
+    // taps 0-3, 4-7 and 8: the chains of k_conv_fwd_wgmma (one stage there == one tap here)
+    mma_chain<BN, CC, kWStages, 0, 4>(acc, part, wfull, wempty, ws, wph, lane, operands);
+    mma_chain<BN, CC, kWStages, 4, 4>(acc, part, wfull, wempty, ws, wph, lane, operands);
+    mma_chain<BN, CC, kWStages, 8, 1>(acc, part, wfull, wempty, ws, wph, lane, operands);
+    // every MMA of the tile has completed: the A buffer goes back to the producer, which loads the next tile's boxes while
+    // this one runs its epilogue
     __syncwarp();
-    if (lane == 0) { mbar_arrive(&wempty[prev]); mbar_arrive(&aempty[ab]); }
+    mbar_arrive_lane0(&aempty[ab], lane);
     if (++ab == kABufs) { ab = 0; aph ^= 1; }
     fwd_epilogue<BN>(acc, y, g, tw_i, th_i, n0, co0, warp, lane, bias, act, z_planes, stats, act_mask, aff_a);
   }
