@@ -9,7 +9,8 @@
  *  - every pointer is a CUDA device pointer owned by the caller (twg_sum_scalars takes a HOST array of device
  *    pointers); the library never allocates or frees device memory at run time.  Mutable global state: the thread-local
  *    last-error string, the launch counter, one-time kernel attribute set-up, and one 32 MB device buffer per device
- *    (allocated when the library loads) for the partial sums of cross-block reductions;
+ *    (allocated when the library loads) for the partial sums of cross-block reductions (plus 64 KB of fp64 partial sums
+ *    for the twg_swd_* evaluation entries);
  *  - results are bit-identical from run to run: reductions add their partial sums in a fixed order, never with fp32
  *    atomics;
  *  - every call takes a cudaStream_t (passed as void*), is asynchronous and graph-capturable.  Calls for one device must
@@ -296,6 +297,34 @@ int twg_adam(float* p, const float* g, float* m, float* v, int64_t n, float lr_t
  * can be replayed while the Adam time step advances) */
 int twg_adam_dev_lr(float* p, const float* g, float* m, float* v, int64_t n, const float* lr_t_dev, float beta1,
                     float beta2, float eps, twg_stream_t stream);
+
+/* ---- sliced Wasserstein distance, an evaluation outside the step: --calc_swd (image_generation.py:147-156, 868-927),
+ *      whose library the reference does not ship (:926-927).  The metric is PGGAN's (Karras et al., ICLR 2018, section 5
+ *      and appendix D; metrics/sliced_wasserstein.py of its release): Laplacian pyramid, 7x7 neighbourhood descriptors,
+ *      per-channel normalisation (finalize_descriptors), sliced W1 over random unit directions (sliced_wasserstein).
+ *      Images are NHWC fp32 RGB.  Finite inputs are a precondition: NaN or infinity gives undefined results. */
+/* Laplacian pyramid (pyr_down / pyr_up with g = [1,4,6,4,1]^T[1,4,6,4,1]/256, mirror borders as
+ * scipy.ndimage.convolve(mode='mirror'); the last level stays Gaussian) of x:[N,R,R,3] into pyr: level l = 0..levels-1 is
+ * [N, R>>l, R>>l, 3] at float offset N*3*sum_{k<l} (R>>k)^2.  R a power of two, R >> (levels-1) >= 4. */
+int twg_swd_pyramid(const float* x, float* pyr, int N, int R, int levels, twg_stream_t stream);
+/* desc[(n*nhoods + k)][c*s*s + dy*s + dx] = level[n][cy - s/2 + dy][cx - s/2 + dx][c] (PGGAN's NCHW component order),
+ * s = nhood_size (odd), centres: int32 {cy, cx} per [n][k], clamped into [s/2, Rl - 1 - s/2] */
+int twg_swd_gather(const float* level, const void* centres, float* desc, int N, int Rl, int nhoods, int nhood_size,
+                   twg_stream_t stream);
+/* stats = {mean[3], rstd[3]} of desc:[rows][3*s*s] per channel over all rows and s*s positions, population std (ddof 0),
+ * summed in fp64; rstd = 1/std, 0 for a channel whose std is 0 */
+int twg_swd_stats(const float* desc, float* stats, int64_t rows, int nhood_size, twg_stream_t stream);
+/* proj[j][i] (column-major, [ndirs][rows]) = sum_k (desc[i][k] - mean[c(k)]) * rstd[c(k)] * dirs[k][j], exact fp32 FMA;
+ * dirs:[3*s*s][ndirs], ndirs a multiple of 128 */
+int twg_swd_project(const float* desc, const float* stats, const float* dirs, float* proj, int64_t rows, int nhood_size,
+                    int ndirs, twg_stream_t stream);
+/* bytes of device workspace twg_swd_sort needs (<0: invalid sizes) */
+int64_t twg_swd_sort_workspace(int segments, int64_t seg_len);
+/* sorts each of `segments` consecutive columns of seg_len (< 2^31) fp32 keys ascending, in place (stable LSD radix sort
+ * over order-preserving uint32 keys; -0 sorts before +0) */
+int twg_swd_sort(float* keys, void* workspace, int segments, int64_t seg_len, twg_stream_t stream);
+/* out_f64[0] = sum_i |a[i] - b[i]| accumulated in fp64 (one double in device memory) */
+int twg_swd_sorted_l1(const float* a, const float* b, void* out_f64, int64_t n, twg_stream_t stream);
 
 #ifdef __cplusplus
 }

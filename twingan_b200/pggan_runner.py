@@ -185,13 +185,14 @@ def warm_start(model, ckpt: Dict[str, object], ignore_missing_vars: bool = False
 
 # -- the loop ----------------------------------------------------------------------------------------------
 BatchFn = Callable[[Stage, int], Tuple[torch.Tensor, torch.Tensor]]
+EvalFn = Callable[[object, int], object]
 
 
 def run_stage(model, stage: Stage, batch_fn: BatchFn, train_dir: Optional[str] = None, start_step: int = 0,
               max_steps: Optional[int] = None, save_every: int = 0, use_graph: bool = True,
               grow_start_number_of_steps: int = 0, dragan_generator: Optional[torch.Generator] = None,
               log_fn: Optional[Callable[[int, Dict[str, float]], None]] = None, alternating: bool = False,
-              prefetch: int = 0) -> int:
+              prefetch: int = 0, eval_every_n_iter_in_training: int = 0, eval_fn: Optional[EvalFn] = None) -> int:
   """Train `model` for one stage, from `start_step` to min(stage.max_number_of_steps, start_step + max_steps).
   Returns the step reached.  Growing stages recompute alpha every step (twingan.py:834-835) and therefore run the
   eager step; stable stages capture the step once and replay it.  `alternating`: the reference's own schedule
@@ -199,7 +200,9 @@ def run_stage(model, stage: Stage, batch_fn: BatchFn, train_dir: Optional[str] =
   the simultaneous mode-B step; `step` then counts runs, like the reference's n_critic_counter.
   `prefetch` > 0: `batch_fn` returns HOST tensors; a background thread keeps that many batches ready in pinned memory and
   the host->device copy of batch k+1 runs on a side stream while step k computes (prefetch.py; the reference's
-  slim.prefetch_queue, model/model_inheritor.py:425-470)."""
+  slim.prefetch_queue, model/model_inheritor.py:425-470).
+  `eval_every_n_iter_in_training` > 0 with `eval_fn`: eval_fn(model, step) after every step that reaches a multiple of it
+  (twingan.py:679-680), e.g. swd.make_eval_fn; the evaluation must leave the model's training state as it found it."""
   from . import twingan
   end = stage.max_number_of_steps if max_steps is None else min(stage.max_number_of_steps, start_step + max_steps)
   graphed = False
@@ -231,6 +234,8 @@ def run_stage(model, stage: Stage, batch_fn: BatchFn, train_dir: Optional[str] =
     step += 1
     if log_fn is not None:
       log_fn(step, {'generator_loss': float(g), 'discriminator_loss': float(d)})
+    if eval_fn is not None and eval_every_n_iter_in_training > 0 and step % eval_every_n_iter_in_training == 0:
+      eval_fn(model, step)
     if train_dir and save_every and step % save_every == 0:
       save_checkpoint(model, train_dir, step)
   model.flags.global_step = step
@@ -244,13 +249,15 @@ def run_stage(model, stage: Stage, batch_fn: BatchFn, train_dir: Optional[str] =
 def run(base_flags, base_dir: str, batch_fn: BatchFn, stages: Optional[Iterable[Stage]] = None,
         max_steps_per_stage: Optional[int] = None, device='cuda', seed: int = 1234, process_group=None,
         save_every: int = 0, use_graph: bool = True, log_fn=None, tf_checkpoint_prefix: Optional[str] = None,
-        prefetch: int = 0):
+        prefetch: int = 0, eval_every_n_iter_in_training: int = 0, eval_fn: Optional[EvalFn] = None):
   """pggan_runner.py main(): walk the stage plan; skip stages whose checkpoint already reached the stage's step count
   (:117-121); resume a partially trained stage from its own directory; otherwise warm-start from the previous
   stage's directory with ignore_missing_vars = is_growing (:137-146).  `tf_checkpoint_prefix`: a TensorFlow V2
   checkpoint of the reference (e.g. its pretrained models) that seeds the first stage that has nothing to start
   from (twingan_b200/tf_checkpoint.py).  `prefetch` > 0: `batch_fn` returns host tensors that are produced on a background
-  thread and copied ahead of the step (run_stage).  Returns the last model."""
+  thread and copied ahead of the step (run_stage).  `eval_every_n_iter_in_training` / `eval_fn`: periodic evaluation as in
+  run_stage, for the stages of 16 x 16 and up (the reference skips SWD below 16, image_generation.py:869-871).  Returns the
+  last model."""
   from . import twingan
   last_train_dir = None
   model = None
@@ -279,6 +286,7 @@ def run(base_flags, base_dir: str, batch_fn: BatchFn, stages: Optional[Iterable[
       tf_checkpoint.import_into(model, tf_checkpoint_prefix, ignore_missing_vars=True)
     run_stage(model, st, batch_fn, train_dir, start_step=start,
               max_steps=None if max_steps_per_stage is None else target - start, save_every=save_every,
-              use_graph=use_graph, log_fn=log_fn, prefetch=prefetch)
+              use_graph=use_graph, log_fn=log_fn, prefetch=prefetch,
+              eval_every_n_iter_in_training=eval_every_n_iter_in_training if st.hw >= 16 else 0, eval_fn=eval_fn)
     last_train_dir = train_dir
   return model
