@@ -83,6 +83,107 @@ def norm_sum_c(R, samples=1) -> float:
   return (16.0 + 2.0 * math.sqrt(R) + 2.0 * math.sqrt(samples)) * U32
 
 
+def dragan_var_rel_bound(R, kappa):
+  """Bound on |var_dev - var| / var for the DRAGAN perturbation's variance over all pixels, taken as E[x^2] - m^2 from
+  unshifted fp32 sums whose threads each add R terms (norm_sum_c(R) of their S each): the difference loses accuracy with
+  the condition kappa = 1 + m^2 / var, E[x^2] + 2 m^2 = var (1 + 3 m^2 / var) <= 3 kappa var."""
+  return 3.0 * (norm_sum_c(R) + U32) * kappa + 4.0 * U32
+
+
+def unit_distance_bound(c_ss, s):
+  """Bound on |(s_dev - 1) - (s - 1)| for s = sqrt(ss) of an fp32 sum of squares ss with c of conv_error_ratio `c_ss`:
+  sqrt halves the relative error of ss and adds its own rounding, and the subtraction of 1 is exact or adds one more.
+  Relative to |s - 1| this is ill-conditioned by s / |s - 1| (the gradient penalty's (||g|| - 1))."""
+  return s * (0.5 * c_ss + 2.0 * U32)
+
+
+def grid_sum_c(R, nb):
+  """c of a grid-stride loss sum (k_l1, k_l1_groups, k_fanout_fwd): each thread adds R terms serially, block_sum over 256
+  threads, one product by w / n per block, then add_partials adds the nb block partials in block order."""
+  return norm_sum_c(R, nb) + 2 * U32
+
+
+def penalty_c_ss(chunk, nb):
+  """c of the per-sample sum of squares of twg_grad_penalty: k_row_sumsq's threads each add cdiv(chunk, 256) squares
+  (one rounding each, the fma), a block_sum over 256 threads, then add_partials adds the nb blocks of a sample."""
+  return norm_sum_c(-(-chunk // 256), nb * 256) + U32
+
+
+def penalty_ref(ss, c_ss, lam, N):
+  """fp64 coefficients lam 2 (s - 1) / (N s) and loss lam mean (s - 1)^2 of k_grad_penalty_finalize from the exact sums
+  of squares ss [N], with their bounds when the device's sums carry c_ss (unit_distance_bound for s - 1; the quotient,
+  products and the 64-thread block sum add a few roundings)."""
+  s = ss.sqrt()
+  e = unit_distance_bound(c_ss, s)
+  coef = lam * 2 * (s - 1) / (N * s)
+  coef_b = lam * 2 / (N * s) * (e + (s - 1).abs() * (0.5 * c_ss + 6 * U32))
+  loss = lam * ((s - 1) ** 2).sum() / N
+  loss_b = lam * (2 * (s - 1).abs() * e + 16 * U32 * (s - 1) ** 2).sum() / N
+  return coef, coef_b, loss, loss_b
+
+
+MB_CLUSTER, MB_THREADS = 8, 512   # k_mbstd_*: one cluster of 8 CTAs of 512 threads per group
+
+
+def mbstd_stats(x, groups):
+  """Per group and feature of x [N, P, C] (any device), fp64: d = x - mean over the group's samples, var (population),
+  sigma = sqrt(var + 1e-8), and A = mean |x| (the scale of the fp32 mean's error), each [groups, Ng, F] or [groups, 1, F]."""
+  N = x.shape[0]
+  x64 = x.double().reshape(groups, N // groups, -1)
+  m = x64.mean(1, keepdim=True)
+  d = x64 - m
+  var = (d * d).mean(1, keepdim=True)
+  return d, var, (var + 1e-8).sqrt(), x64.abs().mean(1, keepdim=True)
+
+
+def mbstd_sig_rel(Ng, A, var):
+  """Relative bound on the fp32 sigma of one feature: the two-pass variance of Ng samples around an fp32 mean m + e
+  (|e| <= Ng u A) adds sum (x - m - e)^2 = var Ng + Ng e^2 -- no first-order term -- plus Ng + 4 roundings; sqrt halves it."""
+  return (Ng + 8) * U32 + 2 * (Ng * U32 * A) ** 2 / var
+
+
+def mbstd_feature_sum_c(F):
+  """c of a sum over the F features of one group: each thread of the cluster adds cdiv(F, 8 * 512) features serially,
+  then a block_sum over 512 threads and the 8 CTAs' sums in rank order."""
+  return norm_sum_c(-(-F // (MB_CLUSTER * MB_THREADS)), MB_CLUSTER * 32)
+
+
+def mbstd_fwd_ref(x, groups):
+  """fp64 statistic s [groups] of twg_mbstd_fwd on x [N, P, C] and its bound."""
+  N, P, C = x.shape
+  _, var, sig, A = mbstd_stats(x, groups)
+  s = sig.mean(-1).reshape(groups)
+  return s, (sig * mbstd_sig_rel(N // groups, A, var)).mean(-1).reshape(groups) + mbstd_feature_sum_c(P * C) * s
+
+
+def mbstd_bwd2_ref(x, ggx, gstat, groups):
+  """fp64 outputs of twg_mbstd_bwd2 on x, ggx [N, P, C] and the statistic channel's gradient gstat [N, P], with bounds:
+  (dG [groups], its bound, dx [groups, Ng, F], its bound).  G = sum gstat is a block sum of Ng P terms; each feature's
+  gd = sum ggx d reads d = x - (m + e) and so carries e sum ggx; dx = G k (ggx - gm - d gd / (Ng var))."""
+  N, P, C = x.shape
+  Ng, F = N // groups, P * C
+  d, var, sig, A = mbstd_stats(x, groups)
+  gg = ggx.double().reshape(groups, Ng, F)
+  Agg = gg.abs().sum(1, keepdim=True)
+  gs = gstat.double().reshape(groups, Ng * P)
+  G, SG = gs.sum(1)[:, None, None], gs.abs().sum(1)[:, None, None]
+  cG = norm_sum_c(-(-(Ng * P) // MB_THREADS), 16)
+  k = 1.0 / (Ng * F * sig)
+  gd = (gg * d).sum(1, keepdim=True)
+  gm = gg.mean(1, keepdim=True)
+  sr = mbstd_sig_rel(Ng, A, var)
+  gd_err = (Ng + 4) * U32 * (gg * d).abs().sum(1, keepdim=True) + Ng * U32 * A * Agg
+  dG = (gd * k).sum(-1).reshape(groups)
+  dG_S = (gd.abs() * k).sum(-1).reshape(groups)
+  dG_b = ((gd_err + (sr + 4 * U32) * gd.abs()) * k).sum(-1).reshape(groups) + mbstd_feature_sum_c(F) * dG_S
+  inner = gg - gm - d * gd / (Ng * var)
+  t3 = (d * gd / (Ng * var)).abs()
+  inner_err = (4 * U32 * (gg.abs() + gm.abs() + t3) + U32 * Agg + (Ng * U32 * A) * gd.abs() / (Ng * var)
+               + d.abs() * gd_err / (Ng * var) + t3 * (2 * sr + 6 * U32))
+  dx_b = (G * k).abs() * inner_err + (cG * SG * k + (G * k).abs() * (sr + 6 * U32)) * inner.abs()
+  return dG, dG_b, G * k * inner, dx_b
+
+
 def mean_bound(R, abs_dev_mean, mean, samples=1):
   """Per-element bound on |mean_dev - mean_ref| for a mean taken from shifted sums with serial runs of R terms: the sum's
   bound on E|y - pivot| (`abs_dev_mean`), plus 4x the final rounding of pivot + E[y - pivot] (<= u |mean|)."""

@@ -1,7 +1,11 @@
-"""Every library launch of the product's training step and inference, recorded once per test session.
+"""Every library launch of the product's training step and inference, recorded once per test session, and the recorder
+the stage tests launch through.
 
-The conv and normaliser audits (test_gpu_conv_conformance.py, test_gpu_norm_conformance.py) each filter this one harvest,
-so the step runs once and there is one copy of the recorder."""
+The conv, normaliser and elementwise audits (test_gpu_conv_conformance.py, test_gpu_norm_conformance.py,
+test_gpu_elementwise_conformance.py) each filter this one harvest, so the step runs once and there is one copy of the
+recorder."""
+import contextlib
+
 import torch
 
 DEV = 'cuda:0'
@@ -11,7 +15,7 @@ _LAUNCHES = None
 def harvest_product_launches():
   """(entry point, args) of every L.call, in order, of one eager training step per image size (4..256, 16 pairs; growing
   at alpha 0.5 from 8 up; instance norm, batch renorm, batch norm, instance norm with residual blocks) followed by its EMA
-  pushes, and of inference on 64 images (instance norm, batch renorm, batch norm).  Cached for the session."""
+  pushes and its optimiser apply, and of inference on 64 images (instance norm, batch renorm, batch norm).  Cached for the session."""
   global _LAUNCHES
   if _LAUNCHES is not None:
     return _LAUNCHES
@@ -39,6 +43,7 @@ def harvest_product_launches():
           t = torch.rand((16, hw, hw, 3), device=DEV, generator=gen)
           _, _, _, stats = model.compute_gradients(s, t, twingan.make_dragan_rand(16, hw, DEV, gen))
           model.apply_stat_updates(stats)
+          model.apply_gradients()
           del model
     for norm in ('instance_norm', 'batch_renorm', 'batch_norm'):
       model = twingan.GanModel(twingan.Flags(train_image_size=256, generator_norm_type=norm), device=DEV)
@@ -49,3 +54,27 @@ def harvest_product_launches():
     del L.call
   _LAUNCHES = seen
   return seen
+
+
+class Recorder:
+  """L.call that also keeps (entry, args): a stage test asserts that it launched the key it stands for, `keys` mapping
+  the recorded launches to the keys of its audit.  Inside spying(), launches the library's Python layer (ops) makes are
+  recorded too."""
+
+  def __init__(self, L, keys):
+    self.L, self.call, self.launches, self._keys = L, L.call, [], keys
+
+  def __call__(self, name, *args):
+    self.launches.append((name, args))
+    self.call(name, *args)
+
+  @contextlib.contextmanager
+  def spying(self):
+    self.L.call = self
+    try:
+      yield self
+    finally:
+      del self.L.call
+
+  def keys(self):
+    return self._keys(self.launches)

@@ -13,14 +13,12 @@ mode) as the training step and inference launch it.
   * the fused layer (ops.GenLayerFn) end to end against the oracle's fp64 chain once per product backward key, at the
     product's N, groups, domains, gy route, pool fold and accumulate, with the device's active set transferred; and the
     single-domain 8x8 layer (NormActFn) for all four kinds, incl. the 3-channel scalar and 256-channel routes."""
-import contextlib
-
 import pytest
 import torch
 
 from tests.parity import (REL_TOL, U32, _log_result, conv_error_ratio, ema_c, exact_elem_c, mean_bound, norm_sum_c, rel_err,
                           rstd_rel_bound, serial_run)
-from tests.product_launches import harvest_product_launches
+from tests.product_launches import Recorder, harvest_product_launches
 from tests.product_norms import PRODUCT_NORM_KEYS
 from tests.test_gpu_conv_conformance import _bits, _split_ref
 
@@ -71,32 +69,11 @@ def norm_keys(launches):
                 '+'.join(filter(None, (_opts(a, _APPLY_PTRS), 'accumulate' if a[13] else '')))))
     elif name == 'twg_norm_update_stats':                                          # kind, C, decay
       keys.add((name, a[2], a[5], round(float(a[3]), 6)))
-    elif name == 'twg_colsum':
-      keys.add((name, a[2], a[3], a[4]))
   return keys
 
 
-class _Recorder:
-  """L.call that also keeps (entry, args): a stage test asserts that it launched the key it stands for.  Inside spying(),
-  launches the library's Python layer (ops) makes are recorded too."""
-
-  def __init__(self, L):
-    self.L, self.call, self.launches = L, L.call, []
-
-  def __call__(self, name, *args):
-    self.launches.append((name, args))
-    self.call(name, *args)
-
-  @contextlib.contextmanager
-  def spying(self):
-    self.L.call = self
-    try:
-      yield self
-    finally:
-      del self.L.call
-
-  def keys(self):
-    return norm_keys(self.launches)
+def _Recorder(L):
+  return Recorder(L, norm_keys)
 
 
 def _p(t):
