@@ -9,7 +9,7 @@ Prints and writes to DIR:
     the step (the sum of all kernel durations);
   * convs.json / the second table: every tensor-core conv launch of the step (entry point and geometry, recorded where
     twingan_b200.ops calls the library) matched to its kernel in the trace, with its time, FLOPs, algorithmic HBM bytes and
-    the modelled L2 -> shared-memory operand bytes of the kernels before and after the column-box forward (conv_traffic);
+    the modelled L2 -> shared-memory operand bytes of the per-tap and the column-box kernels (conv_traffic);
   * trace.json, the profiler's Chrome trace.
 The card name and power limit are read in the same run.  TWG_LIB selects another build of the library.  Needs a GPU."""
 from __future__ import annotations
@@ -51,7 +51,8 @@ def conv_traffic(entry, N, H, W, Cin, Cout, k, pad):
   """{'flops', 'hbm', 'l2_before', 'l2_after', 'cols'} of one tensor-core conv launch.
   flops: 2 MACs per product of the convolution (not the 3 split-bf16 MMAs).  hbm: algorithmic bytes, every operand read and
   every result written once (split planes 4 B per element, fp32 results 4 B).  l2_*: bytes the kernel's TMA loads move from
-  L2 into shared memory, per CTA work item summed over the grid.  cols: the forward / dgrad takes the column-box kernel."""
+  L2 into shared memory, per CTA work item summed over the grid, with the per-tap kernel (before) and the kernel the shape
+  takes (after).  cols: the shape takes the column-box kernel."""
   TW, TH, TN, tiles = _tiles(N, H, W)
   taps, px = k * k, N * H * W
   flops = 2.0 * px * Cin * Cout * taps
@@ -59,10 +60,12 @@ def conv_traffic(entry, N, H, W, Cin, Cout, k, pad):
     CN = _chunk(Cin)
     BNW = 64 if (Cout >= 64 and CN < 64) else (32 if Cout >= 32 else Cout)
     items = tiles * (Cout // BNW) * (Cin // CN)
-    per_item = 2 * 128 * BNW * 2 + taps * 2 * 128 * CN * 2     # gy tile + one x tile per tap, hi and lo planes
-    l2 = float(items * per_item)
-    return {'flops': flops, 'hbm': 4.0 * px * (Cin + Cout) + 4.0 * taps * Cin * Cout, 'l2_before': l2, 'l2_after': l2,
-            'cols': False}
+    gy = 2 * 128 * BNW * 2                                       # gy tile, hi and lo planes
+    before = items * (gy + taps * 2 * 128 * CN * 2)             # one x tile per tap
+    cols = k == 3 and pad == 1 and TW == 16 and TH == 8 and TN == 1 and H >= 10
+    after = items * (gy + 3 * 2 * 160 * CN * 2) if cols else before   # three {CN, 16, 10} column boxes per tile
+    return {'flops': flops, 'hbm': 4.0 * px * (Cin + Cout) + 4.0 * taps * Cin * Cout, 'l2_before': float(before),
+            'l2_after': float(after), 'cols': cols}
   K, Nc = (Cout, Cin) if entry == 'twg_conv_dgrad_planes' else (Cin, Cout)
   CC = _chunk(K)
   BN = min(Nc, 128)
@@ -145,9 +148,9 @@ def main():
   for d in table:
     print('%-64s %8d %11.1f %6.1f%%' % (d['kernel'][:64], d['launches'], d['us'], 100 * d['share']))
 
-  # each tensor-core fwd / dgrad call launches one k_conv_fwd*_wgmma kernel, each wgrad call one k_conv_wgrad_wgmma, in order
+  # each tensor-core fwd / dgrad call launches one k_conv_fwd*_wgmma kernel, each wgrad call one k_conv_wgrad*_wgmma, in order
   fwd_k = [e for e in kernels if 'k_conv_fwd' in e['name'] and 'wgmma' in e['name']]
-  wg_k = [e for e in kernels if 'k_conv_wgrad_wgmma' in e['name']]
+  wg_k = [e for e in kernels if 'k_conv_wgrad' in e['name'] and 'wgmma' in e['name']]
   fwd_c = [c for c in calls if c[0] != 'twg_conv_wgrad_planes']
   wg_c = [c for c in calls if c[0] == 'twg_conv_wgrad_planes']
   if len(fwd_k) != len(fwd_c) or len(wg_k) != len(wg_c):
@@ -162,10 +165,16 @@ def main():
                      thin=bool(k == 3 and gemm_k <= 64 and H >= 64)))
   groups = collections.OrderedDict()
   for row in rows:
-    for gname in ('all tensor-core convs', 'GEMM-K <= 64, 3x3, >= 64^2', 'column-box forward / dgrad'):
+    wgrad = row['entry'] == 'twg_conv_wgrad_planes'
+    for gname in ('all tensor-core convs', 'GEMM-K <= 64, 3x3, >= 64^2', 'column-box forward / dgrad',
+                  'all weight gradients', 'column-box weight gradients'):
       if gname == 'GEMM-K <= 64, 3x3, >= 64^2' and not row['thin']:
         continue
-      if gname == 'column-box forward / dgrad' and not row['cols']:
+      if gname == 'column-box forward / dgrad' and not (row['cols'] and not wgrad):
+        continue
+      if gname == 'all weight gradients' and not wgrad:
+        continue
+      if gname == 'column-box weight gradients' and not (row['cols'] and wgrad):
         continue
       g = groups.setdefault(gname, {'launches': 0, 'us': 0.0, 'flops': 0.0, 'hbm': 0.0, 'l2_before': 0.0, 'l2_after': 0.0})
       g['launches'] += 1

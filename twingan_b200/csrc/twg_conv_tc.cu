@@ -745,6 +745,274 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_wgrad_wgmma(const __grid_c
   }
 }
 
+// ---- column-box weight gradient: 3x3 SAME, 16 x 8 pixel tiles inside one image.  Same grid, pixel split and partial slices
+// as k_conv_wgrad_wgmma, but per tile and plane x arrives as the forward's three boxes {CN, 16, 10, 1}, one per kw, at
+// (w0 + kw - 1, h0 - 1): tap (kh, kw)'s 128-pixel tile is box kw from pixel row 16 kh on.  Every x pixel crosses into shared
+// memory 3 times instead of 9.
+// The MN-major A operand stacks CN-channel tap slots in M at the descriptor's LBO, which must be one uniform stride: taps
+// (kh, kw), (kh + 1, kw), ... are 16 pixel rows apart (whole swizzle atoms at 32, 64 and 128 B), taps (kh, kw), (kh, kw + 1)
+// one box apart.  A warpgroup's units of M = 64 rows (WgUnit) are
+//   CN = 16: one kw column per unit, 3 taps and a padding slot   -- warpgroup 0: kw 0, 1;  warpgroup 1: kw 2
+//   CN = 32: two taps per unit                                    -- 0: (0-1, 0), (2, 0-1), (0-1, 1);  1: (0-1, 2), (2, 2) + pad
+//   CN = 64: one tap per unit, in kw-major order t = 3 kw + kh    -- 0: even t;  1: odd t
+// A padding slot's accumulator rows are discarded; its A rows reach at most 16 pixel rows past its box, which is still this
+// CTA's shared memory (the next box, x stage or the gy ring).
+// Every element gw[tap][ci][co] sees the same arithmetic as in k_conv_wgrad_wgmma -- per tile a fresh fragment of the MMAs
+// ks = 0..7 x (lo.hi, hi.lo, hi.hi) on the same operand values, added to the running sum in fp32, tiles in order -- so the
+// results are bit-identical to it.
+// Pipeline: an x stage holds the boxes of the whole tile where two or more fit (CN <= 32), else of one kw column (CN = 64: the
+// next tile's kw = 0 boxes load while kw = 2 computes); gy tiles have their own ring.  Each warpgroup issues its units as
+// fully unrolled MMA sequences, one commit group per unit, and keeps one group in flight (two fragments) where registers allow;
+// an x stage goes back to the producer once its units' MMAs have completed.
+struct WgUnit { int kw, kh, along_kw, n; };   // taps (kh + q, kw) or, along_kw, (kh, kw + q), q < n; box kw from row 16 kh
+
+__host__ __device__ constexpr int wg_units(int cn, int wg) {
+  return cn == 16 ? (wg == 0 ? 2 : 1) : (cn == 32 ? (wg == 0 ? 3 : 2) : (wg == 0 ? 5 : 4));
+}
+__host__ __device__ constexpr WgUnit wg_unit(int cn, int wg, int j) {
+  if (cn == 16) return WgUnit{wg == 0 ? j : 2, 0, 0, 3};
+  if (cn == 32) {
+    if (wg == 0) return j == 0 ? WgUnit{0, 0, 0, 2} : (j == 1 ? WgUnit{0, 2, 1, 2} : WgUnit{1, 0, 0, 2});
+    return j == 0 ? WgUnit{2, 0, 0, 2} : WgUnit{2, 2, 0, 1};
+  }
+  return WgUnit{(2 * j + wg) / 3, (2 * j + wg) % 3, 0, 1};
+}
+// every tap in exactly one slot, each warpgroup's units in non-decreasing kw (the order the CN = 64 stages arrive in), and no
+// slot beyond the box's 10 rows / the tile's 3 boxes other than one trailing padding slot
+__host__ __device__ constexpr bool wg_units_ok(int cn) {
+  int seen[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+  for (int wg = 0; wg < 2; ++wg)
+    for (int j = 0; j < wg_units(cn, wg); ++j) {
+      const WgUnit u = wg_unit(cn, wg, j);
+      if (j > 0 && u.kw < wg_unit(cn, wg, j - 1).kw) return false;
+      if (u.n < 1 || u.n > 64 / cn || (u.n < 64 / cn && u.n + 1 < 64 / cn)) return false;
+      for (int q = 0; q < u.n; ++q) {
+        const int kh = u.kh + (u.along_kw ? 0 : q), kw = u.kw + (u.along_kw ? q : 0);
+        if (kh > 2 || kw > 2) return false;
+        ++seen[3 * kh + kw];
+      }
+    }
+  for (int t = 0; t < 9; ++t)
+    if (seen[t] != 1) return false;
+  return true;
+}
+static_assert(wg_units_ok(16) && wg_units_ok(32) && wg_units_ok(64), "column-box wgrad: tap units");
+
+// Registers: a warpgroup keeps two fragments (one commit group in flight while the previous one is added) where they fit in
+// ~96 floats beside its accumulators, and at most ~96 floats of fragments and accumulators in all: the rest of the 168 go to
+// descriptors and ring state (above that, ptxas spills).  Accumulators beyond the budget live in shared memory.
+__host__ __device__ constexpr int wg_fragments(int cn, int bnw, int wg) { return (wg_units(cn, wg) + 2) * (bnw / 2) <= 96 ? 2 : 1; }
+__host__ __device__ constexpr int wg_reg_units(int cn, int bnw, int wg) {
+  return (96 / (bnw / 2) - wg_fragments(cn, bnw, wg)) < wg_units(cn, wg) ? (96 / (bnw / 2) - wg_fragments(cn, bnw, wg))
+                                                                          : wg_units(cn, wg);
+}
+
+template <int CN, int BNW>
+struct WgColCfg {
+  static constexpr int kBox = 160 * CN * 2;                 // one {CN, 16, 10, 1} box, one plane
+  static constexpr int kKws = CN == 64 ? 1 : 3;             // kw columns per x stage
+  static constexpr int kXStage = 2 * kKws * kBox;           // [hi: kKws boxes][lo: kKws boxes]
+  static constexpr int kGTile = 128 * BNW * 2;              // gy tile, one plane
+  static constexpr int kGStage = 2 * kGTile;
+  static constexpr int kGStages = 2;
+  static constexpr int kXStagesRaw = (200 * 1024 - kGStages * kGStage) / kXStage;
+  static constexpr int kXStages = kXStagesRaw > 4 ? 4 : kXStagesRaw;
+  // accumulators in shared memory, [warpgroup 0's][warpgroup 1's], each [unit][BNW / 2][128 threads]
+  static constexpr int kSmemAcc0 = wg_units(CN, 0) - wg_reg_units(CN, BNW, 0);
+  static constexpr int kSmemAcc1 = wg_units(CN, 1) - wg_reg_units(CN, BNW, 1);
+  static constexpr int kAccBytes = (kSmemAcc0 + kSmemAcc1) * (BNW / 2) * 128 * 4;
+  static constexpr int kBytes = kXStages * kXStage + kGStages * kGStage + kAccBytes + 1024 /*align*/ + 256 /*barriers*/;
+  static_assert(wg_reg_units(CN, BNW, 0) >= 1 && wg_reg_units(CN, BNW, 1) >= 1, "column-box wgrad: register budget");
+  static_assert(kXStages * kKws >= 4, "column-box wgrad: the x ring must hold more than one tile's boxes");
+  static_assert(kBytes <= 227 * 1024, "column-box wgrad exceeds shared memory");
+};
+
+__device__ __forceinline__ void ring_next(int& s, uint32_t& ph, int stages) {
+  if (++s == stages) { s = 0; ph ^= 1; }
+}
+
+template <int R>
+__device__ __forceinline__ void add_fragment(float (&acc)[R], float (&part)[R]) {
+  fence_acc(part);
+#pragma unroll
+  for (int i = 0; i < R; ++i) { acc[i] += part[i]; part[i] = 0.f; }
+  fence_acc(part);
+}
+// the same fp32 adds into an accumulator in shared memory (element i at sacc[128 i])
+template <int R>
+__device__ __forceinline__ void add_fragment_smem(float* sacc, float (&part)[R]) {
+  fence_acc(part);
+#pragma unroll
+  for (int i = 0; i < R; ++i) { sacc[128 * i] += part[i]; part[i] = 0.f; }
+  fence_acc(part);
+}
+
+// consumer warpgroup WG: its units over the CTA's tiles, then its slice of the partial gw
+template <int CN, int BNW, int WG>
+__device__ __forceinline__ void wgrad_cols_consumer(uint8_t* smem, uint64_t* xfull, uint64_t* xempty, uint64_t* gfull,
+                                                    uint64_t* gempty, float* __restrict__ gw, const TcGeom& g, int t_begin,
+                                                    int t_end, int ci0, int co0, int warp, int lane) {
+  using C = WgColCfg<CN, BNW>;
+  constexpr int NU = wg_units(CN, WG), NP = wg_fragments(CN, BNW, WG), NR = wg_reg_units(CN, BNW, WG);
+  constexpr uint32_t la = swizzle_layout_for(CN), lb = swizzle_layout_for(BNW);
+  constexpr uint32_t sbo_a = 8 * CN * 2, sbo_b = 8 * BNW * 2;   // stride between 8-pixel groups (K)
+  constexpr uint32_t rows16 = 16 * CN * 2;                      // 16 pixel rows of x
+  const uint8_t* sg = smem + C::kXStages * C::kXStage;
+  // units NR .. NU - 1 accumulate in shared memory: this thread's element i of unit j at sacc[128 ((j - NR) BNW / 2 + i)]
+  float* sacc = reinterpret_cast<float*>(smem + C::kXStages * C::kXStage + C::kGStages * C::kGStage) +
+                (WG == 0 ? 0 : C::kSmemAcc0 * (BNW / 2) * 128) + (threadIdx.x & 127);
+  float acc[NR][BNW / 2], part[NP][BNW / 2];
+#pragma unroll
+  for (int u = 0; u < NR; ++u)
+#pragma unroll
+    for (int i = 0; i < BNW / 2; ++i) acc[u][i] = 0.f;
+#pragma unroll
+  for (int i = 0; i < (NU - NR) * (BNW / 2); ++i) sacc[128 * i] = 0.f;
+  // unit j's fragment goes into its accumulator, in registers or in shared memory
+  const auto add_unit = [&](int j, float (&p)[BNW / 2]) {
+    if (j < NR) add_fragment(acc[j < NR ? j : 0], p);
+    else add_fragment_smem(sacc + 128 * (j - NR) * (BNW / 2), p);
+  };
+  const auto acc_at = [&](int j, int i) { return j < NR ? acc[j < NR ? j : 0][i] : sacc[128 * ((j - NR) * (BNW / 2) + i)]; };
+#pragma unroll
+  for (int p = 0; p < NP; ++p)
+#pragma unroll
+    for (int i = 0; i < BNW / 2; ++i) part[p][i] = 0.f;
+  int xs = 0, gs = 0; uint32_t xph = 0, gph = 0;
+  for (int t = t_begin; t < t_end; ++t) {
+    mbar_wait(&gfull[gs], gph);
+    const uint32_t gb_hi = smem_u32(sg + gs * C::kGStage);
+    int prev_x = 0;
+#pragma unroll
+    for (int j = 0; j < NU; ++j) {
+      const WgUnit u = wg_unit(CN, WG, j);
+      const bool new_stage = j == 0 || u.kw / C::kKws != wg_unit(CN, WG, j - 1).kw / C::kKws;
+      if (new_stage && j > 0) {
+        if (NP == 1) { __syncwarp(); mbar_arrive_lane0(&xempty[xs], lane); }   // its MMAs completed at the last wait
+        prev_x = xs;
+        ring_next(xs, xph, C::kXStages);
+      }
+      if (new_stage) mbar_wait(&xfull[xs], xph);
+      uint32_t xa_hi = smem_u32(smem + xs * C::kXStage) + (u.kw % C::kKws) * C::kBox + u.kh * rows16, gb = gb_hi;
+      // per-unit descriptors: without this ptxas keeps every unit's 64-bit descriptors live over the tile and spills
+      asm volatile("" : "+r"(xa_hi), "+r"(gb));
+      const uint32_t lbo = u.along_kw ? (uint32_t)C::kBox : rows16;
+      const uint64_t dah = make_desc(xa_hi, lbo, sbo_a, la), dal = make_desc(xa_hi + C::kKws * C::kBox, lbo, sbo_a, la);
+      const uint64_t dbh = make_desc(gb, C::kGTile, sbo_b, lb), dbl = make_desc(gb + C::kGTile, C::kGTile, sbo_b, lb);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 128 / 16; ++ks) {          // 16 pixels per MMA
+        const uint32_t offa = ks * 2 * sbo_a, offb = ks * 2 * sbo_b;
+        Wgmma<BNW>::template mma<1, 1>(part[j % NP], desc_add(dal, offa), desc_add(dbh, offb));
+        Wgmma<BNW>::template mma<1, 1>(part[j % NP], desc_add(dah, offa), desc_add(dbl, offb));
+        Wgmma<BNW>::template mma<1, 1>(part[j % NP], desc_add(dah, offa), desc_add(dbh, offb));
+      }
+      wgmma_commit();
+      if (NP == 2) {
+        wgmma_wait<1>();                                // unit j - 1 has completed
+        if (j > 0) {
+          add_unit(j - 1, part[(j - 1) % NP]);
+          if (new_stage) { __syncwarp(); mbar_arrive_lane0(&xempty[prev_x], lane); }
+        }
+      } else {
+        wgmma_wait<0>();
+        add_unit(j, part[0]);
+      }
+    }
+    if (NP == 2) {
+      wgmma_wait<0>();
+      add_unit(NU - 1, part[(NU - 1) % NP]);
+    }
+    __syncwarp();
+    mbar_arrive_lane0(&xempty[xs], lane);
+    ring_next(xs, xph, C::kXStages);
+    mbar_arrive_lane0(&gempty[gs], lane);
+    ring_next(gs, gph, C::kGStages);
+  }
+  if (t_begin >= t_end) return;
+  // accumulator row m of unit u = slot m / CN (a tap or padding), input channel m % CN; column = output channel
+  const int quad = lane & 3;
+#pragma unroll
+  for (int j = 0; j < NU; ++j) {
+    const WgUnit u = wg_unit(CN, WG, j);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int m = (warp & 3) * 16 + (lane >> 2) + 8 * i;
+      const int q = m / CN, ci = ci0 + m % CN;
+      if (q >= u.n) continue;
+      const int tap = 3 * (u.kh + (u.along_kw ? 0 : q)) + u.kw + (u.along_kw ? q : 0);
+      // the pixel-split partial buffer: slice blockIdx.x, summed over the splits in order by add_partials
+      float* dst = gw + (int64_t)blockIdx.x * 9 * g.Cin * g.Cout + ((int64_t)tap * g.Cin + ci) * g.Cout + co0 + 2 * quad;
+#pragma unroll
+      for (int k = 0; k < BNW / 8; ++k)
+        *reinterpret_cast<float2*>(dst + 8 * k) = make_float2(acc_at(j, 4 * k + 2 * i), acc_at(j, 4 * k + 2 * i + 1));
+    }
+  }
+}
+
+template <int CN, int BNW>
+__global__ void __launch_bounds__(kThreads, 1) k_conv_wgrad_cols_wgmma(const __grid_constant__ CUtensorMap tm_g_hi,
+                                                                       const __grid_constant__ CUtensorMap tm_g_lo,
+                                                                       const __grid_constant__ CUtensorMap tm_x_hi,
+                                                                       const __grid_constant__ CUtensorMap tm_x_lo,
+                                                                       float* __restrict__ gw, TcGeom g, int tiles_per_cta) {
+  using C = WgColCfg<CN, BNW>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  // x ring, gy ring [hi][lo], accumulators in shared memory, barriers
+  uint8_t* sg = smem + C::kXStages * C::kXStage;
+  uint64_t* xfull = reinterpret_cast<uint64_t*>(sg + C::kGStages * C::kGStage + C::kAccBytes);   // [kXStages]
+  uint64_t* xempty = xfull + C::kXStages;                                         // [kXStages]
+  uint64_t* gfull = xempty + C::kXStages;                                         // [kGStages]
+  uint64_t* gempty = gfull + C::kGStages;                                         // [kGStages]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int co0 = blockIdx.y * BNW;
+  const int ci0 = blockIdx.z * CN;
+  const int total_tiles = g.tiles_w * g.tiles_h * g.tiles_n;
+  const int t_begin = blockIdx.x * tiles_per_cta;
+  const int t_end = min(total_tiles, t_begin + tiles_per_cta);
+
+  if (warp == kConsumerWarps && lane == 0) {
+    prefetch_tmap(&tm_g_hi); prefetch_tmap(&tm_g_lo); prefetch_tmap(&tm_x_hi); prefetch_tmap(&tm_x_lo);
+    for (int s = 0; s < C::kXStages; ++s) { mbar_init(&xfull[s], 1); mbar_init(&xempty[s], kConsumerWarps); }
+    for (int s = 0; s < C::kGStages; ++s) { mbar_init(&gfull[s], 1); mbar_init(&gempty[s], kConsumerWarps); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp == kConsumerWarps) {
+    if (lane == 0) {
+      int xs = 0, gs = 0; uint32_t xph = 0, gph = 0;
+      for (int t = t_begin; t < t_end; ++t) {
+        const int tw_i = t % g.tiles_w, th_i = (t / g.tiles_w) % g.tiles_h, n0 = t / (g.tiles_w * g.tiles_h);
+        const int w0 = tw_i * 16, h0 = th_i * 8;
+        mbar_wait(&gempty[gs], gph ^ 1);
+        mbar_expect_tx(&gfull[gs], C::kGStage);
+        tma_load_4d(&tm_g_hi, &gfull[gs], sg + gs * C::kGStage, co0, w0, h0, n0);
+        tma_load_4d(&tm_g_lo, &gfull[gs], sg + gs * C::kGStage + C::kGTile, co0, w0, h0, n0);
+        ring_next(gs, gph, C::kGStages);
+        for (int kw0 = 0; kw0 < 3; kw0 += C::kKws) {
+          mbar_wait(&xempty[xs], xph ^ 1);
+          mbar_expect_tx(&xfull[xs], C::kXStage);
+          uint8_t* sx = smem + xs * C::kXStage;
+          for (int b = 0; b < C::kKws; ++b) {
+            const int kw = kw0 + b;
+            tma_load_4d(&tm_x_hi, &xfull[xs], sx + b * C::kBox, ci0, w0 + kw - 1, h0 - 1, n0);
+            tma_load_4d(&tm_x_lo, &xfull[xs], sx + (C::kKws + b) * C::kBox, ci0, w0 + kw - 1, h0 - 1, n0);
+          }
+          ring_next(xs, xph, C::kXStages);
+        }
+      }
+    }
+    return;
+  }
+  if (warp < 4)
+    wgrad_cols_consumer<CN, BNW, 0>(smem, xfull, xempty, gfull, gempty, gw, g, t_begin, t_end, ci0, co0, warp, lane);
+  else
+    wgrad_cols_consumer<CN, BNW, 1>(smem, xfull, xempty, gfull, gempty, gw, g, t_begin, t_end, ci0, co0, warp, lane);
+}
+
 // ----------------------------------------------------------------------------------------------------
 // host side
 // ----------------------------------------------------------------------------------------------------
@@ -975,14 +1243,15 @@ int conv_fwd_tc_planes(const void* a_planes, const void* w_planes, float* y, int
   return fail(TWG_ERR_UNSUPPORTED, "tensor-core conv: no kernel for CC=%d BN=%d", CC, BN);
 }
 
-template <int CN, int BNW>
+// kCols: the column-box kernel (xh / xl with the box {CN, 16, 10, 1}); both kernels take the same grid and pixel split
+template <int CN, int BNW, bool kCols>
 static int launch_wgrad(const CUtensorMap& gh, const CUtensorMap& gl, const CUtensorMap& xh, const CUtensorMap& xl,
                         float* gw, const TcGeom& g, cudaStream_t st) {
-  using C = WgCfg<CN, BNW>;
-  auto kern = k_conv_wgrad_wgmma<CN, BNW>;
+  constexpr int kBytes = kCols ? WgColCfg<CN, BNW>::kBytes : WgCfg<CN, BNW>::kBytes;
+  auto kern = kCols ? k_conv_wgrad_cols_wgmma<CN, BNW> : k_conv_wgrad_wgmma<CN, BNW>;
   static std::once_flag once;                 // one-time attribute set-up, safe from several host threads
   static cudaError_t attr_err = cudaSuccess;
-  std::call_once(once, [&] { attr_err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kBytes); });
+  std::call_once(once, [&] { attr_err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kBytes); });
   if (attr_err != cudaSuccess) return fail(TWG_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(attr_err));
   const int total_tiles = g.tiles_w * g.tiles_h * g.tiles_n;
   const int yb = g.Cout / BNW, zb = g.Cin / CN;
@@ -996,8 +1265,8 @@ static int launch_wgrad(const CUtensorMap& gh, const CUtensorMap& gl, const CUte
   const int64_t gw_elems = (int64_t)g.k * g.k * g.Cin * g.Cout;
   float* parts = partials(xb * gw_elems, true, st);
   if (!parts) return fail(TWG_ERR_UNSUPPORTED, "tensor-core wgrad: weight too large for the split buffer");
-  kern<<<grid, kThreads, C::kBytes, st>>>(gh, gl, xh, xl, parts, g, tiles_per_cta);
-  if (int rc = check_launch("twg_conv_wgrad tc")) return rc;
+  kern<<<grid, kThreads, kBytes, st>>>(gh, gl, xh, xl, parts, g, tiles_per_cta);
+  if (int rc = check_launch(kCols ? "twg_conv_wgrad tc cols" : "twg_conv_wgrad tc")) return rc;
   return add_partials(gw, parts, xb, gw_elems, st);
 }
 
@@ -1019,14 +1288,18 @@ int conv_wgrad_tc_planes(const void* x_planes, const void* g_planes, float* gw, 
   // output-channel block (N of the MMA): 64 channels, 32 for 64-channel chunks, whose five tap groups of accumulators
   // would not fit in registers at 64
   const int BNW = (Cout >= 64 && CN < 64) ? 64 : (Cout >= 32 ? 32 : Cout);
+  // 3x3 SAME on 16 x 8 tiles inside one image takes the column-box kernel (same results, a third of the x traffic)
+  const bool cols = k == 3 && pad == 1 && g.TW == 16 && g.TH == 8 && g.TN == 1 && H >= 10;
   CUtensorMap gh, gl, xh, xl;
   int rc;
   if ((rc = make_act_map(&gh, g_hi, N, H, W, Cout, BNW, g.TW, g.TH, g.TN))) return rc;
   if ((rc = make_act_map(&gl, g_lo, N, H, W, Cout, BNW, g.TW, g.TH, g.TN))) return rc;
-  if ((rc = make_act_map(&xh, x_hi, N, H, W, Cin, CN, g.TW, g.TH, g.TN))) return rc;
-  if ((rc = make_act_map(&xl, x_lo, N, H, W, Cin, CN, g.TW, g.TH, g.TN))) return rc;
-#define TWG_WG_CASE(cn, bn) \
-  if (CN == cn && BNW == bn) return launch_wgrad<cn, bn>(gh, gl, xh, xl, gw, g, st);
+  if ((rc = make_act_map(&xh, x_hi, N, H, W, Cin, CN, g.TW, cols ? 10 : g.TH, g.TN))) return rc;
+  if ((rc = make_act_map(&xl, x_lo, N, H, W, Cin, CN, g.TW, cols ? 10 : g.TH, g.TN))) return rc;
+#define TWG_WG_CASE(cn, bn)                                                                     \
+  if (CN == cn && BNW == bn)                                                                    \
+    return cols ? launch_wgrad<cn, bn, true>(gh, gl, xh, xl, gw, g, st)                         \
+                : launch_wgrad<cn, bn, false>(gh, gl, xh, xl, gw, g, st);
   TWG_WG_CASE(16, 16) TWG_WG_CASE(16, 32) TWG_WG_CASE(16, 64)
   TWG_WG_CASE(32, 16) TWG_WG_CASE(32, 32) TWG_WG_CASE(32, 64)
   TWG_WG_CASE(64, 16) TWG_WG_CASE(64, 32)
