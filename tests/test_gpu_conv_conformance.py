@@ -9,8 +9,9 @@
 import pytest
 import torch
 
+from tests import product_launches
 from tests.parity import _log_result, conv_error_ratio, tc_elem_c
-from tests.product_launches import harvest_product_launches
+from tests.product_launches import harvest_product_launches, key_configs
 from tests.test_gpu_kernels import CONV_SHAPES, conv_refs, _dev, _rand
 
 pytestmark = pytest.mark.gpu
@@ -252,126 +253,324 @@ def test_tensor_core_fwd_and_dgrad_are_per_sample(built_lib, shape):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# the batch-dependent host rules of the conv launchers (twg_conv_tc.cu, twg_conv_simt.cu, twg_conv_pw.cu), restated
+# ---------------------------------------------------------------------------------------------------------------------
+NUM_SMS = 132            # kNumSMs of twg_common.cuh
+
+
+def _cdiv(a, b):
+  return -(-a // b)
+
+
+def _pow2_le(v):
+  p = 1
+  while p * 2 <= v:
+    p *= 2
+  return p
+
+
+def pick_tile(N, H, W):
+  """(TW, TH, TN, tiles_w, tiles_h, tiles_n) of pick_tile: a 128-pixel tile of TN images of TH x TW pixels."""
+  TW = _pow2_le(min(W, 16))
+  TH = _pow2_le(min(H, 128 // TW))
+  TN = 128 // (TW * TH)
+  return TW, TH, TN, _cdiv(W, TW), _cdiv(H, TH), _cdiv(N, TN)
+
+
+def tc_ragged(N, H, W):
+  """The last batch tile of a tensor-core conv holds fewer than TN images."""
+  TN = pick_tile(N, H, W)[2]
+  return TN > 1 and N % TN != 0
+
+
+def _chunk_for(c):
+  return 64 if c % 64 == 0 else (32 if c % 32 == 0 else (16 if c % 16 == 0 else 0))
+
+
+def tc_wgrad_grid(N, H, W, Cin, Cout, k, pad):
+  """launch_wgrad's pixel split: {tiles_per_cta, ctas (xb), last_cta_tiles, total_tiles, cols}.  The CTAs of one
+  channel block take consecutive runs of tiles_per_cta tiles; the last run is cut short by total_tiles when
+  last_cta_tiles < tiles_per_cta."""
+  TW, TH, TN, tw, th, tn = pick_tile(N, H, W)
+  CN = _chunk_for(Cin)
+  BNW = 64 if (Cout >= 64 and CN < 64) else (32 if Cout >= 32 else Cout)
+  total = tw * th * tn
+  want = max(1, min(NUM_SMS // ((Cout // BNW) * (Cin // CN)), total))
+  per = _cdiv(total, want)
+  xb = _cdiv(total, per)
+  return {'tiles_per_cta': per, 'ctas': xb, 'last_cta_tiles': total - (xb - 1) * per, 'total_tiles': total,
+          'cols': k == 3 and pad == 1 and TW == 16 and TH == 8 and TN == 1 and H >= 10}
+
+
+def simt_wgrad_splits(N, H, W, Cin, Cout, k, pad):
+  """(splits, pixels per split) of conv_wgrad_simt."""
+  M = N * (H + 2 * pad - k + 1) * (W + 2 * pad - k + 1)
+  tiles = k * k * _cdiv(Cin, 16 if Cin <= 16 else 64) * _cdiv(Cout, 16 if Cout <= 16 else 64)
+  splits = max(1, min(_cdiv(4 * NUM_SMS, tiles), _cdiv(M, 64)))
+  mps = _cdiv(_cdiv(M, splits), 16) * 16
+  return _cdiv(M, mps), mps
+
+
+def pw_wgrad_blocks(N, H, W, Cin, Cout):
+  """(blocks, pixels per block) of pw_wgrad: the wide side L = max(Cin, Cout) gives G = min(L / 4, 32) threads a pixel."""
+  P = N * H * W
+  G = min(max(Cin, Cout) // 4, 32)
+  blocks = min(_cdiv(P, (256 // G) * 16), 4 * NUM_SMS)
+  chunk = _cdiv(P, blocks)
+  return _cdiv(P, chunk), chunk
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # coverage audit
 # ---------------------------------------------------------------------------------------------------------------------
 # argument positions of the geometry (N, H, W, Cin, Cout, k, pad) in each conv entry point
 _GEOM_AT = {'twg_conv_fwd': 3, 'twg_conv_dgrad': 3, 'twg_conv_wgrad': 3, 'twg_conv_fwd_planes': 8,
             'twg_conv_affine_act_fwd_planes': 7, 'twg_conv_dgrad_planes': 3, 'twg_conv_wgrad_planes': 3}
+WGRAD_ENTRIES = ('twg_conv_wgrad', 'twg_conv_wgrad_planes')
+_TC_ENTRIES = ('twg_conv_fwd_planes', 'twg_conv_affine_act_fwd_planes', 'twg_conv_dgrad_planes')
 
 
 def conv_key(name, args):
-  """(entry, H, W, Cin, Cout, k, pad, options) of one conv launch; N is not part of it."""
+  """(entry, [N,] H, W, Cin, Cout, k, pad, options) of one conv launch.  The weight gradients carry N: it sets their
+  pixel split (the summation order, and whether the last CTA is short) and whether the last batch tile is ragged.  The
+  tensor-core forward, dgrad and affine forward carry 'ragged' when their last batch tile is; their per-sample arithmetic
+  does not depend on N otherwise (test_tensor_core_fwd_and_dgrad_are_per_sample).  The exact-fp32 forward and dgrad the
+  product launches are the pointwise kernels, one output pixel at a time."""
   i = _GEOM_AT[name]
   geom = tuple(int(v) for v in args[i + 1:i + 7])
+  N = int(args[i])
   opts = []
-  if name in ('twg_conv_wgrad', 'twg_conv_wgrad_planes') and args[i + 7]:
+  if name in WGRAD_ENTRIES and args[i + 7]:
     opts.append('accumulate')
   if name == 'twg_conv_fwd_planes':
     opts += [o for o, v in (('bias', args[2]), ('act', args[3]), ('zp', args[5]), ('mask', args[6]), ('stats', args[7])) if v]
   if name == 'twg_conv_affine_act_fwd_planes':
     opts += ['flags%d' % int(args[4])] + [o for o, v in (('z', args[5]), ('zp', args[6])) if v]
-  return (name,) + geom + ('+'.join(opts),)
+  if name in _TC_ENTRIES and tc_ragged(N, geom[0], geom[1]):
+    opts.append('ragged')
+  return (name,) + ((N,) if name in WGRAD_ENTRIES else ()) + geom + ('+'.join(opts),)
 
 
-def suite_keys():
+def _with_ragged(opts, N, H, W):
+  return '+'.join(filter(None, (opts, 'ragged' if tc_ragged(N, H, W) else '')))
+
+
+def kernel_suite_keys():
   """The keys the kernel suite runs: test_conv_fwd_dgrad_wgrad at both precisions (with the accumulate check), the
   epilogue matrix and the affine-epilogue test."""
   from twingan_b200 import ops
   keys = set()
   for N, H, W, Cin, Cout, k, pad in CONV_SHAPES:
     g = (H, W, Cin, Cout, k, pad)
-    keys |= {('twg_conv_fwd',) + g + ('',), ('twg_conv_dgrad',) + g + ('',), ('twg_conv_wgrad',) + g + ('',),
-             ('twg_conv_wgrad',) + g + ('accumulate',)}
+    keys |= {('twg_conv_fwd',) + g + ('',), ('twg_conv_dgrad',) + g + ('',), ('twg_conv_wgrad', N) + g + ('',),
+             ('twg_conv_wgrad', N) + g + ('accumulate',)}
     if ops.conv_path(N, H, W, Cin, Cout, k, pad) == ops.CONV_TC:
-      keys |= {('twg_conv_fwd_planes',) + g + ('',), ('twg_conv_dgrad_planes',) + g + ('',),
-               ('twg_conv_wgrad_planes',) + g + ('',), ('twg_conv_wgrad_planes',) + g + ('accumulate',)}
+      keys |= {('twg_conv_fwd_planes',) + g + (_with_ragged('', N, H, W),),
+               ('twg_conv_dgrad_planes',) + g + (_with_ragged('', N, H, W),),
+               ('twg_conv_wgrad_planes', N) + g + ('',), ('twg_conv_wgrad_planes', N) + g + ('accumulate',)}
   for N, H, W, Cin, Cout, k, pad in EPI_SHAPES:
     fused = ops._epilogue_slots(N, H, W, Cin, Cout, k, pad) > 0
     for opts in _all_option_sets():
       if expected_rc(opts, fused)[0] == 0:
-        keys.add(('twg_conv_fwd_planes', H, W, Cin, Cout, k, pad, '+'.join(opts)))
+        keys.add(('twg_conv_fwd_planes', H, W, Cin, Cout, k, pad, _with_ragged('+'.join(opts), N, H, W)))
   for N, H, W, Cin, Cout in AFFINE_SHAPES:
     for flags in range(4):
       for outs in ('z', 'z+zp', 'zp'):
-        keys.add(('twg_conv_affine_act_fwd_planes', H, W, Cin, Cout, 3, 1, 'flags%d+%s' % (flags, outs)))
+        keys.add(('twg_conv_affine_act_fwd_planes', H, W, Cin, Cout, 3, 1,
+                  _with_ragged('flags%d+%s' % (flags, outs), N, H, W)))
   return keys
+
+
+def suite_keys():
+  """The keys of the kernel suite and of the product-batch cases of test_gpu_conv_batch.py."""
+  from tests.test_gpu_conv_batch import BATCH_CONV_CASES
+  return kernel_suite_keys() | {key for key, _ in BATCH_CONV_CASES}
 
 
 def harvest_product_convs():
   """The keys of every conv launch in the shared harvest of the product (tests/product_launches.py)."""
-  return {conv_key(name, args) for name, args in harvest_product_launches() if name in _GEOM_AT}
+  return conv_keys(harvest_product_launches())
+
+
+def conv_keys(launches):
+  return {conv_key(name, args) for name, args in launches if name in _GEOM_AT}
 
 
 # The conv launches of the product, harvested by harvest_product_convs.  A change that adds, removes or re-dispatches a conv
 # must update this set and, for each new key, add a case to the kernel suite.
 PRODUCT_CONVS = {
     'twg_conv_affine_act_fwd_planes': [
-        (128, 128, 32, 32, 3, 1, 'flags3+z'), (128, 128, 32, 32, 3, 1, 'flags3+zp'), (128, 128, 32, 64, 3, 1,
-        'flags3+z'), (256, 256, 16, 16, 3, 1, 'flags3+z'), (256, 256, 16, 16, 3, 1, 'flags3+zp'), (256, 256, 16,
-        32, 3, 1, 'flags3+z'), (256, 256, 64, 16, 3, 1, 'flags3+zp')],
+        (128, 128, 32, 32, 3, 1, 'flags3+z'), (128, 128, 32, 32, 3, 1, 'flags3+zp'), (128, 128, 32, 64, 3, 1, 'flags3+z'),
+        (256, 256, 16, 16, 3, 1, 'flags3+z'), (256, 256, 16, 16, 3, 1, 'flags3+zp'), (256, 256, 16, 32, 3, 1, 'flags3+z'),
+        (256, 256, 64, 16, 3, 1, 'flags3+zp')],
     'twg_conv_dgrad': [
-        (1, 1, 256, 1, 1, 0, ''), (4, 4, 3, 256, 1, 0, ''), (4, 4, 256, 3, 1, 0, ''), (8, 8, 3, 256, 1, 0, ''),
-        (8, 8, 256, 3, 1, 0, ''), (16, 16, 3, 256, 1, 0, ''), (16, 16, 256, 3, 1, 0, ''), (32, 32, 3, 128, 1, 0,
-        ''), (32, 32, 128, 3, 1, 0, ''), (64, 64, 3, 64, 1, 0, ''), (64, 64, 64, 3, 1, 0, ''), (128, 128, 3, 32,
-        1, 0, ''), (128, 128, 32, 3, 1, 0, ''), (256, 256, 3, 16, 1, 0, ''), (256, 256, 16, 3, 1, 0, '')],
+        (1, 1, 256, 1, 1, 0, ''), (128, 128, 3, 32, 1, 0, ''), (128, 128, 32, 3, 1, 0, ''), (16, 16, 256, 3, 1, 0, ''), (16,
+        16, 3, 256, 1, 0, ''), (256, 256, 16, 3, 1, 0, ''), (256, 256, 3, 16, 1, 0, ''), (32, 32, 128, 3, 1, 0, ''), (32,
+        32, 3, 128, 1, 0, ''), (4, 4, 256, 3, 1, 0, ''), (4, 4, 3, 256, 1, 0, ''), (64, 64, 3, 64, 1, 0, ''), (64, 64, 64,
+        3, 1, 0, ''), (8, 8, 256, 3, 1, 0, ''), (8, 8, 3, 256, 1, 0, '')],
     'twg_conv_dgrad_planes': [
-        (1, 1, 4096, 256, 1, 0, ''), (4, 4, 256, 256, 3, 1, ''), (4, 4, 384, 256, 3, 1, ''), (8, 8, 256, 256, 3,
-        1, ''), (8, 8, 512, 256, 1, 0, ''), (8, 8, 512, 256, 3, 1, ''), (16, 16, 256, 256, 3, 1, ''), (16, 16,
-        512, 256, 1, 0, ''), (16, 16, 512, 256, 3, 1, ''), (32, 32, 128, 128, 3, 1, ''), (32, 32, 128, 256, 1,
-        0, ''), (32, 32, 128, 256, 3, 1, ''), (32, 32, 512, 128, 1, 0, ''), (32, 32, 512, 128, 3, 1, ''), (64,
-        64, 64, 64, 3, 1, ''), (64, 64, 64, 128, 1, 0, ''), (64, 64, 64, 128, 3, 1, ''), (64, 64, 256, 64, 1, 0,
-        ''), (64, 64, 256, 64, 3, 1, ''), (128, 128, 32, 32, 3, 1, ''), (128, 128, 32, 64, 1, 0, ''), (128, 128,
-        32, 64, 3, 1, ''), (128, 128, 128, 32, 1, 0, ''), (128, 128, 128, 32, 3, 1, ''), (256, 256, 16, 16, 3,
-        1, ''), (256, 256, 16, 32, 1, 0, ''), (256, 256, 16, 32, 3, 1, ''), (256, 256, 64, 16, 1, 0, ''), (256,
-        256, 64, 16, 3, 1, '')],
+        (1, 1, 4096, 256, 1, 0, 'ragged'), (128, 128, 128, 32, 1, 0, ''), (128, 128, 128, 32, 3, 1, ''), (128, 128, 32, 32,
+        3, 1, ''), (128, 128, 32, 64, 1, 0, ''), (128, 128, 32, 64, 3, 1, ''), (16, 16, 256, 256, 3, 1, ''), (16, 16, 512,
+        256, 1, 0, ''), (16, 16, 512, 256, 3, 1, ''), (256, 256, 16, 16, 3, 1, ''), (256, 256, 16, 32, 1, 0, ''), (256, 256,
+        16, 32, 3, 1, ''), (256, 256, 64, 16, 1, 0, ''), (256, 256, 64, 16, 3, 1, ''), (32, 32, 128, 128, 3, 1, ''), (32,
+        32, 128, 256, 1, 0, ''), (32, 32, 128, 256, 3, 1, ''), (32, 32, 512, 128, 1, 0, ''), (32, 32, 512, 128, 3, 1, ''),
+        (4, 4, 256, 256, 3, 1, ''), (4, 4, 256, 256, 3, 1, 'ragged'), (4, 4, 384, 256, 3, 1, ''), (4, 4, 384, 256, 3, 1,
+        'ragged'), (64, 64, 256, 64, 1, 0, ''), (64, 64, 256, 64, 3, 1, ''), (64, 64, 64, 128, 1, 0, ''), (64, 64, 64, 128,
+        3, 1, ''), (64, 64, 64, 64, 3, 1, ''), (8, 8, 256, 256, 3, 1, ''), (8, 8, 256, 256, 3, 1, 'ragged'), (8, 8, 512,
+        256, 1, 0, ''), (8, 8, 512, 256, 3, 1, '')],
     'twg_conv_fwd': [
-        (1, 1, 256, 1, 1, 0, ''), (4, 4, 3, 256, 1, 0, ''), (4, 4, 256, 3, 1, 0, ''), (8, 8, 3, 256, 1, 0, ''),
-        (8, 8, 256, 3, 1, 0, ''), (16, 16, 3, 256, 1, 0, ''), (16, 16, 256, 3, 1, 0, ''), (32, 32, 3, 128, 1, 0,
-        ''), (32, 32, 128, 3, 1, 0, ''), (64, 64, 3, 64, 1, 0, ''), (64, 64, 64, 3, 1, 0, ''), (128, 128, 3, 32,
-        1, 0, ''), (128, 128, 32, 3, 1, 0, ''), (256, 256, 3, 16, 1, 0, ''), (256, 256, 16, 3, 1, 0, '')],
+        (1, 1, 256, 1, 1, 0, ''), (128, 128, 3, 32, 1, 0, ''), (128, 128, 32, 3, 1, 0, ''), (16, 16, 256, 3, 1, 0, ''), (16,
+        16, 3, 256, 1, 0, ''), (256, 256, 16, 3, 1, 0, ''), (256, 256, 3, 16, 1, 0, ''), (32, 32, 128, 3, 1, 0, ''), (32,
+        32, 3, 128, 1, 0, ''), (4, 4, 256, 3, 1, 0, ''), (4, 4, 3, 256, 1, 0, ''), (64, 64, 3, 64, 1, 0, ''), (64, 64, 64,
+        3, 1, 0, ''), (8, 8, 256, 3, 1, 0, ''), (8, 8, 3, 256, 1, 0, '')],
     'twg_conv_fwd_planes': [
-        (1, 1, 4096, 256, 1, 0, ''), (4, 4, 256, 256, 3, 1, ''), (4, 4, 384, 256, 3, 1, ''), (8, 8, 256, 256, 3,
-        1, ''), (8, 8, 512, 256, 1, 0, ''), (8, 8, 512, 256, 3, 1, ''), (16, 16, 256, 256, 3, 1, ''), (16, 16,
-        512, 256, 1, 0, 'bias'), (16, 16, 512, 256, 3, 1, ''), (32, 32, 128, 128, 3, 1, ''), (32, 32, 128, 128,
-        3, 1, 'bias+act+zp'), (32, 32, 128, 256, 1, 0, ''), (32, 32, 128, 256, 1, 0, 'bias'), (32, 32, 128, 256,
-        3, 1, ''), (32, 32, 128, 256, 3, 1, 'bias+act'), (32, 32, 512, 128, 1, 0, 'bias'), (32, 32, 512, 128, 3,
-        1, ''), (64, 64, 64, 64, 3, 1, ''), (64, 64, 64, 64, 3, 1, 'bias+act+zp'), (64, 64, 64, 128, 1, 0, ''),
-        (64, 64, 64, 128, 1, 0, 'bias'), (64, 64, 64, 128, 3, 1, ''), (64, 64, 64, 128, 3, 1, 'bias+act'), (64,
-        64, 256, 64, 1, 0, 'bias'), (64, 64, 256, 64, 3, 1, ''), (128, 128, 32, 32, 3, 1, ''), (128, 128, 32,
-        32, 3, 1, 'bias+act+zp+mask'), (128, 128, 32, 32, 3, 1, 'stats'), (128, 128, 32, 64, 1, 0, ''), (128,
-        128, 32, 64, 1, 0, 'bias'), (128, 128, 32, 64, 3, 1, ''), (128, 128, 32, 64, 3, 1, 'bias+act+mask'),
-        (128, 128, 32, 64, 3, 1, 'stats'), (128, 128, 128, 32, 1, 0, 'bias'), (128, 128, 128, 32, 3, 1, ''),
-        (256, 256, 16, 16, 3, 1, ''), (256, 256, 16, 16, 3, 1, 'bias+act+zp+mask'), (256, 256, 16, 16, 3, 1,
-        'stats'), (256, 256, 16, 32, 1, 0, ''), (256, 256, 16, 32, 1, 0, 'bias'), (256, 256, 16, 32, 3, 1, ''),
-        (256, 256, 16, 32, 3, 1, 'bias+act+mask'), (256, 256, 16, 32, 3, 1, 'stats'), (256, 256, 64, 16, 1, 0,
-        'bias'), (256, 256, 64, 16, 3, 1, ''), (256, 256, 64, 16, 3, 1, 'stats')],
+        (1, 1, 4096, 256, 1, 0, 'ragged'), (128, 128, 128, 32, 1, 0, 'bias'), (128, 128, 128, 32, 3, 1, ''), (128, 128, 32,
+        32, 3, 1, ''), (128, 128, 32, 32, 3, 1, 'bias+act+zp+mask'), (128, 128, 32, 32, 3, 1, 'stats'), (128, 128, 32, 64,
+        1, 0, ''), (128, 128, 32, 64, 1, 0, 'bias'), (128, 128, 32, 64, 3, 1, ''), (128, 128, 32, 64, 3, 1,
+        'bias+act+mask'), (128, 128, 32, 64, 3, 1, 'stats'), (16, 16, 256, 256, 3, 1, ''), (16, 16, 512, 256, 1, 0, ''),
+        (16, 16, 512, 256, 1, 0, 'bias'), (16, 16, 512, 256, 3, 1, ''), (256, 256, 16, 16, 3, 1, ''), (256, 256, 16, 16, 3,
+        1, 'bias+act+zp+mask'), (256, 256, 16, 16, 3, 1, 'stats'), (256, 256, 16, 32, 1, 0, ''), (256, 256, 16, 32, 1, 0,
+        'bias'), (256, 256, 16, 32, 3, 1, ''), (256, 256, 16, 32, 3, 1, 'bias+act+mask'), (256, 256, 16, 32, 3, 1, 'stats'),
+        (256, 256, 64, 16, 1, 0, 'bias'), (256, 256, 64, 16, 3, 1, ''), (256, 256, 64, 16, 3, 1, 'stats'), (32, 32, 128,
+        128, 3, 1, ''), (32, 32, 128, 128, 3, 1, 'bias+act+zp'), (32, 32, 128, 256, 1, 0, ''), (32, 32, 128, 256, 1, 0,
+        'bias'), (32, 32, 128, 256, 3, 1, ''), (32, 32, 128, 256, 3, 1, 'bias+act'), (32, 32, 512, 128, 1, 0, ''), (32, 32,
+        512, 128, 1, 0, 'bias'), (32, 32, 512, 128, 3, 1, ''), (4, 4, 256, 256, 3, 1, ''), (4, 4, 256, 256, 3, 1, 'ragged'),
+        (4, 4, 384, 256, 3, 1, ''), (4, 4, 384, 256, 3, 1, 'ragged'), (64, 64, 256, 64, 1, 0, 'bias'), (64, 64, 256, 64, 3,
+        1, ''), (64, 64, 64, 128, 1, 0, ''), (64, 64, 64, 128, 1, 0, 'bias'), (64, 64, 64, 128, 3, 1, ''), (64, 64, 64, 128,
+        3, 1, 'bias+act'), (64, 64, 64, 64, 3, 1, ''), (64, 64, 64, 64, 3, 1, 'bias+act+zp'), (8, 8, 256, 256, 3, 1, ''),
+        (8, 8, 256, 256, 3, 1, 'ragged'), (8, 8, 512, 256, 1, 0, ''), (8, 8, 512, 256, 3, 1, ''), (8, 8, 512, 256, 3, 1,
+        'ragged')],
     'twg_conv_wgrad': [
-        (1, 1, 256, 1, 1, 0, 'accumulate'), (4, 4, 3, 256, 1, 0, 'accumulate'), (4, 4, 256, 3, 1, 0,
-        'accumulate'), (8, 8, 3, 256, 1, 0, 'accumulate'), (8, 8, 256, 3, 1, 0, 'accumulate'), (16, 16, 3, 256,
-        1, 0, 'accumulate'), (16, 16, 256, 3, 1, 0, 'accumulate'), (32, 32, 3, 128, 1, 0, 'accumulate'), (32,
-        32, 128, 3, 1, 0, 'accumulate'), (64, 64, 3, 64, 1, 0, 'accumulate'), (64, 64, 64, 3, 1, 0,
-        'accumulate'), (128, 128, 3, 32, 1, 0, 'accumulate'), (128, 128, 32, 3, 1, 0, 'accumulate'), (256, 256,
-        3, 16, 1, 0, 'accumulate'), (256, 256, 16, 3, 1, 0, 'accumulate')],
+        (12, 1, 1, 256, 1, 1, 0, 'accumulate'), (12, 128, 128, 3, 32, 1, 0, 'accumulate'), (12, 128, 128, 32, 3, 1, 0,
+        'accumulate'), (12, 256, 256, 16, 3, 1, 0, 'accumulate'), (12, 256, 256, 3, 16, 1, 0, 'accumulate'), (12, 32, 32, 3,
+        128, 1, 0, 'accumulate'), (12, 64, 64, 3, 64, 1, 0, 'accumulate'), (16, 1, 1, 256, 1, 1, 0, 'accumulate'), (16, 128,
+        128, 3, 32, 1, 0, 'accumulate'), (16, 128, 128, 32, 3, 1, 0, 'accumulate'), (16, 16, 16, 3, 256, 1, 0,
+        'accumulate'), (16, 256, 256, 16, 3, 1, 0, 'accumulate'), (16, 256, 256, 3, 16, 1, 0, 'accumulate'), (16, 32, 32,
+        128, 3, 1, 0, 'accumulate'), (16, 32, 32, 3, 128, 1, 0, 'accumulate'), (16, 4, 4, 3, 256, 1, 0, 'accumulate'), (16,
+        64, 64, 3, 64, 1, 0, 'accumulate'), (16, 64, 64, 64, 3, 1, 0, 'accumulate'), (16, 8, 8, 3, 256, 1, 0, 'accumulate'),
+        (24, 1, 1, 256, 1, 1, 0, 'accumulate'), (24, 128, 128, 3, 32, 1, 0, 'accumulate'), (24, 16, 16, 3, 256, 1, 0,
+        'accumulate'), (24, 256, 256, 3, 16, 1, 0, 'accumulate'), (24, 32, 32, 3, 128, 1, 0, 'accumulate'), (24, 4, 4, 3,
+        256, 1, 0, 'accumulate'), (24, 64, 64, 3, 64, 1, 0, 'accumulate'), (24, 8, 8, 3, 256, 1, 0, 'accumulate'), (3, 1, 1,
+        256, 1, 1, 0, 'accumulate'), (3, 128, 128, 3, 32, 1, 0, 'accumulate'), (3, 256, 256, 3, 16, 1, 0, 'accumulate'),
+        (32, 128, 128, 3, 32, 1, 0, 'accumulate'), (32, 16, 16, 256, 3, 1, 0, 'accumulate'), (32, 16, 16, 3, 256, 1, 0,
+        'accumulate'), (32, 256, 256, 3, 16, 1, 0, 'accumulate'), (32, 32, 32, 128, 3, 1, 0, 'accumulate'), (32, 32, 32, 3,
+        128, 1, 0, 'accumulate'), (32, 4, 4, 256, 3, 1, 0, 'accumulate'), (32, 4, 4, 3, 256, 1, 0, 'accumulate'), (32, 64,
+        64, 3, 64, 1, 0, 'accumulate'), (32, 64, 64, 64, 3, 1, 0, 'accumulate'), (32, 8, 8, 256, 3, 1, 0, 'accumulate'),
+        (32, 8, 8, 3, 256, 1, 0, 'accumulate'), (36, 1, 1, 256, 1, 1, 0, 'accumulate'), (36, 128, 128, 3, 32, 1, 0,
+        'accumulate'), (36, 256, 256, 3, 16, 1, 0, 'accumulate'), (36, 32, 32, 3, 128, 1, 0, 'accumulate'), (36, 64, 64, 3,
+        64, 1, 0, 'accumulate'), (4, 1, 1, 256, 1, 1, 0, 'accumulate'), (4, 128, 128, 3, 32, 1, 0, 'accumulate'), (4, 64,
+        64, 3, 64, 1, 0, 'accumulate'), (48, 1, 1, 256, 1, 1, 0, 'accumulate'), (48, 128, 128, 3, 32, 1, 0, 'accumulate'),
+        (48, 128, 128, 32, 3, 1, 0, 'accumulate'), (48, 16, 16, 3, 256, 1, 0, 'accumulate'), (48, 256, 256, 16, 3, 1, 0,
+        'accumulate'), (48, 256, 256, 3, 16, 1, 0, 'accumulate'), (48, 32, 32, 128, 3, 1, 0, 'accumulate'), (48, 32, 32, 3,
+        128, 1, 0, 'accumulate'), (48, 4, 4, 3, 256, 1, 0, 'accumulate'), (48, 64, 64, 3, 64, 1, 0, 'accumulate'), (48, 64,
+        64, 64, 3, 1, 0, 'accumulate'), (48, 8, 8, 3, 256, 1, 0, 'accumulate'), (6, 128, 128, 3, 32, 1, 0, 'accumulate'),
+        (6, 256, 256, 3, 16, 1, 0, 'accumulate'), (64, 128, 128, 32, 3, 1, 0, 'accumulate'), (64, 16, 16, 256, 3, 1, 0,
+        'accumulate'), (64, 256, 256, 16, 3, 1, 0, 'accumulate'), (64, 32, 32, 128, 3, 1, 0, 'accumulate'), (64, 4, 4, 256,
+        3, 1, 0, 'accumulate'), (64, 64, 64, 64, 3, 1, 0, 'accumulate'), (64, 8, 8, 256, 3, 1, 0, 'accumulate'), (8, 1, 1,
+        256, 1, 1, 0, 'accumulate'), (8, 128, 128, 3, 32, 1, 0, 'accumulate'), (8, 16, 16, 3, 256, 1, 0, 'accumulate'), (8,
+        32, 32, 3, 128, 1, 0, 'accumulate'), (8, 4, 4, 3, 256, 1, 0, 'accumulate'), (8, 64, 64, 3, 64, 1, 0, 'accumulate'),
+        (8, 8, 8, 3, 256, 1, 0, 'accumulate'), (9, 1, 1, 256, 1, 1, 0, 'accumulate'), (9, 128, 128, 3, 32, 1, 0,
+        'accumulate'), (9, 256, 256, 3, 16, 1, 0, 'accumulate')],
     'twg_conv_wgrad_planes': [
-        (1, 1, 4096, 256, 1, 0, 'accumulate'), (4, 4, 256, 256, 3, 1, 'accumulate'), (4, 4, 384, 256, 3, 1,
-        'accumulate'), (8, 8, 256, 256, 3, 1, 'accumulate'), (8, 8, 512, 256, 1, 0, 'accumulate'), (8, 8, 512,
-        256, 3, 1, 'accumulate'), (16, 16, 256, 256, 3, 1, 'accumulate'), (16, 16, 512, 256, 1, 0,
-        'accumulate'), (16, 16, 512, 256, 3, 1, 'accumulate'), (32, 32, 128, 128, 3, 1, 'accumulate'), (32, 32,
-        128, 256, 1, 0, 'accumulate'), (32, 32, 128, 256, 3, 1, 'accumulate'), (32, 32, 512, 128, 1, 0,
-        'accumulate'), (32, 32, 512, 128, 3, 1, 'accumulate'), (64, 64, 64, 64, 3, 1, 'accumulate'), (64, 64,
-        64, 128, 1, 0, 'accumulate'), (64, 64, 64, 128, 3, 1, 'accumulate'), (64, 64, 256, 64, 1, 0,
-        'accumulate'), (64, 64, 256, 64, 3, 1, 'accumulate'), (128, 128, 32, 32, 3, 1, 'accumulate'), (128, 128,
-        32, 64, 1, 0, 'accumulate'), (128, 128, 32, 64, 3, 1, 'accumulate'), (128, 128, 128, 32, 1, 0,
-        'accumulate'), (128, 128, 128, 32, 3, 1, 'accumulate'), (256, 256, 16, 16, 3, 1, 'accumulate'), (256,
-        256, 16, 32, 1, 0, 'accumulate'), (256, 256, 16, 32, 3, 1, 'accumulate'), (256, 256, 64, 16, 1, 0,
-        'accumulate'), (256, 256, 64, 16, 3, 1, 'accumulate')],
+        (12, 1, 1, 4096, 256, 1, 0, 'accumulate'), (12, 128, 128, 128, 32, 1, 0, 'accumulate'), (12, 128, 128, 128, 32, 3,
+        1, 'accumulate'), (12, 128, 128, 32, 32, 3, 1, 'accumulate'), (12, 128, 128, 32, 64, 1, 0, 'accumulate'), (12, 128,
+        128, 32, 64, 3, 1, 'accumulate'), (12, 16, 16, 256, 256, 3, 1, 'accumulate'), (12, 16, 16, 512, 256, 1, 0,
+        'accumulate'), (12, 16, 16, 512, 256, 3, 1, 'accumulate'), (12, 256, 256, 16, 16, 3, 1, 'accumulate'), (12, 256,
+        256, 16, 32, 1, 0, 'accumulate'), (12, 256, 256, 16, 32, 3, 1, 'accumulate'), (12, 256, 256, 64, 16, 1, 0,
+        'accumulate'), (12, 256, 256, 64, 16, 3, 1, 'accumulate'), (12, 32, 32, 128, 128, 3, 1, 'accumulate'), (12, 32, 32,
+        128, 256, 1, 0, 'accumulate'), (12, 32, 32, 128, 256, 3, 1, 'accumulate'), (12, 32, 32, 512, 128, 1, 0,
+        'accumulate'), (12, 32, 32, 512, 128, 3, 1, 'accumulate'), (12, 4, 4, 256, 256, 3, 1, 'accumulate'), (12, 4, 4, 384,
+        256, 3, 1, 'accumulate'), (12, 64, 64, 256, 64, 1, 0, 'accumulate'), (12, 64, 64, 256, 64, 3, 1, 'accumulate'), (12,
+        64, 64, 64, 128, 1, 0, 'accumulate'), (12, 64, 64, 64, 128, 3, 1, 'accumulate'), (12, 64, 64, 64, 64, 3, 1,
+        'accumulate'), (12, 8, 8, 256, 256, 3, 1, 'accumulate'), (12, 8, 8, 512, 256, 1, 0, 'accumulate'), (12, 8, 8, 512,
+        256, 3, 1, 'accumulate'), (16, 1, 1, 4096, 256, 1, 0, 'accumulate'), (16, 128, 128, 128, 32, 1, 0, 'accumulate'),
+        (16, 128, 128, 128, 32, 3, 1, 'accumulate'), (16, 128, 128, 32, 32, 3, 1, 'accumulate'), (16, 128, 128, 32, 64, 1,
+        0, 'accumulate'), (16, 128, 128, 32, 64, 3, 1, 'accumulate'), (16, 16, 16, 256, 256, 3, 1, 'accumulate'), (16, 16,
+        16, 512, 256, 1, 0, 'accumulate'), (16, 16, 16, 512, 256, 3, 1, 'accumulate'), (16, 256, 256, 16, 16, 3, 1,
+        'accumulate'), (16, 256, 256, 16, 32, 1, 0, 'accumulate'), (16, 256, 256, 16, 32, 3, 1, 'accumulate'), (16, 256,
+        256, 64, 16, 3, 1, 'accumulate'), (16, 32, 32, 128, 128, 3, 1, 'accumulate'), (16, 32, 32, 128, 256, 1, 0,
+        'accumulate'), (16, 32, 32, 128, 256, 3, 1, 'accumulate'), (16, 32, 32, 512, 128, 1, 0, 'accumulate'), (16, 32, 32,
+        512, 128, 3, 1, 'accumulate'), (16, 4, 4, 256, 256, 3, 1, 'accumulate'), (16, 4, 4, 384, 256, 3, 1, 'accumulate'),
+        (16, 64, 64, 256, 64, 1, 0, 'accumulate'), (16, 64, 64, 256, 64, 3, 1, 'accumulate'), (16, 64, 64, 64, 128, 1, 0,
+        'accumulate'), (16, 64, 64, 64, 128, 3, 1, 'accumulate'), (16, 64, 64, 64, 64, 3, 1, 'accumulate'), (16, 8, 8, 256,
+        256, 3, 1, 'accumulate'), (16, 8, 8, 512, 256, 1, 0, 'accumulate'), (16, 8, 8, 512, 256, 3, 1, 'accumulate'), (24,
+        1, 1, 4096, 256, 1, 0, 'accumulate'), (24, 128, 128, 32, 32, 3, 1, 'accumulate'), (24, 128, 128, 32, 64, 1, 0,
+        'accumulate'), (24, 128, 128, 32, 64, 3, 1, 'accumulate'), (24, 16, 16, 256, 256, 3, 1, 'accumulate'), (24, 256,
+        256, 16, 16, 3, 1, 'accumulate'), (24, 256, 256, 16, 32, 1, 0, 'accumulate'), (24, 256, 256, 16, 32, 3, 1,
+        'accumulate'), (24, 32, 32, 128, 128, 3, 1, 'accumulate'), (24, 32, 32, 128, 256, 1, 0, 'accumulate'), (24, 32, 32,
+        128, 256, 3, 1, 'accumulate'), (24, 4, 4, 384, 256, 3, 1, 'accumulate'), (24, 64, 64, 64, 128, 1, 0, 'accumulate'),
+        (24, 64, 64, 64, 128, 3, 1, 'accumulate'), (24, 64, 64, 64, 64, 3, 1, 'accumulate'), (24, 8, 8, 256, 256, 3, 1,
+        'accumulate'), (3, 1, 1, 4096, 256, 1, 0, 'accumulate'), (3, 128, 128, 32, 32, 3, 1, 'accumulate'), (3, 128, 128,
+        32, 64, 1, 0, 'accumulate'), (3, 128, 128, 32, 64, 3, 1, 'accumulate'), (3, 16, 16, 256, 256, 3, 1, 'accumulate'),
+        (3, 256, 256, 16, 16, 3, 1, 'accumulate'), (3, 256, 256, 16, 32, 1, 0, 'accumulate'), (3, 256, 256, 16, 32, 3, 1,
+        'accumulate'), (3, 32, 32, 128, 128, 3, 1, 'accumulate'), (3, 32, 32, 128, 256, 1, 0, 'accumulate'), (3, 32, 32,
+        128, 256, 3, 1, 'accumulate'), (3, 4, 4, 384, 256, 3, 1, 'accumulate'), (3, 64, 64, 64, 128, 1, 0, 'accumulate'),
+        (3, 64, 64, 64, 128, 3, 1, 'accumulate'), (3, 64, 64, 64, 64, 3, 1, 'accumulate'), (3, 8, 8, 256, 256, 3, 1,
+        'accumulate'), (32, 128, 128, 32, 32, 3, 1, 'accumulate'), (32, 128, 128, 32, 64, 1, 0, 'accumulate'), (32, 128,
+        128, 32, 64, 3, 1, 'accumulate'), (32, 16, 16, 256, 256, 3, 1, 'accumulate'), (32, 16, 16, 512, 256, 1, 0,
+        'accumulate'), (32, 16, 16, 512, 256, 3, 1, 'accumulate'), (32, 256, 256, 16, 16, 3, 1, 'accumulate'), (32, 256,
+        256, 16, 32, 1, 0, 'accumulate'), (32, 256, 256, 16, 32, 3, 1, 'accumulate'), (32, 32, 32, 128, 128, 3, 1,
+        'accumulate'), (32, 32, 32, 128, 256, 1, 0, 'accumulate'), (32, 32, 32, 128, 256, 3, 1, 'accumulate'), (32, 32, 32,
+        512, 128, 1, 0, 'accumulate'), (32, 32, 32, 512, 128, 3, 1, 'accumulate'), (32, 4, 4, 256, 256, 3, 1, 'accumulate'),
+        (32, 64, 64, 256, 64, 1, 0, 'accumulate'), (32, 64, 64, 256, 64, 3, 1, 'accumulate'), (32, 64, 64, 64, 128, 1, 0,
+        'accumulate'), (32, 64, 64, 64, 128, 3, 1, 'accumulate'), (32, 64, 64, 64, 64, 3, 1, 'accumulate'), (32, 8, 8, 256,
+        256, 3, 1, 'accumulate'), (32, 8, 8, 512, 256, 1, 0, 'accumulate'), (32, 8, 8, 512, 256, 3, 1, 'accumulate'), (36,
+        1, 1, 4096, 256, 1, 0, 'accumulate'), (36, 128, 128, 32, 32, 3, 1, 'accumulate'), (36, 128, 128, 32, 64, 1, 0,
+        'accumulate'), (36, 128, 128, 32, 64, 3, 1, 'accumulate'), (36, 16, 16, 256, 256, 3, 1, 'accumulate'), (36, 256,
+        256, 16, 16, 3, 1, 'accumulate'), (36, 256, 256, 16, 32, 1, 0, 'accumulate'), (36, 256, 256, 16, 32, 3, 1,
+        'accumulate'), (36, 32, 32, 128, 128, 3, 1, 'accumulate'), (36, 32, 32, 128, 256, 1, 0, 'accumulate'), (36, 32, 32,
+        128, 256, 3, 1, 'accumulate'), (36, 4, 4, 384, 256, 3, 1, 'accumulate'), (36, 64, 64, 64, 128, 1, 0, 'accumulate'),
+        (36, 64, 64, 64, 128, 3, 1, 'accumulate'), (36, 64, 64, 64, 64, 3, 1, 'accumulate'), (36, 8, 8, 256, 256, 3, 1,
+        'accumulate'), (4, 1, 1, 4096, 256, 1, 0, 'accumulate'), (4, 128, 128, 32, 32, 3, 1, 'accumulate'), (4, 128, 128,
+        32, 64, 1, 0, 'accumulate'), (4, 128, 128, 32, 64, 3, 1, 'accumulate'), (4, 16, 16, 256, 256, 3, 1, 'accumulate'),
+        (4, 32, 32, 128, 128, 3, 1, 'accumulate'), (4, 32, 32, 128, 256, 1, 0, 'accumulate'), (4, 32, 32, 128, 256, 3, 1,
+        'accumulate'), (4, 4, 4, 384, 256, 3, 1, 'accumulate'), (4, 64, 64, 64, 128, 1, 0, 'accumulate'), (4, 64, 64, 64,
+        128, 3, 1, 'accumulate'), (4, 64, 64, 64, 64, 3, 1, 'accumulate'), (4, 8, 8, 256, 256, 3, 1, 'accumulate'), (48, 1,
+        1, 4096, 256, 1, 0, 'accumulate'), (48, 128, 128, 128, 32, 1, 0, 'accumulate'), (48, 128, 128, 128, 32, 3, 1,
+        'accumulate'), (48, 128, 128, 32, 32, 3, 1, 'accumulate'), (48, 128, 128, 32, 64, 1, 0, 'accumulate'), (48, 128,
+        128, 32, 64, 3, 1, 'accumulate'), (48, 16, 16, 256, 256, 3, 1, 'accumulate'), (48, 16, 16, 512, 256, 1, 0,
+        'accumulate'), (48, 16, 16, 512, 256, 3, 1, 'accumulate'), (48, 256, 256, 16, 16, 3, 1, 'accumulate'), (48, 256,
+        256, 16, 32, 1, 0, 'accumulate'), (48, 256, 256, 16, 32, 3, 1, 'accumulate'), (48, 256, 256, 64, 16, 1, 0,
+        'accumulate'), (48, 256, 256, 64, 16, 3, 1, 'accumulate'), (48, 32, 32, 128, 128, 3, 1, 'accumulate'), (48, 32, 32,
+        128, 256, 1, 0, 'accumulate'), (48, 32, 32, 128, 256, 3, 1, 'accumulate'), (48, 32, 32, 512, 128, 1, 0,
+        'accumulate'), (48, 32, 32, 512, 128, 3, 1, 'accumulate'), (48, 4, 4, 256, 256, 3, 1, 'accumulate'), (48, 4, 4, 384,
+        256, 3, 1, 'accumulate'), (48, 64, 64, 256, 64, 1, 0, 'accumulate'), (48, 64, 64, 256, 64, 3, 1, 'accumulate'), (48,
+        64, 64, 64, 128, 1, 0, 'accumulate'), (48, 64, 64, 64, 128, 3, 1, 'accumulate'), (48, 64, 64, 64, 64, 3, 1,
+        'accumulate'), (48, 8, 8, 256, 256, 3, 1, 'accumulate'), (48, 8, 8, 512, 256, 1, 0, 'accumulate'), (48, 8, 8, 512,
+        256, 3, 1, 'accumulate'), (6, 128, 128, 32, 32, 3, 1, 'accumulate'), (6, 128, 128, 32, 64, 1, 0, 'accumulate'), (6,
+        128, 128, 32, 64, 3, 1, 'accumulate'), (6, 16, 16, 256, 256, 3, 1, 'accumulate'), (6, 256, 256, 16, 16, 3, 1,
+        'accumulate'), (6, 256, 256, 16, 32, 1, 0, 'accumulate'), (6, 256, 256, 16, 32, 3, 1, 'accumulate'), (6, 32, 32,
+        128, 128, 3, 1, 'accumulate'), (6, 32, 32, 128, 256, 1, 0, 'accumulate'), (6, 32, 32, 128, 256, 3, 1, 'accumulate'),
+        (6, 64, 64, 64, 128, 1, 0, 'accumulate'), (6, 64, 64, 64, 128, 3, 1, 'accumulate'), (6, 64, 64, 64, 64, 3, 1,
+        'accumulate'), (6, 8, 8, 256, 256, 3, 1, 'accumulate'), (64, 128, 128, 128, 32, 1, 0, 'accumulate'), (64, 128, 128,
+        128, 32, 3, 1, 'accumulate'), (64, 128, 128, 32, 32, 3, 1, 'accumulate'), (64, 16, 16, 256, 256, 3, 1,
+        'accumulate'), (64, 16, 16, 512, 256, 1, 0, 'accumulate'), (64, 16, 16, 512, 256, 3, 1, 'accumulate'), (64, 256,
+        256, 16, 16, 3, 1, 'accumulate'), (64, 256, 256, 64, 16, 1, 0, 'accumulate'), (64, 256, 256, 64, 16, 3, 1,
+        'accumulate'), (64, 32, 32, 128, 128, 3, 1, 'accumulate'), (64, 32, 32, 512, 128, 1, 0, 'accumulate'), (64, 32, 32,
+        512, 128, 3, 1, 'accumulate'), (64, 4, 4, 256, 256, 3, 1, 'accumulate'), (64, 64, 64, 256, 64, 1, 0, 'accumulate'),
+        (64, 64, 64, 256, 64, 3, 1, 'accumulate'), (64, 64, 64, 64, 64, 3, 1, 'accumulate'), (64, 8, 8, 256, 256, 3, 1,
+        'accumulate'), (64, 8, 8, 512, 256, 1, 0, 'accumulate'), (64, 8, 8, 512, 256, 3, 1, 'accumulate'), (8, 1, 1, 4096,
+        256, 1, 0, 'accumulate'), (8, 128, 128, 32, 32, 3, 1, 'accumulate'), (8, 128, 128, 32, 64, 1, 0, 'accumulate'), (8,
+        128, 128, 32, 64, 3, 1, 'accumulate'), (8, 16, 16, 256, 256, 3, 1, 'accumulate'), (8, 32, 32, 128, 128, 3, 1,
+        'accumulate'), (8, 32, 32, 128, 256, 1, 0, 'accumulate'), (8, 32, 32, 128, 256, 3, 1, 'accumulate'), (8, 4, 4, 384,
+        256, 3, 1, 'accumulate'), (8, 64, 64, 64, 128, 1, 0, 'accumulate'), (8, 64, 64, 64, 128, 3, 1, 'accumulate'), (8,
+        64, 64, 64, 64, 3, 1, 'accumulate'), (8, 8, 8, 256, 256, 3, 1, 'accumulate'), (9, 1, 1, 4096, 256, 1, 0,
+        'accumulate'), (9, 128, 128, 32, 32, 3, 1, 'accumulate'), (9, 128, 128, 32, 64, 1, 0, 'accumulate'), (9, 128, 128,
+        32, 64, 3, 1, 'accumulate'), (9, 16, 16, 256, 256, 3, 1, 'accumulate'), (9, 256, 256, 16, 16, 3, 1, 'accumulate'),
+        (9, 256, 256, 16, 32, 1, 0, 'accumulate'), (9, 256, 256, 16, 32, 3, 1, 'accumulate'), (9, 32, 32, 128, 128, 3, 1,
+        'accumulate'), (9, 32, 32, 128, 256, 1, 0, 'accumulate'), (9, 32, 32, 128, 256, 3, 1, 'accumulate'), (9, 4, 4, 384,
+        256, 3, 1, 'accumulate'), (9, 64, 64, 64, 128, 1, 0, 'accumulate'), (9, 64, 64, 64, 128, 3, 1, 'accumulate'), (9,
+        64, 64, 64, 64, 3, 1, 'accumulate'), (9, 8, 8, 256, 256, 3, 1, 'accumulate')],
 }
 PRODUCT_CONV_KEYS = {(entry,) + key for entry, keys in PRODUCT_CONVS.items() for key in keys}
 
 
 def test_every_product_conv_is_a_kernel_suite_case(built_lib):
   seen = harvest_product_convs()
-  _log_result({'test': 'conv_coverage', 'harvested': len(seen), 'keys': sorted(seen)})
-  assert seen == PRODUCT_CONV_KEYS, ('new', sorted(seen - PRODUCT_CONV_KEYS), 'gone', sorted(PRODUCT_CONV_KEYS - seen))
-  missing = sorted(seen - suite_keys())
+  where = key_configs(conv_keys)
+  _log_result({'test': 'conv_coverage', 'harvested': len(seen), 'harvest_s': product_launches.HARVEST_SECONDS,
+               'keys': sorted(seen, key=str)})
+  assert seen == PRODUCT_CONV_KEYS, ('new', sorted(((k, where[k]) for k in seen - PRODUCT_CONV_KEYS), key=str),
+                                     'gone', sorted(PRODUCT_CONV_KEYS - seen, key=str))
+  missing = sorted(((k, where[k]) for k in seen - suite_keys()), key=str)
   assert not missing, missing

@@ -19,7 +19,8 @@ from tests.parity import (MB_THREADS, U32, _log_result, conv_error_ratio, dragan
                           mbstd_bwd2_ref, mbstd_fwd_ref, mbstd_sig_rel, mbstd_stats, norm_sum_c, penalty_c_ss, penalty_ref)
 from tests.product_elementwise import (EXTRA_ELEMENTWISE, PRODUCT_ELEMENTWISE_KEYS, colsum_geom, colsum_plain_geom,
                                        grid_for, penalty_geom, pool_rows_route, vec_geom)
-from tests.product_launches import Recorder, harvest_product_launches
+from tests import product_launches
+from tests.product_launches import Recorder, harvest_product_launches, key_configs
 from tests.test_gpu_conv_conformance import _GEOM_AT, _bits, _split_ref
 
 pytestmark = pytest.mark.gpu
@@ -891,9 +892,11 @@ def test_every_product_launch_belongs_to_one_audit(built_lib):
   unowned = [n for n, c in claims.items() if not c]
   shared = {n: c for n, c in claims.items() if len(c) > 1}
   seen = elementwise_keys(launches)
-  _log_result({'test': 'elementwise_coverage', 'harvested': len(seen), 'entries': len(names), 'keys': sorted(seen, key=str)})
+  where = key_configs(elementwise_keys)
+  _log_result({'test': 'elementwise_coverage', 'harvested': len(seen), 'entries': len(names),
+               'harvest_s': product_launches.HARVEST_SECONDS, 'keys': sorted(seen, key=str)})
   assert not unowned and not shared, ('unowned', unowned, 'shared', shared)
-  assert seen == PRODUCT_ELEMENTWISE_KEYS, ('new', sorted(seen - PRODUCT_ELEMENTWISE_KEYS, key=str),
+  assert seen == PRODUCT_ELEMENTWISE_KEYS, ('new', sorted(((k, where[k]) for k in seen - PRODUCT_ELEMENTWISE_KEYS), key=str),
                                             'gone', sorted(PRODUCT_ELEMENTWISE_KEYS - seen, key=str))
-  missing = sorted((k for k in seen if k not in SUITE_ELEMENTWISE_KEYS or k[0] not in _RUNNERS), key=str)
+  missing = sorted(((k, where[k]) for k in seen if k not in SUITE_ELEMENTWISE_KEYS or k[0] not in _RUNNERS), key=str)
   assert not missing, missing

@@ -18,7 +18,8 @@ import torch
 
 from tests.parity import (REL_TOL, U32, _log_result, conv_error_ratio, ema_c, exact_elem_c, mean_bound, norm_sum_c, rel_err,
                           rstd_rel_bound, serial_run)
-from tests.product_launches import Recorder, harvest_product_launches
+from tests import product_launches
+from tests.product_launches import Recorder, harvest_product_launches, key_configs
 from tests.product_norms import PRODUCT_NORM_KEYS
 from tests.test_gpu_conv_conformance import _bits, _split_ref
 
@@ -603,10 +604,12 @@ def test_normaliser_stage_against_fp64(built_lib, key):
 
 def test_every_product_normaliser_launch_is_a_suite_case(built_lib):
   seen = norm_keys(harvest_product_launches())
-  _log_result({'test': 'norm_coverage', 'harvested': len(seen), 'keys': sorted(seen, key=str)})
-  assert seen == PRODUCT_NORM_KEYS, ('new', sorted(seen - PRODUCT_NORM_KEYS, key=str),
+  where = key_configs(norm_keys)
+  _log_result({'test': 'norm_coverage', 'harvested': len(seen), 'harvest_s': product_launches.HARVEST_SECONDS,
+               'keys': sorted(seen, key=str)})
+  assert seen == PRODUCT_NORM_KEYS, ('new', sorted(((k, where[k]) for k in seen - PRODUCT_NORM_KEYS), key=str),
                                      'gone', sorted(PRODUCT_NORM_KEYS - seen, key=str))
-  missing = sorted((k for k in seen if k not in SUITE_NORM_KEYS or k[0] not in _RUNNERS), key=str)
+  missing = sorted(((k, where[k]) for k in seen if k not in SUITE_NORM_KEYS or k[0] not in _RUNNERS), key=str)
   assert not missing, missing
 
 

@@ -27,6 +27,15 @@ def test_step_parity(built_lib, hw, batch, mc, norm, growing, prec):
   ops.set_precision(1)
 
 
+def test_step_parity_8_growing_at_3_pairs_on_tensor_cores(built_lib):
+  """8x8 growing at 3 pairs, 256 channels, tensor cores: the smallest real-width layers where a stage runner's batch
+  (pggan_runner.TWINGAN_HW_TO_BATCH_SIZE trains 256x256 at 3 pairs, and its discriminator runs these layers) leaves
+  the last 2-image batch tile ragged (D at N = 9, the DRAGAN pass at 3) and the last CTA of the 256 -> 256 weight
+  gradient short (5 tiles over CTAs of 2, 2 and 1)."""
+  res = run_step_parity(hw=8, batch=3, max_num_channels=256, norm='instance_norm', is_growing=True, prec=1, verbose=True)
+  assert res['ok'], 'worst=%g bad=%s' % (res['worst'], dict(list(res['bad'].items())[:5]))
+
+
 @pytest.mark.parametrize('hw,batch,mc,norm,growing', [CASES[1], CASES[2], CASES[4]])
 def test_step_parity_pass_by_pass(built_lib, hw, batch, mc, norm, growing):
   """The same step with the reference's own pass structure (16 separate passes, Flags.batch_passes = False)."""
