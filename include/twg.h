@@ -326,6 +326,20 @@ int twg_swd_sort(float* keys, void* workspace, int segments, int64_t seg_len, tw
 /* out_f64[0] = sum_i |a[i] - b[i]| accumulated in fp64 (one double in device memory) */
 int twg_swd_sorted_l1(const float* a, const float* b, void* out_f64, int64_t n, twg_stream_t stream);
 
+/* ---- image translation front and back end, outside the step: inference/image_translation_infer.py:54-58 (ImageInferer:
+ *      tf.image.convert_image_dtype, then tf.image.resize_images, bilinear, to image_hw) and util_io.imsave. */
+/* A ragged batch of B decoded RGB images -> out:[B, hw, hw, 3] fp32 NHWC (16-byte aligned), the input of the model.
+ * `payload`: the images back to back, uint8 HWC, tightly packed, each at any byte offset; `table`: DEVICE array [B][3] of
+ * int64 {byte offset, H, W}.  The table is read on the device only: the caller validates every row against the payload
+ * (twingan_b200.ops.pack_images).  Per output pixel: p = float(u8) * fl32(1/255); scale = (float)H / hw, in_y = y * scale
+ * in fp32, y0 = (int)in_y, y1 = min(y0 + 1, H - 1), ly = in_y - y0 (x alike); top = p00 + (p01 - p00) * lx, bot = p10 +
+ * (p11 - p10) * lx, out = top + (bot - top) * ly, each operation rounded in fp32 (TF 1.8 resize_bilinear_op.cc,
+ * align_corners=False, no half-pixel centres).  An image already at hw x hw comes out exactly as u8 * fl32(1/255). */
+int twg_images_u8_to_batch(const void* payload, const int64_t* table, float* out, int B, int hw, twg_stream_t stream);
+/* out_u8[i] = (uint8)trunc(min(max(fl32(x[i] * 255), 0), 255)): bit for bit numpy's
+ * np.clip(x * 255.0, 0, 255).astype(np.uint8) on float32 x (util_io.imsave).  NaN maps to 0. */
+int twg_batch_to_u8(const float* x, void* out_u8, int64_t n, twg_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

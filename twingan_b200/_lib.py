@@ -17,7 +17,7 @@ LIB_PATH = os.environ.get('TWG_LIB') or os.path.join(_HERE, 'libtwg.so')   # TWG
 
 _CTYPES = {
     'const float*': ctypes.c_void_p, 'float*': ctypes.c_void_p, 'void*': ctypes.c_void_p,
-    'const void*': ctypes.c_void_p, 'twg_stream_t': ctypes.c_void_p,
+    'const void*': ctypes.c_void_p, 'const int64_t*': ctypes.c_void_p, 'twg_stream_t': ctypes.c_void_p,
     'int': ctypes.c_int, 'int64_t': ctypes.c_int64, 'float': ctypes.c_float,
     'const char*': ctypes.c_char_p, 'void': None,
 }

@@ -1490,6 +1490,75 @@ def growing_image(x, alpha):
     return lerp(x, low, alpha)
 
 
+# ------------------------------------------------------------------------------------------------
+# image translation front and back end (inference/image_translation_infer.py:54-58, util_io.imsave)
+# ------------------------------------------------------------------------------------------------
+
+def pack_images(images) -> Tuple[torch.Tensor, torch.Tensor]:
+  """Decoded uint8 [H, W, 3] RGB arrays (numpy or CPU tensors) -> (payload, table) host tensors for images_u8_to_batch:
+  payload uint8 [sum of H*W*3], the images back to back; table int64 [B, 3] of {byte offset, H, W}."""
+  import numpy as np
+  arrs = []
+  for i, im in enumerate(images):
+    a = im.numpy() if isinstance(im, torch.Tensor) else np.asarray(im)
+    if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3:
+      raise ValueError('image %d: want a uint8 [H, W, 3] array, got %s %s' % (i, a.dtype, tuple(a.shape)))
+    if a.shape[0] < 1 or a.shape[1] < 1:
+      raise ValueError('image %d is empty (%d x %d)' % (i, a.shape[0], a.shape[1]))
+    arrs.append(np.ascontiguousarray(a))
+  if not arrs:
+    raise ValueError('pack_images: no images')
+  table = np.zeros((len(arrs), 3), np.int64)
+  off = 0
+  for i, a in enumerate(arrs):
+    table[i] = (off, a.shape[0], a.shape[1])
+    off += a.size
+  payload = torch.from_numpy(np.concatenate([a.reshape(-1) for a in arrs]))
+  table = torch.from_numpy(table)
+  check_table(table, payload.numel())
+  return payload, table
+
+
+def check_table(table: torch.Tensor, payload_bytes: int) -> None:
+  """Every row {offset, H, W} of a host table must describe a non-empty image inside a payload of `payload_bytes` bytes
+  (the kernel reads the table on the device and cannot check it)."""
+  if table.device.type != 'cpu' or table.dtype != torch.int64 or table.dim() != 2 or table.shape[1] != 3 \
+      or table.shape[0] < 1:
+    raise ValueError('image table: want a host int64 [B, 3] tensor, got %s %s on %s'
+                     % (table.dtype, tuple(table.shape), table.device))
+  for i, (off, h, w) in enumerate(table.tolist()):
+    if h < 1 or w < 1 or off < 0 or off + h * w * 3 > payload_bytes:
+      raise ValueError('image table row %d {offset %d, H %d, W %d} does not fit a payload of %d bytes'
+                       % (i, off, h, w, payload_bytes))
+
+
+def images_u8_to_batch(payload: torch.Tensor, table: torch.Tensor, hw: int, out: Optional[torch.Tensor] = None
+                       ) -> torch.Tensor:
+  """Ragged uint8 images -> the model's fp32 [B, hw, hw, 3] input in one launch (convert_image_dtype + TF-1 bilinear
+  resize, twg_images_u8_to_batch).  `payload`: uint8 CUDA tensor; `table`: int64 [B, 3] -- a host table is checked
+  against the payload and uploaded; a device table must come from pack_images (through a copy of it)."""
+  if not payload.is_cuda or payload.dtype != torch.uint8:
+    raise TwgError('images_u8_to_batch: payload must be a uint8 CUDA tensor (no CPU fallback)')
+  if table.device.type == 'cpu':
+    check_table(table, payload.numel())
+    table = table.to(payload.device, non_blocking=False)
+  elif table.dtype != torch.int64 or table.dim() != 2 or table.shape[1] != 3:
+    raise ValueError('image table: want int64 [B, 3], got %s %s' % (table.dtype, tuple(table.shape)))
+  B = int(table.shape[0])
+  if out is None:
+    out = torch.empty((B, hw, hw, 3), device=payload.device, dtype=torch.float32)
+  lib().call('twg_images_u8_to_batch', payload.data_ptr(), table.contiguous().data_ptr(), _p(out), B, int(hw), _st())
+  return out
+
+
+def batch_to_u8(x: torch.Tensor) -> torch.Tensor:
+  """uint8 image of the model output, clip(x * 255, 0, 255) truncated (util_io.imsave; twg_batch_to_u8)."""
+  x = _check(x)
+  out = torch.empty(x.shape, device=x.device, dtype=torch.uint8)
+  lib().call('twg_batch_to_u8', _p(x), out.data_ptr(), x.numel(), _st())
+  return out
+
+
 def adam_(p, g, m, v, lr_t, beta1, beta2, eps):
   """lr_t: python float, or a 1-element device tensor (graph-replayable)."""
   if isinstance(lr_t, torch.Tensor):

@@ -183,6 +183,74 @@ def warm_start(model, ckpt: Dict[str, object], ignore_missing_vars: bool = False
   return missing
 
 
+# -- loading a trained model for inference / evaluation ------------------------------------------------------
+_TF_STATE_RE = re.compile(r'^model_checkpoint_path:\s*"([^"]*)"\s*$', re.M)
+
+
+def step_of(path: str, default: int = 0) -> int:
+  """The step a checkpoint's name carries (model.ckpt-<step>[.pt], like the reference's '.ckpt-' split), else `default`."""
+  m = re.search(r'-(\d+)(\.pt)?$', path)
+  return int(m.group(1)) if m else default
+
+
+def resolve_model_path(path: str) -> Tuple[str, str]:
+  """('pt', file) or ('tf', checkpoint prefix) for a model path given as
+    * a model.ckpt-<step>.pt of this runner;
+    * a directory holding such files (the newest one);
+    * the prefix of a TensorFlow V2 checkpoint of the reference (<prefix>.index exists);
+    * a directory holding a TensorFlow `checkpoint` state file (model_checkpoint_path: "...", relative to the directory
+      unless absolute: tf.train.get_checkpoint_state, as util_io.get_model_filenames reads it).
+  A frozen graph (.pb / .pbtxt) or a metagraph (.meta) is refused: only checkpoints of the variables can be loaded."""
+  if path.endswith(('.pb', '.pbtxt', '.meta')):
+    raise ValueError('%s: loading a frozen graph or a metagraph is not supported; pass a checkpoint (a model.ckpt-<step>.pt, '
+                     'a TensorFlow checkpoint prefix, or a directory holding either)' % path)
+  if os.path.isdir(path):
+    own = latest_checkpoint(path)
+    if own is not None:
+      return 'pt', own[0]
+    state = os.path.join(path, 'checkpoint')
+    if os.path.isfile(state):
+      m = _TF_STATE_RE.search(open(state, encoding='utf-8').read())
+      if not m:
+        raise ValueError('%s has no model_checkpoint_path entry' % state)
+      prefix = m.group(1) if os.path.isabs(m.group(1)) else os.path.join(path, m.group(1))
+      if not os.path.isfile(prefix + '.index'):
+        raise FileNotFoundError('%s names %s, which has no .index file' % (state, prefix))
+      return 'tf', prefix
+    raise FileNotFoundError('no checkpoint in directory %s (no model.ckpt-<step>.pt, no TensorFlow checkpoint file)' % path)
+  if os.path.isfile(path):
+    return 'pt', path
+  if os.path.isfile(path + '.index'):
+    return 'tf', path
+  raise FileNotFoundError('no checkpoint at %s (neither a file nor a TensorFlow prefix with a .index file)' % path)
+
+
+def load_for_inference(path: str, flags, device='cuda'):
+  """(twingan.GanModel, step) of the checkpoint `path` names (any form of resolve_model_path), weights and normaliser
+  moving statistics restored, optimiser state not.  flags.train_image_size must equal a .pt checkpoint's; None takes it
+  from the checkpoint, which a TensorFlow checkpoint does not record, so there it is required."""
+  from . import tf_checkpoint, twingan
+  kind, where = resolve_model_path(path)
+  if kind == 'pt':
+    ckpt = load_checkpoint(where)
+    trained = int(ckpt['train_image_size']) if 'train_image_size' in ckpt else None
+    if flags.train_image_size is None:
+      if trained is None:
+        raise ValueError('%s does not record its image size; give it explicitly' % where)
+      flags = replace(flags, train_image_size=trained)
+    elif trained is not None and trained != flags.train_image_size:
+      raise ValueError('%s was trained at %d x %d, not %d x %d'
+                       % (where, trained, trained, flags.train_image_size, flags.train_image_size))
+    model = twingan.GanModel(flags, device=device)
+    warm_start(model, ckpt, ignore_missing_vars=False, restore_optimizer=False)
+    return model, step_of(where, int(ckpt.get('global_step', 0)))
+  if flags.train_image_size is None:
+    raise ValueError('%s is a TensorFlow checkpoint, which does not record its image size; give it explicitly' % where)
+  model = twingan.GanModel(flags, device=device)
+  tf_checkpoint.import_into(model, where, ignore_missing_vars=False, load_adam=False)
+  return model, step_of(where)
+
+
 # -- the loop ----------------------------------------------------------------------------------------------
 BatchFn = Callable[[Stage, int], Tuple[torch.Tensor, torch.Tensor]]
 EvalFn = Callable[[object, int], object]

@@ -11,8 +11,6 @@ writes <eval_dir>/swd_eval_step_<step>_<n>_images.txt in the reference's layout:
 from __future__ import annotations
 
 import argparse
-import os
-import re
 import sys
 
 from . import swd
@@ -21,7 +19,8 @@ from . import swd
 def _parser() -> argparse.ArgumentParser:
   p = argparse.ArgumentParser(prog='python -m twingan_b200.swd_eval', description=__doc__.split('\n\n')[0])
   p.add_argument('--checkpoint_path', required=True,
-                 help='a model.ckpt-<step>.pt of pggan_runner, or the prefix of a TensorFlow checkpoint of the reference')
+                 help='a model.ckpt-<step>.pt of pggan_runner, or the prefix of a TensorFlow checkpoint of the reference, '
+                      'or a directory holding either (pggan_runner.resolve_model_path)')
   p.add_argument('--dataset_dir', required=True, help='image_only TFRecords of the source domain')
   p.add_argument('--unpaired_target_dataset_dir', required=True, help='image_only TFRecords of the target domain')
   p.add_argument('--dataset_split_name', default='train')
@@ -33,32 +32,6 @@ def _parser() -> argparse.ArgumentParser:
   p.add_argument('--batch_size', type=int, default=64, help='images translated per model call')
   p.add_argument('--seed', type=int, default=0, help='seeds the image draws, the neighbourhoods and the directions')
   return p
-
-
-def _step_of(path: str, default: int = 0) -> int:
-  """The step a checkpoint's name carries (model.ckpt-<step>[.pt], like the reference's '.ckpt-' split), else `default`."""
-  m = re.search(r'-(\d+)(\.pt)?$', path)
-  return int(m.group(1)) if m else default
-
-
-def _load_model(args):
-  from . import pggan_runner, tf_checkpoint, twingan
-  flags = twingan.Flags(train_image_size=args.train_image_size, pggan_max_num_channels=args.pggan_max_num_channels,
-                        generator_norm_type=args.generator_norm_type)
-  path = args.checkpoint_path
-  if os.path.isfile(path):
-    ckpt = pggan_runner.load_checkpoint(path)
-    if int(ckpt.get('train_image_size', args.train_image_size)) != args.train_image_size:
-      raise ValueError('%s was trained at %d x %d, not --train_image_size=%d'
-                       % (path, ckpt['train_image_size'], ckpt['train_image_size'], args.train_image_size))
-    model = twingan.GanModel(flags, device='cuda')
-    pggan_runner.warm_start(model, ckpt, ignore_missing_vars=False, restore_optimizer=False)
-    return model, _step_of(path, int(ckpt.get('global_step', 0)))
-  if os.path.isfile(path + '.index'):
-    model = twingan.GanModel(flags, device='cuda')
-    tf_checkpoint.import_into(model, path, ignore_missing_vars=False, load_adam=False)
-    return model, _step_of(path)
-  raise FileNotFoundError('no checkpoint at %s (neither a file nor a TensorFlow prefix with a .index file)' % path)
 
 
 def main(argv=None):
@@ -80,7 +53,10 @@ def main(argv=None):
     if len(ds) < args.swd_num_images:
       parser.error('%s has %d %s images, fewer than --swd_num_images=%d'
                    % (name, len(ds), args.dataset_split_name, args.swd_num_images))
-  model, step = _load_model(args)
+  from . import pggan_runner, twingan
+  flags = twingan.Flags(train_image_size=args.train_image_size, pggan_max_num_channels=args.pggan_max_num_channels,
+                        generator_norm_type=args.generator_norm_type)
+  model, step = pggan_runner.load_for_inference(args.checkpoint_path, flags)
   result = swd.evaluate_translation(model, source, target, args.swd_num_images, args.seed, args.batch_size)
   path = swd.write_result(args.eval_dir, step, args.swd_num_images, result, is_training=False)
   print(open(path).read(), end='')

@@ -573,11 +573,24 @@ class GanModel:
 
   # -- inference (inference/image_translation_infer.py:46-99; twingan.py:310-365) --------------------
   @torch.no_grad()
-  def infer(self, sources):
-    """custom_generated_t_style_source: G(E(x; '_s', eval); '_t', eval, UNet skips)."""
-    code, ep = self._encoder(sources, '_s', is_training=False)
-    out, _ = self._generator(code, '_t', ep, sources.shape, is_training=False)
+  def infer(self, sources, target_domain: str = 't'):
+    """target_domain 't': custom_generated_t_style_source, G(E(x; '_s', eval); '_t', eval, UNet skips);
+    's': custom_generated_s_style_target, G(E(x; '_t', eval); '_s', eval, UNet skips) (twingan.py:337-365) -- `sources`
+    are then images of the target domain."""
+    src, dst = _DIRECTIONS[check_target_domain(target_domain)]
+    code, ep = self._encoder(sources, src, is_training=False)
+    out, _ = self._generator(code, dst, ep, sources.shape, is_training=False)
     return out
+
+
+# target domain of a translation -> (encoder postfix, generator postfix)
+_DIRECTIONS = {'t': ('_s', '_t'), 's': ('_t', '_s')}
+
+
+def check_target_domain(target_domain: str) -> str:
+  if target_domain not in _DIRECTIONS:
+    raise ValueError("target_domain must be 't' (source -> target) or 's' (target -> source), got %r" % (target_domain,))
+  return target_domain
 
 
 class InferencePipeline(object):
@@ -586,11 +599,13 @@ class InferencePipeline(object):
   copy of batch k+1 and the device->host copy of result k-1 run on side streams while batch k computes; the device
   staging slots and the pinned result slots are allocated once and reused across `run` calls.
   `use_graph`: the ~90 kernel launches of a batch are captured once per batch shape into a CUDA graph over a static input
-  buffer and replayed (the weights are read through the persistent weight-plane table, so a later `load_dict` is seen)."""
+  buffer and replayed (the weights are read through the persistent weight-plane table, so a later `load_dict` is seen).
+  `target_domain`: the direction of GanModel.infer every batch takes (and its graphs capture)."""
 
-  def __init__(self, model: GanModel, depth: int = 2, use_graph: bool = False):
+  def __init__(self, model: GanModel, depth: int = 2, use_graph: bool = False, target_domain: str = 't'):
     from .prefetch import HostReturner
     self.model, self.depth = model, depth
+    self.target_domain = check_target_domain(target_domain)
     self.feed = None
     self.back = HostReturner(model.device, depth)
     self.use_graph = bool(use_graph) and model.device.type == 'cuda'
@@ -598,7 +613,7 @@ class InferencePipeline(object):
 
   def _infer(self, x):
     if not self.use_graph:
-      return self.model.infer(x)
+      return self.model.infer(x, self.target_domain)
     key = tuple(x.shape)
     ent = self._graphs.get(key)
     if ent is None:
@@ -608,10 +623,10 @@ class InferencePipeline(object):
       side.wait_stream(torch.cuda.current_stream(dev))
       with torch.cuda.stream(side):
         for _ in range(2):                              # warm-up on the capture stream (lazy one-time set-up, allocator)
-          self.model.infer(static_in)
+          self.model.infer(static_in, self.target_domain)
         graph = torch.cuda.CUDAGraph()
         graph.capture_begin()
-        static_out = self.model.infer(static_in)
+        static_out = self.model.infer(static_in, self.target_domain)
         graph.capture_end()
       torch.cuda.current_stream(dev).wait_stream(side)
       ent = (graph, static_in, static_out)
