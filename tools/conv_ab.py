@@ -45,9 +45,13 @@ def worker(lib_path, batch, iters):
   st = ops._st()
   res = {}
   for case in product_cases():
-    entry, H, W, Cin, Cout, k, pad, opts = case
+    entry = case[0]
+    if entry == 'twg_conv_wgrad_planes':     # weight-gradient keys carry their batch (it sets the pixel split)
+      N, H, W, Cin, Cout, k, pad, opts = case[1:]
+    else:
+      H, W, Cin, Cout, k, pad, opts = case[1:]
+      N = batch
     opts = set(opts.split('+')) - {''}
-    N = batch
     seed = int(hashlib.sha256(repr(case).encode()).hexdigest()[:8], 16)
     gen = torch.Generator(device=dev).manual_seed(seed)
     rnd = lambda *shape, s=1.0: torch.randn(shape, device=dev, generator=gen) * s

@@ -51,8 +51,8 @@ def conv_traffic(entry, N, H, W, Cin, Cout, k, pad):
   """{'flops', 'hbm', 'l2_before', 'l2_after', 'cols'} of one tensor-core conv launch.
   flops: 2 MACs per product of the convolution (not the 3 split-bf16 MMAs).  hbm: algorithmic bytes, every operand read and
   every result written once (split planes 4 B per element, fp32 results 4 B).  l2_*: bytes the kernel's TMA loads move from
-  L2 into shared memory, per CTA work item summed over the grid, with the per-tap kernel (before) and the kernel the shape
-  takes (after).  cols: the shape takes the column-box kernel."""
+  L2 into shared memory, per CTA work item summed over the grid (resident weights: once per CTA), with the per-tap kernel
+  (before) and the kernel the shape takes (after).  cols: the shape takes the column-box kernel."""
   TW, TH, TN, tiles = _tiles(N, H, W)
   taps, px = k * k, N * H * W
   flops = 2.0 * px * Cin * Cout * taps
@@ -73,7 +73,9 @@ def conv_traffic(entry, N, H, W, Cin, Cout, k, pad):
   weights = taps * 2 * BN * K * 2                                 # one weight tile per (tap, chunk), hi and lo
   before = items * (taps * 2 * 128 * K * 2 + weights)            # one shifted 128-pixel A tile per (tap, chunk)
   cols = k == 3 and pad == 1 and K == CC and TW == 16 and TH == 8 and TN == 1 and H >= 10
-  after = items * (3 * 2 * 160 * K * 2 + weights) if cols else before   # three {K, 16, 10} column boxes per tile
+  # the column-box keys with one small weight block (cols_resident) load it once per persistent CTA (one per SM)
+  w_loads = min(items, 132) if cols and K <= 32 and BN <= 64 else items
+  after = items * 3 * 2 * 160 * K * 2 + w_loads * weights if cols else before   # three {K, 16, 10} column boxes per tile
   return {'flops': flops, 'hbm': 4.0 * px * (K + Nc) + 4.0 * taps * K * Nc, 'l2_before': float(before),
           'l2_after': float(after), 'cols': cols}
 

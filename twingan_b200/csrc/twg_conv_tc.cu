@@ -479,7 +479,8 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_fwd_wgmma(const __grid_con
 // operand values, so the results are bit-identical to it.
 // The CTAs are persistent: CTA b computes work items b, b + gridDim.x, ... (item = tile + tiles * output-channel block),
 // each exactly once; the A boxes are double-buffered where they fit (CC <= 32), so the next tile's boxes load while the
-// current one computes, and weight tiles stream through their own per-tap ring.
+// current one computes, and weight tiles stream through their own per-tap ring.  The keys with a small single weight block
+// keep it in shared memory instead (cols_resident, conv_cols_resident below).
 template <int CC, int BN>
 struct ColSmem {
   static constexpr int kBox = 160 * CC * 2;                         // one box, one plane
@@ -495,6 +496,176 @@ struct ColSmem {
   static_assert(kBytes <= 227 * 1024, "column-box conv exceeds shared memory");
 };
 
+// The keys with one output-channel block (BN == Cout <= 64) and a chunk of CC <= 32 keep all 9 hi / lo weight tiles (at
+// most 72 KB) in shared memory for the CTA's lifetime instead of streaming them through the per-tap ring for every tile,
+// and still fit two or more A buffers beside them.  (At CC = 64 one A buffer is 120 KB: with resident weights it stays a
+// single buffer, and on an H100 that measured no faster than the streaming kernel, so CC = 64 keeps that.)  Where two
+// 128-row accumulators fit in registers (BN <= 32; at BN = 64 ptxas spills) each consumer warpgroup also takes a tile
+// stream of its own.
+__host__ __device__ constexpr bool cols_resident(int cc, int bn) { return cc <= 32 && bn <= 64; }
+__host__ __device__ constexpr bool cols_dual(int cc, int bn) { return cols_resident(cc, bn) && bn <= 32; }
+
+template <int CC, int BN>
+struct ColResSmem {
+  static constexpr int kBox = 160 * CC * 2;                         // one box, one plane
+  static constexpr int kABuf = 6 * kBox;                            // [hi: kw 0, 1, 2][lo: kw 0, 1, 2]
+  static constexpr int kBTileRaw = BN * CC * 2;
+  static constexpr int kBTile = (kBTileRaw + 1023) / 1024 * 1024;
+  static constexpr int kW = 9 * 2 * kBTile;                         // [tap][hi, lo]
+  static constexpr int kABufsRaw = (220 * 1024 - kW) / kABuf;
+  static constexpr int kABufs = kABufsRaw > 4 ? 4 : kABufsRaw;
+  static constexpr int kBytes = kW + kABufs * kABuf + 1024 /*align*/ + 256 /*barriers*/;
+  static_assert(kABufs >= 2, "column-box conv: too few A buffers beside the weights");
+  static_assert(kBytes <= 227 * 1024, "column-box conv exceeds shared memory");
+};
+
+template <int CC, int BN>
+constexpr int col_smem_bytes() {
+  if constexpr (cols_resident(CC, BN)) return ColResSmem<CC, BN>::kBytes;
+  else return ColSmem<CC, BN>::kBytes;
+}
+
+// One accumulation chain of the resident-weight consumer: taps J0 .. J0 + NST - 1 of the warpgroup's KB m64 blocks, all
+// issued before one wait, each block into its own fragment part[b] that is then added to acc[b] (mma_chain's chains and
+// per-block MMA order, without its per-stage handshakes: weights and A boxes are resident for the whole tile).
+// operands(tap, b, dah, dal, dbh, dbl) gives block b's A hi / lo and the tap's B hi / lo descriptors.
+template <int BN, int CC, int KB, int J0, int NST, class Operands>
+__device__ __forceinline__ void mma_chain_resident(float (&acc)[KB][BN / 2], float (&part)[KB][BN / 2],
+                                                   const Operands& operands) {
+  wgmma_fence();
+#pragma unroll
+  for (int j = 0; j < NST; ++j) {
+#pragma unroll
+    for (int b = 0; b < KB; ++b) {
+      uint64_t dah, dal, dbh, dbl;
+      operands(J0 + j, b, dah, dal, dbh, dbl);
+      asm volatile("" : "+l"(dah), "+l"(dal), "+l"(dbh), "+l"(dbl));
+#pragma unroll
+      for (int ks = 0; ks < CC / 16; ++ks) {
+        const uint32_t off = ks * 32;   // 16 bf16 along K inside the swizzle atom
+        Wgmma<BN>::template mma<0, 0>(part[b], desc_add(dal, off), desc_add(dbh, off));
+        Wgmma<BN>::template mma<0, 0>(part[b], desc_add(dah, off), desc_add(dbl, off));
+        Wgmma<BN>::template mma<0, 0>(part[b], desc_add(dah, off), desc_add(dbh, off));
+      }
+    }
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+#pragma unroll
+  for (int b = 0; b < KB; ++b) {
+    fence_acc(part[b]);
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) { acc[b][i] += part[b][i]; part[b][i] = 0.f; }
+    fence_acc(part[b]);
+  }
+}
+
+// Column-box forward / dgrad with resident weights (cols_resident keys).  The producer loads the 9 hi / lo weight tiles
+// once, under one mbarrier, then the CTA's tiles' A boxes in order through a ring of kABufs buffers.
+//   dual (BN <= 32): warpgroup wg takes every other work item of the CTA (items wg, wg + 2, ...) and computes all 128 rows
+//     of it as two m64 blocks with two accumulators, so one warpgroup's epilogue overlaps the other's MMAs.
+//   otherwise (BN = 64): both warpgroups share every item, 64 rows each, as in the streaming kernel.
+// Block r (rows 64 r .. 64 r + 63) is computed and stored exactly as consumer warpgroup r of the streaming kernel does it --
+// same MMAs in the same order on the same operands, same statistics slots (warp 4 r + warp % 4) -- so every output is
+// bit-identical to it.
+template <int CC, int BN>
+__device__ __forceinline__ void conv_cols_resident(uint8_t* smem, const CUtensorMap* tm_a_hi, const CUtensorMap* tm_a_lo,
+                                                   const CUtensorMap* tm_b_hi, const CUtensorMap* tm_b_lo,
+                                                   float* __restrict__ y, const TcGeom& g, const float* __restrict__ bias,
+                                                   int act, void* __restrict__ z_planes, float4* __restrict__ stats,
+                                                   uint8_t* __restrict__ act_mask, const float* __restrict__ aff_a) {
+  using SM = ColResSmem<CC, BN>;
+  constexpr int kABufs = SM::kABufs;
+  constexpr bool kDual = cols_dual(CC, BN);
+  constexpr int KB = kDual ? 2 : 1;                                      // m64 blocks per warpgroup and item
+  uint8_t* sw = smem + kABufs * SM::kABuf;                                 // weights [tap][hi, lo]
+  uint64_t* afull = reinterpret_cast<uint64_t*>(sw + SM::kW);              // [kABufs]
+  uint64_t* aempty = afull + kABufs;                                       // [kABufs]
+  uint64_t* wfull = aempty + kABufs;                                       // [1]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tiles = g.tiles_w * g.tiles_h * g.tiles_n;   // == work items: one output-channel block
+
+  if (warp == kConsumerWarps && lane == 0) {
+    prefetch_tmap(tm_a_hi); prefetch_tmap(tm_a_lo); prefetch_tmap(tm_b_hi); prefetch_tmap(tm_b_lo);
+    for (int s = 0; s < kABufs; ++s) { mbar_init(&afull[s], 1); mbar_init(&aempty[s], kDual ? 4 : kConsumerWarps); }
+    mbar_init(wfull, 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp == kConsumerWarps) {
+    if (lane == 0) {
+      mbar_expect_tx(wfull, 18 * SM::kBTileRaw);
+      for (int tap = 0; tap < 9; ++tap) {
+        tma_load_2d(tm_b_hi, wfull, sw + (2 * tap) * SM::kBTile, 0, tap * BN);
+        tma_load_2d(tm_b_lo, wfull, sw + (2 * tap + 1) * SM::kBTile, 0, tap * BN);
+      }
+      int ab = 0; uint32_t aph = 0;
+      for (int u = blockIdx.x; u < tiles; u += gridDim.x) {
+        const int tw_i = u % g.tiles_w, th_i = (u / g.tiles_w) % g.tiles_h, n0 = u / (g.tiles_w * g.tiles_h);
+        const int w0 = tw_i * 16, h0 = th_i * 8;
+        mbar_wait(&aempty[ab], aph ^ 1);
+        mbar_expect_tx(&afull[ab], SM::kABuf);
+        uint8_t* sa = smem + ab * SM::kABuf;
+        for (int kw = 0; kw < 3; ++kw) {
+          tma_load_4d(tm_a_hi, &afull[ab], sa + kw * SM::kBox, 0, w0 + kw - 1, h0 - 1, n0);
+          tma_load_4d(tm_a_lo, &afull[ab], sa + (3 + kw) * SM::kBox, 0, w0 + kw - 1, h0 - 1, n0);
+        }
+        if (++ab == kABufs) { ab = 0; aph ^= 1; }
+      }
+    }
+    return;
+  }
+
+  const int wg = warp >> 2;
+  constexpr uint32_t layout = swizzle_layout_for(CC);
+  constexpr uint32_t sbo = 8 * CC * 2;     // 8 rows of CC bf16
+  // tap 0's hi weight tile; tap t's hi / lo tiles are 2 t / 2 t + 1 tiles further
+  const uint64_t dbh0 = make_desc(smem_u32(sw), 16, sbo, layout);
+  // item i of the CTA (work item blockIdx.x + i gridDim.x) sits in A buffer i % kABufs, phase (i / kABufs) & 1.  A
+  // warpgroup waits for its items in order, and the producer loads all items in order, so by the time it waits for item i
+  // item i - kABufs (<= its previous item when kABufs >= 2) has been loaded and the parity names the right phase.
+  const int i0 = kDual ? wg : 0, di = kDual ? 2 : 1;
+  bool weights_ready = false;
+  for (int i = i0, u = blockIdx.x + i0 * gridDim.x; u < tiles; i += di, u += di * gridDim.x) {
+    const int tw_i = u % g.tiles_w, th_i = (u / g.tiles_w) % g.tiles_h, n0 = u / (g.tiles_w * g.tiles_h);
+    const int ab = i % kABufs;
+    if (!weights_ready) { mbar_wait(wfull, 0); weights_ready = true; }
+    float acc[KB][BN / 2], part[KB][BN / 2];
+#pragma unroll
+    for (int b = 0; b < KB; ++b)
+#pragma unroll
+      for (int j = 0; j < BN / 2; ++j) { acc[b][j] = 0.f; part[b][j] = 0.f; }
+    mbar_wait(&afull[ab], (uint32_t)(i / kABufs) & 1u);
+    // hi box 0 from pixel row 0; block r's tap (kh, kw) view starts kw boxes and 16 (kh + 4 r) pixel rows further
+    const uint64_t dah0 = make_desc(smem_u32(smem + ab * SM::kABuf), 16, sbo, layout);
+    // the weight descriptors are the same for every item: hidden from the compiler per item, so that it does not hoist
+    // them out of the loop into registers the accumulators need (mma_chain_resident does the same per tap)
+    uint64_t dbt = dbh0;
+    asm volatile("" : "+l"(dbt));
+    const auto operands = [&](int tap, int b, uint64_t& dah, uint64_t& dal, uint64_t& dbh, uint64_t& dbl) {
+      const int kh = tap / 3, kw = tap - kh * 3;
+      const int r = kDual ? b : wg;
+      dah = desc_add(dah0, kw * SM::kBox + (kh + 4 * r) * (16 * CC * 2)); dal = desc_add(dah, 3 * SM::kBox);
+      dbh = desc_add(dbt, 2 * tap * SM::kBTile); dbl = desc_add(dbh, SM::kBTile);
+    };
+    // taps 0-3, 4-7 and 8: the chains of k_conv_fwd_wgmma
+    mma_chain_resident<BN, CC, KB, 0, 4>(acc, part, operands);
+    mma_chain_resident<BN, CC, KB, 4, 4>(acc, part, operands);
+    mma_chain_resident<BN, CC, KB, 8, 1>(acc, part, operands);
+    // every MMA of the item has completed: its A buffer goes back to the producer
+    __syncwarp();
+    mbar_arrive_lane0(&aempty[ab], lane);
+#pragma unroll
+    for (int b = 0; b < KB; ++b) {
+      const int r = kDual ? b : wg;
+      fwd_epilogue<BN>(acc[b], y, g, tw_i, th_i, n0, 0, 4 * r + (warp & 3), lane, bias, act, z_planes, stats, act_mask,
+                       aff_a);
+    }
+  }
+}
+
 template <int CC, int BN>
 __global__ void __launch_bounds__(kThreads, 1) k_conv_fwd_cols_wgmma(const __grid_constant__ CUtensorMap tm_a_hi,
                                                                      const __grid_constant__ CUtensorMap tm_a_lo,
@@ -505,10 +676,15 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv_fwd_cols_wgmma(const __gri
                                                                      void* __restrict__ z_planes, float4* __restrict__ stats,
                                                                      uint8_t* __restrict__ act_mask,
                                                                      const float* __restrict__ aff_a) {
-  using SM = ColSmem<CC, BN>;
-  constexpr int kABufs = SM::kABufs, kWStages = SM::kWStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  if constexpr (cols_resident(CC, BN)) {
+    conv_cols_resident<CC, BN>(smem, &tm_a_hi, &tm_a_lo, &tm_b_hi, &tm_b_lo, y, g, bias, act, z_planes, stats, act_mask,
+                               aff_a);
+    return;
+  }
+  using SM = ColSmem<CC, BN>;
+  constexpr int kABufs = SM::kABufs, kWStages = SM::kWStages;
   uint8_t* sw = smem + kABufs * SM::kABuf;                                     // weight ring [kWStages][hi][lo]
   uint64_t* afull = reinterpret_cast<uint64_t*>(sw + kWStages * SM::kWStage);  // [kABufs]
   uint64_t* aempty = afull + kABufs;                                           // [kABufs]
@@ -1124,21 +1300,23 @@ template <int CC, int BN>
 static int launch_fwd_cols(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl,
                            float* y, const TcGeom& g, const float* bias, int act, void* z_planes, float4* stats,
                            uint8_t* act_mask, const float* aff_a, cudaStream_t st) {
-  using SM = ColSmem<CC, BN>;
+  constexpr int kBytes = col_smem_bytes<CC, BN>();
+  // the resident-weight kernel holds one output-channel block, at weight rows tap * BN
+  if (cols_resident(CC, BN) && g.Cout != BN) return fail(TWG_ERR_UNSUPPORTED, "tensor-core conv: column-box Cout != BN");
   auto kern = k_conv_fwd_cols_wgmma<CC, BN>;
   static std::once_flag once;                 // one-time attribute set-up, safe from several host threads
   static cudaError_t attr_err = cudaSuccess;
   static int per_sm = 1;
   std::call_once(once, [&] {
-    attr_err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::kBytes);
+    attr_err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kBytes);
     if (attr_err == cudaSuccess)
-      attr_err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, SM::kBytes);
+      attr_err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, kBytes);
     if (per_sm < 1) per_sm = 1;
   });
   if (attr_err != cudaSuccess) return fail(TWG_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(attr_err));
   const int64_t work = (int64_t)g.tiles_w * g.tiles_h * g.tiles_n * (g.Cout / BN);
   const int64_t ctas = work < (int64_t)kNumSMs * per_sm ? work : (int64_t)kNumSMs * per_sm;
-  kern<<<(unsigned)ctas, kThreads, SM::kBytes, st>>>(ah, al, bh, bl, y, g, bias, act, z_planes, stats, act_mask, aff_a);
+  kern<<<(unsigned)ctas, kThreads, kBytes, st>>>(ah, al, bh, bl, y, g, bias, act, z_planes, stats, act_mask, aff_a);
   return check_launch("twg_conv tc cols");
 }
 
