@@ -759,11 +759,13 @@ def train_step(cfg: Config, params, adam_m, adam_v, norm_state, sources, targets
   return g_loss, d_loss, named, grads, t
 
 
-def inference(cfg: Config, params, norm_state, sources: Tensor) -> Tensor:
-  """inference/image_translation_infer.py:46-99 compute: G(E(x;'_s',eval);'_t',eval, skips) (twingan.py:310-365)."""
+def inference(cfg: Config, params, norm_state, sources: Tensor, target_domain: str = 't') -> Tensor:
+  """inference/image_translation_infer.py:46-99 compute (twingan.py:310-365): target_domain 't',
+  G(E(x;'_s',eval);'_t',eval, skips); 's', G(E(x;'_t',eval);'_s',eval, skips), `sources` then being target images."""
+  src, dst = {'t': ('_s', '_t'), 's': ('_t', '_s')}[target_domain]
   nets = Nets(cfg, params, norm_state)
-  code, ep = nets.encoder(sources, '_s', is_training=False)
-  out, _ = nets.generator(code, '_t', ep if cfg.use_unet else None, is_training=False)
+  code, ep = nets.encoder(sources, src, is_training=False)
+  out, _ = nets.generator(code, dst, ep if cfg.use_unet else None, is_training=False)
   return out
 
 

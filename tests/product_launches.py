@@ -28,6 +28,72 @@ _FLAG_VARIANTS = (
 )
 _FLAG_STAGES = ((256, False), (64, True))          # one stable and one growing resolution, each with the cycle GAN loss
 _INFER_BATCHES = (64, 1, 37)                       # the SWD evaluation's default batch, single images, a partial batch
+_INFER_ALPHAS = (0.5, 1.0)                         # mid fade-in, and a growing stage's last step
+_S_DIRECTION_GROWING_HW = 64                       # the growing stage that also runs the target -> source direction
+_SWD_RESOLUTIONS = (16, 32, 64, 128, 256)
+_SWD_IMAGES = 70                                   # one batch of 64 and a ragged one of 6; even, for the real floor
+
+
+def inference_configs():
+  """The evaluation-mode configurations of the harvest after the 256x256 one, in order: (label, hw, growing, alpha,
+  target_domain, Flags keyword arguments).  GanModel.infer at every stage of pggan_runner.stage_plan(4, 256), as the SWD
+  hook runs it during training and translate / swd_eval run it on a stage checkpoint: growing stages at alpha 0.5 and
+  1.0, the four normaliser / residual variants, direction 't', and 's' at the 256x256 stable stage and one growing
+  stage."""
+  from twingan_b200 import pggan_runner as R
+  out = []
+  for s in R.stage_plan(4, 256):
+    for norm, res in _VARIANTS:
+      for alpha in (_INFER_ALPHAS if s.is_growing else (0.0,)):
+        dirs = ('t', 's') if (s.hw == 256 and not s.is_growing) or (
+            s.hw == _S_DIRECTION_GROWING_HW and s.is_growing and alpha == _INFER_ALPHAS[0]) else ('t',)
+        for d in dirs:
+          label = 'inference %s%s %s%s %s' % (s.name, ' alpha=%g' % alpha if s.is_growing else '', norm,
+                                              ' res' if res else '', d)
+          out.append((label, s.hw, s.is_growing, alpha, d, {'generator_norm_type': norm, 'use_res_block': res}))
+  return out
+
+
+def _harvest_inference(gen):
+  """Launches GanModel.infer for every configuration of inference_configs() on _INFER_BATCHES; yields each label before
+  its launches."""
+  from twingan_b200 import twingan
+  model, built = None, None
+  for label, hw, growing, alpha, d, kw in inference_configs():
+    if built != (hw, growing, tuple(sorted(kw.items()))):
+      del model
+      model = twingan.GanModel(twingan.Flags(train_image_size=hw, is_growing=growing, **kw), device=DEV)
+      built = (hw, growing, tuple(sorted(kw.items())))
+    model.flags.alpha_grow = alpha
+    for n in _INFER_BATCHES:
+      yield '%s batch %d' % (label, n)
+      model.infer(torch.rand((n, hw, hw, 3), device=DEV, generator=gen), target_domain=d)
+  del model
+
+
+def _harvest_swd(gen):
+  """The launches of the SWD hook (swd.evaluate_translation): one SlicedWasserstein per resolution, with the real-vs-real
+  floor, fed in batches of 64 and a ragged last batch."""
+  from twingan_b200 import swd
+  for R in _SWD_RESOLUTIONS:
+    yield 'swd %d images=%d' % (R, _SWD_IMAGES)
+    sw = swd.SlicedWasserstein(R, _SWD_IMAGES, DEV, seed=R, real_floor=True)
+    for i in range(0, _SWD_IMAGES, 64):
+      n = min(64, _SWD_IMAGES - i)
+      for kind in swd.KINDS:
+        sw.feed(kind, torch.rand((n, R, R, 3), device=DEV, generator=gen))
+    sw.result()
+
+
+def _harvest_translate_front_end():
+  """The uint8 front end and quantisation of `python -m twingan_b200.translate` on one small ragged batch."""
+  import numpy as np
+  from twingan_b200 import ops
+  yield 'translate front end'
+  rng = np.random.default_rng(0)
+  images = [rng.integers(0, 256, (h, w, 3), dtype=np.uint8) for h, w in ((37, 50), (32, 32), (5, 71))]
+  payload, table = ops.pack_images(images)
+  ops.batch_to_u8(ops.images_u8_to_batch(payload.to(DEV), table, 32))
 
 
 def harvest_configs():
@@ -62,8 +128,9 @@ def harvest_configs():
 def harvest_product_launches():
   """(entry point, args) of every L.call, in order, of one eager training step per configuration of harvest_configs()
   (growing at alpha 0.5), each followed by its EMA pushes and its optimiser apply, and of inference at 256x256 on batches of
-  64, 1 and 37 images (instance norm, batch renorm, batch norm).  Cached for the session; launch_configs() names the
-  configuration of each launch."""
+  64, 1 and 37 images (instance norm, batch renorm, batch norm); then of inference at every stage
+  (inference_configs()), of the SWD evaluation at every resolution from 16 to 256 and of the translate front end.
+  Cached for the session; launch_configs() names the configuration of each launch."""
   global _LAUNCHES, _CONFIGS, HARVEST_SECONDS
   if _LAUNCHES is not None:
     return _LAUNCHES
@@ -99,6 +166,9 @@ def harvest_product_launches():
         label[0] = 'inference 256 %s batch %d' % (norm, n)
         model.infer(torch.rand((n, 256, 256, 3), device=DEV, generator=gen))
       del model
+    for part in (_harvest_inference(gen), _harvest_swd(gen), _harvest_translate_front_end()):
+      for label[0] in part:      # each part yields a label, then launches under it when resumed
+        pass
     torch.cuda.synchronize()
   finally:
     del L.call

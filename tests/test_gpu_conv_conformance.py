@@ -424,22 +424,22 @@ PRODUCT_CONVS = {
         32, 3, 128, 1, 0, ''), (4, 4, 256, 3, 1, 0, ''), (4, 4, 3, 256, 1, 0, ''), (64, 64, 3, 64, 1, 0, ''), (64, 64, 64,
         3, 1, 0, ''), (8, 8, 256, 3, 1, 0, ''), (8, 8, 3, 256, 1, 0, '')],
     'twg_conv_fwd_planes': [
-        (1, 1, 4096, 256, 1, 0, 'ragged'), (128, 128, 128, 32, 1, 0, 'bias'), (128, 128, 128, 32, 3, 1, ''), (128, 128, 32,
-        32, 3, 1, ''), (128, 128, 32, 32, 3, 1, 'bias+act+zp+mask'), (128, 128, 32, 32, 3, 1, 'stats'), (128, 128, 32, 64,
-        1, 0, ''), (128, 128, 32, 64, 1, 0, 'bias'), (128, 128, 32, 64, 3, 1, ''), (128, 128, 32, 64, 3, 1,
-        'bias+act+mask'), (128, 128, 32, 64, 3, 1, 'stats'), (16, 16, 256, 256, 3, 1, ''), (16, 16, 512, 256, 1, 0, ''),
-        (16, 16, 512, 256, 1, 0, 'bias'), (16, 16, 512, 256, 3, 1, ''), (256, 256, 16, 16, 3, 1, ''), (256, 256, 16, 16, 3,
-        1, 'bias+act+zp+mask'), (256, 256, 16, 16, 3, 1, 'stats'), (256, 256, 16, 32, 1, 0, ''), (256, 256, 16, 32, 1, 0,
-        'bias'), (256, 256, 16, 32, 3, 1, ''), (256, 256, 16, 32, 3, 1, 'bias+act+mask'), (256, 256, 16, 32, 3, 1, 'stats'),
-        (256, 256, 64, 16, 1, 0, 'bias'), (256, 256, 64, 16, 3, 1, ''), (256, 256, 64, 16, 3, 1, 'stats'), (32, 32, 128,
-        128, 3, 1, ''), (32, 32, 128, 128, 3, 1, 'bias+act+zp'), (32, 32, 128, 256, 1, 0, ''), (32, 32, 128, 256, 1, 0,
-        'bias'), (32, 32, 128, 256, 3, 1, ''), (32, 32, 128, 256, 3, 1, 'bias+act'), (32, 32, 512, 128, 1, 0, ''), (32, 32,
-        512, 128, 1, 0, 'bias'), (32, 32, 512, 128, 3, 1, ''), (4, 4, 256, 256, 3, 1, ''), (4, 4, 256, 256, 3, 1, 'ragged'),
-        (4, 4, 384, 256, 3, 1, ''), (4, 4, 384, 256, 3, 1, 'ragged'), (64, 64, 256, 64, 1, 0, 'bias'), (64, 64, 256, 64, 3,
-        1, ''), (64, 64, 64, 128, 1, 0, ''), (64, 64, 64, 128, 1, 0, 'bias'), (64, 64, 64, 128, 3, 1, ''), (64, 64, 64, 128,
-        3, 1, 'bias+act'), (64, 64, 64, 64, 3, 1, ''), (64, 64, 64, 64, 3, 1, 'bias+act+zp'), (8, 8, 256, 256, 3, 1, ''),
-        (8, 8, 256, 256, 3, 1, 'ragged'), (8, 8, 512, 256, 1, 0, ''), (8, 8, 512, 256, 3, 1, ''), (8, 8, 512, 256, 3, 1,
-        'ragged')],
+        (1, 1, 4096, 256, 1, 0, 'ragged'), (128, 128, 128, 32, 1, 0, ''), (128, 128, 128, 32, 1, 0, 'bias'), (128, 128, 128,
+        32, 3, 1, ''), (128, 128, 32, 32, 3, 1, ''), (128, 128, 32, 32, 3, 1, 'bias+act+zp+mask'), (128, 128, 32, 32, 3, 1,
+        'stats'), (128, 128, 32, 64, 1, 0, ''), (128, 128, 32, 64, 1, 0, 'bias'), (128, 128, 32, 64, 3, 1, ''), (128, 128,
+        32, 64, 3, 1, 'bias+act+mask'), (128, 128, 32, 64, 3, 1, 'stats'), (16, 16, 256, 256, 3, 1, ''), (16, 16, 512, 256,
+        1, 0, ''), (16, 16, 512, 256, 1, 0, 'bias'), (16, 16, 512, 256, 3, 1, ''), (256, 256, 16, 16, 3, 1, ''), (256, 256,
+        16, 16, 3, 1, 'bias+act+zp+mask'), (256, 256, 16, 16, 3, 1, 'stats'), (256, 256, 16, 32, 1, 0, ''), (256, 256, 16,
+        32, 1, 0, 'bias'), (256, 256, 16, 32, 3, 1, ''), (256, 256, 16, 32, 3, 1, 'bias+act+mask'), (256, 256, 16, 32, 3, 1,
+        'stats'), (256, 256, 64, 16, 1, 0, ''), (256, 256, 64, 16, 1, 0, 'bias'), (256, 256, 64, 16, 3, 1, ''), (256, 256,
+        64, 16, 3, 1, 'stats'), (32, 32, 128, 128, 3, 1, ''), (32, 32, 128, 128, 3, 1, 'bias+act+zp'), (32, 32, 128, 256, 1,
+        0, ''), (32, 32, 128, 256, 1, 0, 'bias'), (32, 32, 128, 256, 3, 1, ''), (32, 32, 128, 256, 3, 1, 'bias+act'), (32,
+        32, 512, 128, 1, 0, ''), (32, 32, 512, 128, 1, 0, 'bias'), (32, 32, 512, 128, 3, 1, ''), (4, 4, 256, 256, 3, 1, ''),
+        (4, 4, 256, 256, 3, 1, 'ragged'), (4, 4, 384, 256, 3, 1, ''), (4, 4, 384, 256, 3, 1, 'ragged'), (64, 64, 256, 64, 1,
+        0, ''), (64, 64, 256, 64, 1, 0, 'bias'), (64, 64, 256, 64, 3, 1, ''), (64, 64, 64, 128, 1, 0, ''), (64, 64, 64, 128,
+        1, 0, 'bias'), (64, 64, 64, 128, 3, 1, ''), (64, 64, 64, 128, 3, 1, 'bias+act'), (64, 64, 64, 64, 3, 1, ''), (64,
+        64, 64, 64, 3, 1, 'bias+act+zp'), (8, 8, 256, 256, 3, 1, ''), (8, 8, 256, 256, 3, 1, 'ragged'), (8, 8, 512, 256, 1,
+        0, ''), (8, 8, 512, 256, 1, 0, 'ragged'), (8, 8, 512, 256, 3, 1, ''), (8, 8, 512, 256, 3, 1, 'ragged')],
     'twg_conv_wgrad': [
         (12, 1, 1, 256, 1, 1, 0, 'accumulate'), (12, 128, 128, 3, 32, 1, 0, 'accumulate'), (12, 128, 128, 32, 3, 1, 0,
         'accumulate'), (12, 256, 256, 16, 3, 1, 0, 'accumulate'), (12, 256, 256, 3, 16, 1, 0, 'accumulate'), (12, 32, 32, 3,

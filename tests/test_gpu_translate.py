@@ -88,9 +88,7 @@ def test_target_to_source_direction_matches_the_oracle(built_lib, norm):
   params = O.init_params(cfg, randomize_affine=True)
   state = O.init_norm_state(cfg, seed=5)
   _, tgt, _ = O.make_inputs(cfg, 3, seed=2)
-  nets = O.Nets(cfg, params, state)
-  code, ep = nets.encoder(tgt, '_t', is_training=False)
-  ref_s, _ = nets.generator(code, '_s', ep, is_training=False)
+  ref_s = O.inference(cfg, params, state, tgt, target_domain='s')
   ref_t = O.inference(cfg, params, state, tgt)
   model = twingan.GanModel(twingan.Flags(train_image_size=32, pggan_max_num_channels=32, generator_norm_type=norm),
                            device=DEV)
