@@ -22,49 +22,6 @@ namespace twg {
 // ----------------------------------------------------------------------------------------------------
 // PTX wrappers
 // ----------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// one arrive per warp, from lane 0, as a predicated instruction rather than a branch: between the MMAs of a chain a branch
-// costs registers (k_conv_fwd_cols_wgmma<16, 128> spills with `if (lane == 0) mbar_arrive(bar)`)
-__device__ __forceinline__ void mbar_arrive_lane0(uint64_t* bar, int lane) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.eq.s32 p, %1, 0;\n@p mbarrier.arrive.shared::cta.b64 _, [%0];\n}\n"
-      ::"r"(smem_u32(bar)), "r"(lane) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  // try_wait suspends for a bounded time per attempt; a pipeline bug must surface as a trap, never as a hung GPU
-  uint32_t done = 0;
-  uint64_t t0 = 0;
-  for (uint32_t spin = 0; !done; ++spin) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-        "selp.u32 %0, 1, 0, p;\n"
-        "}\n"
-        : "=r"(done)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    if (!done && (spin & 1023) == 1023) {
-      uint64_t now;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
-      if (t0 == 0) t0 = now;
-      else if (now - t0 > 2000000000ull) __trap();    // 2 s without progress: abort the kernel (no printf here: a call
-                                                      // in the kernel would serialise the wgmma pipeline)
-    }
-  }
-}
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-
 __device__ __forceinline__ void tma_load_4d(const CUtensorMap* tm, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3) {
   asm volatile(
       "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"

@@ -5,6 +5,7 @@
 #include <cooperative_groups.h>
 
 #include "twg_common.cuh"
+#include "twg_stream.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -659,6 +660,41 @@ __global__ void __launch_bounds__(256) k_sum_sq(const float* __restrict__ x, dou
   if (threadIdx.x == 0) { out2[0] = (double)a1; out2[1] = (double)a2; }     // launched as one block
 }
 
+// k_sum_sq as one block with x arriving through a StreamRing (twelve stages of 16 KB): thread t adds x[t], x[t + 256],
+// ... in that order, as in k_sum_sq launched as one block, so the two sums are the same bits.  One block of direct scalar
+// loads walks the batch at the latency of one load per element per thread.
+constexpr int kSumSqStages = 12;
+__global__ void __launch_bounds__(256) k_sum_sq_stream(const float* __restrict__ x, double* __restrict__ out2, int64_t n) {
+  extern __shared__ __align__(128) unsigned char ring_mem[];
+  __shared__ float sm[32];
+  constexpr int kPer = kStreamStage / 4 / 256;          // elements of a stage per thread
+  StreamRing<1, kSumSqStages> ring;
+  const void* const arrays[1] = {x};
+  ring.start(ring_mem, arrays, n * 4);
+  float a1 = 0.f, a2 = 0.f;
+  for (int k = 0; k < ring.chunks; ++k) {
+    ring.wait(k);
+    const float* xs = reinterpret_cast<const float*>(ring.at(k, 0));
+    const int64_t left = n - (int64_t)k * (kStreamStage / 4);
+    float v[kPer];
+#pragma unroll
+    for (int j = 0; j < kPer; ++j) {
+      const int i = j * 256 + threadIdx.x;
+      v[j] = xs[i < left ? i : 0];
+    }
+    ring.release(k);
+#pragma unroll
+    for (int j = 0; j < kPer; ++j) {
+      if (j * 256 + (int)threadIdx.x >= left) continue;
+      a1 += v[j];
+      a2 += v[j] * v[j];
+    }
+  }
+  a1 = block_sum(a1, sm);
+  a2 = block_sum(a2, sm);
+  if (threadIdx.x == 0) { out2[0] = (double)a1; out2[1] = (double)a2; }
+}
+
 __global__ void __launch_bounds__(256) k_dragan_xhat(const float* __restrict__ x, const float* __restrict__ alpha,
                                                      const float* __restrict__ noise, float* __restrict__ xhat,
                                                      const double* __restrict__ s2, int N, int64_t per) {
@@ -1118,7 +1154,17 @@ int twg_dragan_xhat(const float* x, const float* alpha, const float* noise, floa
   double* s2 = reinterpret_cast<double*>(scratch2);  // caller provides >= 16 bytes, 8-byte aligned
   cudaMemsetAsync(s2, 0, 16, S(stream));
   const int64_t total = (int64_t)N * per_sample;
-  k_sum_sq<<<1, 256, 0, S(stream)>>>(x, s2, total);     // one block: the sums come out the same on every run
+  // one block: the sums come out the same on every run.  The bulk copies of the streamed form move whole 16-byte units.
+  if (stream_fills(total * 4) && total % 4 == 0 && reinterpret_cast<uintptr_t>(x) % 16 == 0) {
+    constexpr int kBytes = StreamRing<1, kSumSqStages>::kBytes;
+    static std::once_flag once;
+    static cudaError_t attr_err = cudaSuccess;
+    if (allow_ring(k_sum_sq_stream, kBytes, once, attr_err) != cudaSuccess)
+      return fail(TWG_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(attr_err));
+    k_sum_sq_stream<<<1, 256, kBytes, S(stream)>>>(x, s2, total);
+  } else {
+    k_sum_sq<<<1, 256, 0, S(stream)>>>(x, s2, total);
+  }
   int rc = check_launch("twg_dragan_xhat/sum");
   if (rc) return rc;
   k_dragan_xhat<<<grid_for(total, 4), 256, 0, S(stream)>>>(x, alpha, noise, xhat, s2, N, per_sample);

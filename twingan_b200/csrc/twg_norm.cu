@@ -1,6 +1,7 @@
 // Normaliser (instance / batch / batch-renorm / none) + leaky-ReLU + pixel-norm: statistics, forward apply and both
 // backward passes.  NHWC fp32, vectorised float4 along C; every per-(n, c) sum is added by one block in a fixed order.
 #include "twg_common.cuh"
+#include "twg_stream.cuh"
 
 namespace twg {
 
@@ -11,6 +12,13 @@ namespace twg {
 // Shifted sums: sums[n][c] = {sum (y - p), sum (y - p)^2} with the pivot p = y[first sample of n's pivot group][pixel 0][c].
 // tf.nn.moments is two-pass; a single pass over raw y, y^2 in fp32 cancels catastrophically once |mean| >> std
 // (relative variance error ~ 6e-8 * mean^2 / var).  With a pivot drawn from the data the shifted mean is O(std).
+// one float4 of a pixel into its thread's eight shifted sums
+__device__ __forceinline__ void moments_add(float4 d, const float4& pv, float* acc) {
+  d.x -= pv.x; d.y -= pv.y; d.z -= pv.z; d.w -= pv.w;
+  acc[0] += d.x; acc[1] += d.y; acc[2] += d.z; acc[3] += d.w;
+  acc[4] += d.x * d.x; acc[5] += d.y * d.y; acc[6] += d.z * d.z; acc[7] += d.w * d.w;
+}
+
 template <int V>
 __global__ void __launch_bounds__(256) k_moments_vec(const float* __restrict__ y, float* __restrict__ sums, int HW,
                                                      int C, int G, int pivot_group) {
@@ -37,12 +45,57 @@ __global__ void __launch_bounds__(256) k_moments_vec(const float* __restrict__ y
     for (int u = 0; u < U; ++u) {
       if (pb + u * gpb >= HW) continue;
 #pragma unroll
-      for (int v = 0; v < V; ++v) {
-        float4 d = t[u][v];
-        d.x -= pv[v].x; d.y -= pv[v].y; d.z -= pv[v].z; d.w -= pv[v].w;
-        acc[8 * v + 0] += d.x; acc[8 * v + 1] += d.y; acc[8 * v + 2] += d.z; acc[8 * v + 3] += d.w;
-        acc[8 * v + 4] += d.x * d.x; acc[8 * v + 5] += d.y * d.y; acc[8 * v + 6] += d.z * d.z; acc[8 * v + 7] += d.w * d.w;
-      }
+      for (int v = 0; v < V; ++v) moments_add(t[u][v], pv[v], &acc[8 * v]);
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 8 * V; ++k) {
+    const float s = block_tree_sum(acc[k], G, sm);
+    if (threadIdx.x < G) {
+      int v = k / 8, j = k % 8;
+      int c = (lg + v * 32) * 4 + (j & 3);
+      sums[((int64_t)n * C + c) * 2 + (j >> 2)] = s;
+    }
+  }
+}
+
+// k_moments_vec with the sample arriving through a StreamRing: the same thread adds the same pixels in the same order
+// and the same tree adds the threads, so the sums are the same bits.  A stage is 4 / V pixels per thread.
+constexpr int kMomentsStages = 12;
+template <int V>
+__global__ void __launch_bounds__(256) k_moments_stream(const float* __restrict__ y, float* __restrict__ sums, int HW,
+                                                        int C, int G, int pivot_group) {
+  extern __shared__ __align__(128) unsigned char ring_mem[];
+  __shared__ float sm[256];
+  constexpr int PX = 4 / V;
+  const int n = blockIdx.y, q = C / 4;
+  const int gpb = 256 / G, grp = threadIdx.x / G, lg = threadIdx.x % G;
+  StreamRing<1, kMomentsStages> ring;
+  const void* const arrays[1] = {y + (int64_t)n * HW * C};
+  ring.start(ring_mem, arrays, (int64_t)HW * C * 4);
+  float4 pv[V];
+#pragma unroll
+  for (int v = 0; v < V; ++v) pv[v] = ld4(y, (int64_t)(n / pivot_group * pivot_group) * HW * q + lg + v * 32);
+  float acc[8 * V];
+#pragma unroll
+  for (int i = 0; i < 8 * V; ++i) acc[i] = 0.f;
+  for (int k = 0; k < ring.chunks; ++k) {
+    ring.wait(k);
+    const float4* ys = ring.at(k, 0);
+    float4 t[PX][V];
+#pragma unroll
+    for (int j = 0; j < PX; ++j) {
+      const int slot = j * gpb + grp;                  // pixel of the chunk; a short last chunk re-reads its pixel 0
+      const int sv = k * PX * gpb + slot < HW ? slot : 0;
+#pragma unroll
+      for (int v = 0; v < V; ++v) t[j][v] = ys[sv * q + lg + v * 32];
+    }
+    ring.release(k);
+#pragma unroll
+    for (int j = 0; j < PX; ++j) {
+      if (k * PX * gpb + j * gpb + grp >= HW) continue;
+#pragma unroll
+      for (int v = 0; v < V; ++v) moments_add(t[j][v], pv[v], &acc[8 * v]);
     }
   }
 #pragma unroll
@@ -339,6 +392,71 @@ __global__ void __launch_bounds__(256) k_norm_act_fwd_scalar(const float* __rest
 // ------------------------------------------------------------------------------------------------
 // backward pass 1: gu and per-(n,c) {sum gu, sum gu*yhat}
 // ------------------------------------------------------------------------------------------------
+// a.x b.x + a.y b.y + a.z b.z + a.w b.w with the roundings pinned.  Written as a sum of products, which product stays a
+// multiplication and which are fused into the chain is the compiler's choice, and it chose differently between
+// instantiations and between kernels that inline the same source: these are the two forms its choices came to, spelled
+// out so that every kernel that shares bwd_reduce_pixel computes the same bits.
+__device__ __forceinline__ float dot4_x_first(const float4& a, const float4& b) {
+  return fmaf(a.w, b.w, fmaf(a.z, b.z, fmaf(a.y, b.y, a.x * b.x)));
+}
+__device__ __forceinline__ float dot4_y_first(const float4& a, const float4& b) {
+  return fmaf(a.w, b.w, fmaf(a.z, b.z, fmaf(a.x, b.x, a.y * b.y)));
+}
+
+// One pixel of backward pass 1: g (the gradient w.r.t. the layer output, G lanes x V float4) becomes gu in place; a valid
+// pixel stores it at float4 index `at` (+ 32 v) of gu and adds it into the thread's sums.  All lanes of a warp call this
+// together (the pixel-norm sums shuffle across the G lanes of a pixel).
+template <int V>
+__device__ __forceinline__ void bwd_reduce_pixel(const float4 (&yy)[V], float4 (&g)[V], const float4 (&aa)[V],
+                                                 const float4 (&bb)[V], const float4 (&mm)[V], const float4 (&rr)[V],
+                                                 bool act, bool pix, int G, float invC, bool valid, float* __restrict__ gu,
+                                                 int64_t at, float (&acc)[8 * V]) {
+  float4 uu[V], vv[V];
+  float ss = 0.f;
+#pragma unroll
+  for (int v = 0; v < V; ++v) {
+    uu[v] = make_float4(fmaf(aa[v].x, yy[v].x, bb[v].x), fmaf(aa[v].y, yy[v].y, bb[v].y),
+                        fmaf(aa[v].z, yy[v].z, bb[v].z), fmaf(aa[v].w, yy[v].w, bb[v].w));
+    vv[v] = uu[v];
+    if (act) { vv[v].x = lrelu(uu[v].x); vv[v].y = lrelu(uu[v].y); vv[v].z = lrelu(uu[v].z); vv[v].w = lrelu(uu[v].w); }
+    ss += V == 1 ? dot4_x_first(vv[v], vv[v]) : dot4_y_first(vv[v], vv[v]);
+  }
+  if (pix) {
+    ss = group_sum(ss, G);
+    const float rinv = rsqrtf(ss * invC + kPixEps);
+    float dot = 0.f;
+#pragma unroll
+    for (int v = 0; v < V; ++v) {
+      vv[v].x *= rinv; vv[v].y *= rinv; vv[v].z *= rinv; vv[v].w *= rinv;  // vv = z
+      dot += dot4_y_first(g[v], vv[v]);
+    }
+    dot = group_sum(dot, G) * invC;
+#pragma unroll
+    for (int v = 0; v < V; ++v) {
+      g[v].x = rinv * (g[v].x - vv[v].x * dot); g[v].y = rinv * (g[v].y - vv[v].y * dot);
+      g[v].z = rinv * (g[v].z - vv[v].z * dot); g[v].w = rinv * (g[v].w - vv[v].w * dot);
+    }
+  }
+  if (act) {
+#pragma unroll
+    for (int v = 0; v < V; ++v) {
+      g[v].x *= lrelu_slope(uu[v].x); g[v].y *= lrelu_slope(uu[v].y);
+      g[v].z *= lrelu_slope(uu[v].z); g[v].w *= lrelu_slope(uu[v].w);
+    }
+  }
+  if (valid) {
+#pragma unroll
+    for (int v = 0; v < V; ++v) {
+      st4(gu, at + v * 32, g[v]);
+      acc[8 * v + 0] += g[v].x; acc[8 * v + 1] += g[v].y; acc[8 * v + 2] += g[v].z; acc[8 * v + 3] += g[v].w;
+      acc[8 * v + 4] += g[v].x * (yy[v].x - mm[v].x) * rr[v].x;
+      acc[8 * v + 5] += g[v].y * (yy[v].y - mm[v].y) * rr[v].y;
+      acc[8 * v + 6] += g[v].z * (yy[v].z - mm[v].z) * rr[v].z;
+      acc[8 * v + 7] += g[v].w * (yy[v].w - mm[v].w) * rr[v].w;
+    }
+  }
+}
+
 template <int V>
 __global__ void __launch_bounds__(256) k_norm_act_bwd_reduce_vec(
     const float* __restrict__ y, const float* __restrict__ a, const float* __restrict__ b,
@@ -387,52 +505,92 @@ __global__ void __launch_bounds__(256) k_norm_act_bwd_reduce_vec(
       }
     }
 #pragma unroll
-    for (int u = 0; u < U; ++u) {
-      float4 uu[V], vv[V];
-      float ss = 0.f;
+    for (int u = 0; u < U; ++u)
+      bwd_reduce_pixel<V>(yy[u], g[u], aa, bb, mm, rr, act, pix, G, invC, valid[u], gu, base[u] + lg, acc);
+  }
+#pragma unroll
+  for (int k = 0; k < 8 * V; ++k) {
+    const float s = block_tree_sum(acc[k], G, sm);
+    if (threadIdx.x < G) {
+      int v = k / 8, j = k % 8;
+      int c = (lg + v * 32) * 4 + (j & 3);
+      red[((int64_t)n * C + c) * 2 + (j >> 2)] = s;
+    }
+  }
+}
+
+// k_norm_act_bwd_reduce_vec with the sample's y and gz arriving through a StreamRing (six stages of 16 KB each, 192 KB
+// per block): the same thread takes the same pixels in the same order through bwd_reduce_pixel and the same tree adds the
+// threads, so gu and red are the same bits.  gpool is a quarter of the traffic and its rows are not contiguous with a
+// chunk's, so it stays a direct load, issued one chunk ahead.  gu is stored from registers.
+constexpr int kReduceStages = 6;
+template <int V>
+__global__ void __launch_bounds__(256) k_norm_act_bwd_reduce_stream(
+    const float* __restrict__ y, const float* __restrict__ a, const float* __restrict__ b,
+    const float* __restrict__ mean, const float* __restrict__ rstd, const float* __restrict__ gz,
+    float* __restrict__ gu, float* __restrict__ red, int HW, int C, int G, int flags,
+    const float* __restrict__ gpool, int W) {
+  extern __shared__ __align__(128) unsigned char ring_mem[];
+  __shared__ float sm[256];
+  constexpr int PX = 4 / V;                            // pixels of a stage per thread
+  const int n = blockIdx.y, q = C / 4;
+  const int gpb = 256 / G, grp = threadIdx.x / G, lg = threadIdx.x % G;
+  const bool act = flags & TWG_FLAG_LRELU, pix = flags & TWG_FLAG_PIXNORM;
+  const float invC = 1.f / (float)C;
+  StreamRing<2, kReduceStages> ring;
+  const void* const arrays[2] = {y + (int64_t)n * HW * C, gz ? gz + (int64_t)n * HW * C : nullptr};
+  ring.start(ring_mem, arrays, (int64_t)HW * C * 4);
+  float4 aa[V], bb[V], mm[V], rr[V];
+#pragma unroll
+  for (int v = 0; v < V; ++v) {
+    const int64_t i = (int64_t)n * q + lg + v * 32;
+    aa[v] = ld4(a, i); bb[v] = ld4(b, i); mm[v] = ld4(mean, i); rr[v] = ld4(rstd, i);
+  }
+  float acc[8 * V];
+#pragma unroll
+  for (int i = 0; i < 8 * V; ++i) acc[i] = 0.f;
+  float4 gp[PX][V];                                    // the pooled gradient of the thread's pixels of the next chunk
+  auto load_pool = [&](int k) {
+#pragma unroll
+    for (int j = 0; j < PX; ++j) {
+      const int p = (k * PX + j) * gpb + grp;
+      const int pp = p < HW ? p : 0;
+      const int h = pp / W, w = pp - h * W;
+      const int64_t pq = (((int64_t)n * (HW / W / 2) + (h >> 1)) * (W >> 1) + (w >> 1)) * q;
+#pragma unroll
+      for (int v = 0; v < V; ++v) gp[j][v] = ld4(gpool, pq + lg + v * 32);
+    }
+  };
+  if (gpool) load_pool(0);
+  for (int k = 0; k < ring.chunks; ++k) {
+    ring.wait(k);
+    const float4* ys = ring.at(k, 0);
+    const float4* gs = ring.at(k, 1);
+    float4 yy[PX][V], g[PX][V];
+    bool valid[PX];
+#pragma unroll
+    for (int j = 0; j < PX; ++j) {
+      const int slot = j * gpb + grp;                  // pixel of the chunk; a short last chunk re-reads its pixel 0
+      valid[j] = k * PX * gpb + slot < HW;
+      const int sv = valid[j] ? slot : 0;
 #pragma unroll
       for (int v = 0; v < V; ++v) {
-        uu[v] = make_float4(fmaf(aa[v].x, yy[u][v].x, bb[v].x), fmaf(aa[v].y, yy[u][v].y, bb[v].y),
-                            fmaf(aa[v].z, yy[u][v].z, bb[v].z), fmaf(aa[v].w, yy[u][v].w, bb[v].w));
-        vv[v] = uu[v];
-        if (act) { vv[v].x = lrelu(uu[v].x); vv[v].y = lrelu(uu[v].y); vv[v].z = lrelu(uu[v].z); vv[v].w = lrelu(uu[v].w); }
-        ss += vv[v].x * vv[v].x + vv[v].y * vv[v].y + vv[v].z * vv[v].z + vv[v].w * vv[v].w;
-      }
-      if (pix) {
-        ss = group_sum(ss, G);
-        const float rinv = rsqrtf(ss * invC + kPixEps);
-        float dot = 0.f;
-#pragma unroll
-        for (int v = 0; v < V; ++v) {
-          vv[v].x *= rinv; vv[v].y *= rinv; vv[v].z *= rinv; vv[v].w *= rinv;  // vv = z
-          dot += g[u][v].x * vv[v].x + g[u][v].y * vv[v].y + g[u][v].z * vv[v].z + g[u][v].w * vv[v].w;
+        yy[j][v] = ys[sv * q + lg + v * 32];
+        g[j][v] = gz ? gs[sv * q + lg + v * 32] : make_float4(0, 0, 0, 0);
+        if (gpool) {
+          const float4 t = gp[j][v];
+          g[j][v].x = fmaf(0.25f, t.x, g[j][v].x); g[j][v].y = fmaf(0.25f, t.y, g[j][v].y);
+          g[j][v].z = fmaf(0.25f, t.z, g[j][v].z); g[j][v].w = fmaf(0.25f, t.w, g[j][v].w);
         }
-        dot = group_sum(dot, G) * invC;
-#pragma unroll
-        for (int v = 0; v < V; ++v) {
-          g[u][v].x = rinv * (g[u][v].x - vv[v].x * dot); g[u][v].y = rinv * (g[u][v].y - vv[v].y * dot);
-          g[u][v].z = rinv * (g[u][v].z - vv[v].z * dot); g[u][v].w = rinv * (g[u][v].w - vv[v].w * dot);
-        }
-      }
-      if (act) {
-#pragma unroll
-        for (int v = 0; v < V; ++v) {
-          g[u][v].x *= lrelu_slope(uu[v].x); g[u][v].y *= lrelu_slope(uu[v].y);
-          g[u][v].z *= lrelu_slope(uu[v].z); g[u][v].w *= lrelu_slope(uu[v].w);
-        }
-      }
-      if (valid[u]) {
-#pragma unroll
-        for (int v = 0; v < V; ++v) {
-          st4(gu, base[u] + lg + v * 32, g[u][v]);
-          acc[8 * v + 0] += g[u][v].x; acc[8 * v + 1] += g[u][v].y; acc[8 * v + 2] += g[u][v].z; acc[8 * v + 3] += g[u][v].w;
-          acc[8 * v + 4] += g[u][v].x * (yy[u][v].x - mm[v].x) * rr[v].x;
-          acc[8 * v + 5] += g[u][v].y * (yy[u][v].y - mm[v].y) * rr[v].y;
-          acc[8 * v + 6] += g[u][v].z * (yy[u][v].z - mm[v].z) * rr[v].z;
-          acc[8 * v + 7] += g[u][v].w * (yy[u][v].w - mm[v].w) * rr[v].w;
-        }
+        if (!valid[j]) g[j][v] = make_float4(0, 0, 0, 0);
       }
     }
+    ring.release(k);
+    if (gpool && k + 1 < ring.chunks) load_pool(k + 1);
+#pragma unroll
+    for (int j = 0; j < PX; ++j)
+      bwd_reduce_pixel<V>(yy[j], g[j], aa, bb, mm, rr, act, pix, G, invC, valid[j], gu,
+                          ((int64_t)n * HW + (k * PX + j) * gpb + grp) * q + lg, acc);
   }
 #pragma unroll
   for (int k = 0; k < 8 * V; ++k) {
@@ -597,6 +755,31 @@ __global__ void __launch_bounds__(256) k_norm_act_bwd_apply(const float* __restr
 
 using namespace twg;
 
+// the streamed kernels: one block per sample, as in the kernels they stand in for
+template <int V>
+static int launch_moments_stream(const float* y, float* sums, int N, int HW, int C, int G, int pivot_group, cudaStream_t st) {
+  constexpr int kBytes = StreamRing<1, kMomentsStages>::kBytes;
+  static std::once_flag once;
+  static cudaError_t attr_err = cudaSuccess;
+  if (allow_ring(k_moments_stream<V>, kBytes, once, attr_err) != cudaSuccess)
+    return fail(TWG_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(attr_err));
+  k_moments_stream<V><<<dim3(1, N), 256, kBytes, st>>>(y, sums, HW, C, G, pivot_group);
+  return 0;
+}
+
+template <int V>
+static int launch_bwd_reduce_stream(const float* y, const float* a, const float* b, const float* mean, const float* rstd,
+                                    const float* gz, float* gu, float* red, int N, int HW, int C, int G, int flags,
+                                    const float* gpool, int W, cudaStream_t st) {
+  constexpr int kBytes = StreamRing<2, kReduceStages>::kBytes;
+  static std::once_flag once;
+  static cudaError_t attr_err = cudaSuccess;
+  if (allow_ring(k_norm_act_bwd_reduce_stream<V>, kBytes, once, attr_err) != cudaSuccess)
+    return fail(TWG_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(attr_err));
+  k_norm_act_bwd_reduce_stream<V><<<dim3(1, N), 256, kBytes, st>>>(y, a, b, mean, rstd, gz, gu, red, HW, C, G, flags, gpool, W);
+  return 0;
+}
+
 extern "C" {
 
 int twg_moments(const float* y, float* sums, int N, int HW, int C, int pivot_group, twg_stream_t stream) {
@@ -604,7 +787,12 @@ int twg_moments(const float* y, float* sums, int N, int HW, int C, int pivot_gro
     return fail(TWG_ERR_INVALID, "twg_moments: bad args");
   const dim3 grid(1, N);                    // one block per sample writes all of its sums
   VecGeom g = vec_geom(C);
-  if (g.ok) {
+  if (g.ok && stream_fills((int64_t)HW * C * 4)) {
+    int rc = g.V == 1 ? launch_moments_stream<1>(y, sums, N, HW, C, g.G, pivot_group, S(stream))
+             : g.V == 2 ? launch_moments_stream<2>(y, sums, N, HW, C, g.G, pivot_group, S(stream))
+                        : launch_moments_stream<4>(y, sums, N, HW, C, g.G, pivot_group, S(stream));
+    if (rc) return rc;
+  } else if (g.ok) {
     if (g.V == 1) k_moments_vec<1><<<grid, 256, 0, S(stream)>>>(y, sums, HW, C, g.G, pivot_group);
     else if (g.V == 2) k_moments_vec<2><<<grid, 256, 0, S(stream)>>>(y, sums, HW, C, g.G, pivot_group);
     else k_moments_vec<4><<<grid, 256, 0, S(stream)>>>(y, sums, HW, C, g.G, pivot_group);
@@ -689,7 +877,12 @@ int twg_norm_act_bwd_reduce(const float* y, const float* a, const float* b, cons
     return fail(TWG_ERR_UNSUPPORTED, "twg_norm_act_bwd_reduce: the pool gradient needs even H, W and a vectorisable C");
   const dim3 grid(1, N);                    // one block per sample writes all of its sums
   VecGeom g = vec_geom(C);
-  if (g.ok) {
+  if (g.ok && stream_fills((int64_t)HW * C * 4)) {
+    int rc = g.V == 1 ? launch_bwd_reduce_stream<1>(y, a, b, mean, rstd, gz, gu, red, N, HW, C, g.G, flags, gpool, W, S(stream))
+             : g.V == 2 ? launch_bwd_reduce_stream<2>(y, a, b, mean, rstd, gz, gu, red, N, HW, C, g.G, flags, gpool, W, S(stream))
+                        : launch_bwd_reduce_stream<4>(y, a, b, mean, rstd, gz, gu, red, N, HW, C, g.G, flags, gpool, W, S(stream));
+    if (rc) return rc;
+  } else if (g.ok) {
     if (g.V == 1) k_norm_act_bwd_reduce_vec<1><<<grid, 256, 0, S(stream)>>>(y, a, b, mean, rstd, gz, gu, red, HW, C, g.G, flags, gpool, W);
     else if (g.V == 2) k_norm_act_bwd_reduce_vec<2><<<grid, 256, 0, S(stream)>>>(y, a, b, mean, rstd, gz, gu, red, HW, C, g.G, flags, gpool, W);
     else k_norm_act_bwd_reduce_vec<4><<<grid, 256, 0, S(stream)>>>(y, a, b, mean, rstd, gz, gu, red, HW, C, g.G, flags, gpool, W);
