@@ -1,7 +1,11 @@
 // Normaliser (instance / batch / batch-renorm / none) + leaky-ReLU + pixel-norm: statistics, forward apply and both
 // backward passes.  NHWC fp32, vectorised float4 along C; every per-(n, c) sum is added by one block in a fixed order.
+#include <cooperative_groups.h>
+
 #include "twg_common.cuh"
 #include "twg_stream.cuh"
+
+namespace cg = cooperative_groups;
 
 namespace twg {
 
@@ -403,14 +407,24 @@ __device__ __forceinline__ float dot4_y_first(const float4& a, const float4& b) 
   return fmaf(a.w, b.w, fmaf(a.z, b.z, fmaf(a.x, b.x, a.y * b.y)));
 }
 
-// One pixel of backward pass 1: g (the gradient w.r.t. the layer output, G lanes x V float4) becomes gu in place; a valid
-// pixel stores it at float4 index `at` (+ 32 v) of gu and adds it into the thread's sums.  All lanes of a warp call this
-// together (the pixel-norm sums shuffle across the G lanes of a pixel).
+// g - z dot, then * rinv: the pixel-norm step of the gradient, with the contraction nvcc chose in every kernel written out
+__device__ __forceinline__ float pixnorm_grad(float g, float z, float dot, float rinv) {
+  return __fmul_rn(rinv, __fmaf_rn(z, -dot, g));
+}
+// g (y - m) without r: the product sums add it as fma(g (y - m), r, acc), the form nvcc contracted
+// `acc += g * (y - m) * r` to in every kernel, spelled out so that a kernel whose adds happen elsewhere keeps the bits
+__device__ __forceinline__ float4 yhat_num4(const float4& g, const float4& y, const float4& m) {
+  return make_float4(__fmul_rn(g.x, __fsub_rn(y.x, m.x)), __fmul_rn(g.y, __fsub_rn(y.y, m.y)),
+                     __fmul_rn(g.z, __fsub_rn(y.z, m.z)), __fmul_rn(g.w, __fsub_rn(y.w, m.w)));
+}
+
+// One pixel of backward pass 1, up to its sums: g (the gradient w.r.t. the layer output, G lanes x V float4) becomes gu in
+// place, and a valid pixel stores it at float4 index `at` (+ 32 v) of gu.  All lanes of a warp call this together (the
+// pixel-norm sums shuffle across the G lanes of a pixel).
 template <int V>
-__device__ __forceinline__ void bwd_reduce_pixel(const float4 (&yy)[V], float4 (&g)[V], const float4 (&aa)[V],
-                                                 const float4 (&bb)[V], const float4 (&mm)[V], const float4 (&rr)[V],
-                                                 bool act, bool pix, int G, float invC, bool valid, float* __restrict__ gu,
-                                                 int64_t at, float (&acc)[8 * V]) {
+__device__ __forceinline__ void bwd_gu_pixel(const float4 (&yy)[V], float4 (&g)[V], const float4 (&aa)[V],
+                                             const float4 (&bb)[V], bool act, bool pix, int G, float invC, bool valid,
+                                             float* __restrict__ gu, int64_t at) {
   float4 uu[V], vv[V];
   float ss = 0.f;
 #pragma unroll
@@ -423,18 +437,18 @@ __device__ __forceinline__ void bwd_reduce_pixel(const float4 (&yy)[V], float4 (
   }
   if (pix) {
     ss = group_sum(ss, G);
-    const float rinv = rsqrtf(ss * invC + kPixEps);
+    const float rinv = rsqrtf(__fmaf_rn(ss, invC, kPixEps));
     float dot = 0.f;
 #pragma unroll
     for (int v = 0; v < V; ++v) {
       vv[v].x *= rinv; vv[v].y *= rinv; vv[v].z *= rinv; vv[v].w *= rinv;  // vv = z
       dot += dot4_y_first(g[v], vv[v]);
     }
-    dot = group_sum(dot, G) * invC;
+    dot = __fmul_rn(group_sum(dot, G), invC);
 #pragma unroll
     for (int v = 0; v < V; ++v) {
-      g[v].x = rinv * (g[v].x - vv[v].x * dot); g[v].y = rinv * (g[v].y - vv[v].y * dot);
-      g[v].z = rinv * (g[v].z - vv[v].z * dot); g[v].w = rinv * (g[v].w - vv[v].w * dot);
+      g[v].x = pixnorm_grad(g[v].x, vv[v].x, dot, rinv); g[v].y = pixnorm_grad(g[v].y, vv[v].y, dot, rinv);
+      g[v].z = pixnorm_grad(g[v].z, vv[v].z, dot, rinv); g[v].w = pixnorm_grad(g[v].w, vv[v].w, dot, rinv);
     }
   }
   if (act) {
@@ -446,13 +460,25 @@ __device__ __forceinline__ void bwd_reduce_pixel(const float4 (&yy)[V], float4 (
   }
   if (valid) {
 #pragma unroll
+    for (int v = 0; v < V; ++v) st4(gu, at + v * 32, g[v]);
+  }
+}
+
+// One pixel of backward pass 1: bwd_gu_pixel, then a valid pixel adds gu into the thread's sums.
+template <int V>
+__device__ __forceinline__ void bwd_reduce_pixel(const float4 (&yy)[V], float4 (&g)[V], const float4 (&aa)[V],
+                                                 const float4 (&bb)[V], const float4 (&mm)[V], const float4 (&rr)[V],
+                                                 bool act, bool pix, int G, float invC, bool valid, float* __restrict__ gu,
+                                                 int64_t at, float (&acc)[8 * V]) {
+  bwd_gu_pixel<V>(yy, g, aa, bb, act, pix, G, invC, valid, gu, at);
+  if (valid) {
+#pragma unroll
     for (int v = 0; v < V; ++v) {
-      st4(gu, at + v * 32, g[v]);
-      acc[8 * v + 0] += g[v].x; acc[8 * v + 1] += g[v].y; acc[8 * v + 2] += g[v].z; acc[8 * v + 3] += g[v].w;
-      acc[8 * v + 4] += g[v].x * (yy[v].x - mm[v].x) * rr[v].x;
-      acc[8 * v + 5] += g[v].y * (yy[v].y - mm[v].y) * rr[v].y;
-      acc[8 * v + 6] += g[v].z * (yy[v].z - mm[v].z) * rr[v].z;
-      acc[8 * v + 7] += g[v].w * (yy[v].w - mm[v].w) * rr[v].w;
+      const float4 t = yhat_num4(g[v], yy[v], mm[v]);
+      acc[8 * v + 0] = __fadd_rn(acc[8 * v + 0], g[v].x); acc[8 * v + 1] = __fadd_rn(acc[8 * v + 1], g[v].y);
+      acc[8 * v + 2] = __fadd_rn(acc[8 * v + 2], g[v].z); acc[8 * v + 3] = __fadd_rn(acc[8 * v + 3], g[v].w);
+      acc[8 * v + 4] = __fmaf_rn(t.x, rr[v].x, acc[8 * v + 4]); acc[8 * v + 5] = __fmaf_rn(t.y, rr[v].y, acc[8 * v + 5]);
+      acc[8 * v + 6] = __fmaf_rn(t.z, rr[v].z, acc[8 * v + 6]); acc[8 * v + 7] = __fmaf_rn(t.w, rr[v].w, acc[8 * v + 7]);
     }
   }
 }
@@ -598,6 +624,130 @@ __global__ void __launch_bounds__(256) k_norm_act_bwd_reduce_stream(
     if (threadIdx.x < G) {
       int v = k / 8, j = k % 8;
       int c = (lg + v * 32) * 4 + (j & 3);
+      red[((int64_t)n * C + c) * 2 + (j >> 2)] = s;
+    }
+  }
+}
+
+// k_norm_act_bwd_reduce_vec spread over a cluster of K CTAs per sample (gridDim = (K, N)), every sum added in the order
+// of the one-block kernels.  There, thread t = grp G + lg is a chain: it adds pixels grp, grp + gpb, grp + 2 gpb, ... into
+// 8 V sums, and block_tree_sum then adds the 256 chains.  Here CTA r owns the chains of groups [r gpb / K, (r + 1) gpb / K)
+// and gives each of them K threads, which take turns along the chain's pixels: in a batch of U K chain pixels, thread
+// k = threadIdx.x / (256 / K) computes pixels u K + k (u < U) through bwd_gu_pixel, stores gu and stages what each pixel
+// adds to the sums in shared memory.  One thread per (chain, sum) then adds the batch's pixels in chain order, while the
+// next batch's loads are in flight (two stage buffers, one barrier per batch).  At the end every CTA writes its chains'
+// sums into rank 0's shared memory at index t, and rank 0 runs the unchanged block_tree_sum.
+constexpr int kSplitWords = 8192;                      // staged floats per batch: U K pixels x 8 V sums x 256 / K chains
+constexpr int kSplitBytes = 2 * kSplitWords * 4;
+template <int V>
+__global__ void __launch_bounds__(256) k_norm_act_bwd_reduce_split(
+    const float* __restrict__ y, const float* __restrict__ a, const float* __restrict__ b,
+    const float* __restrict__ mean, const float* __restrict__ rstd, const float* __restrict__ gz,
+    float* __restrict__ gu, float* __restrict__ red, int HW, int C, int G, int flags,
+    const float* __restrict__ gpool, int W) {
+  extern __shared__ __align__(16) float stage[];       // [2][U K][8 V / 4][256 / K][4]
+  __shared__ float sm[256];
+  constexpr int U = 4 / V;                             // pixels of a batch per thread
+  cg::cluster_group cl = cg::this_cluster();
+  const int K = (int)cl.num_blocks(), rank = (int)cl.block_rank();
+  const int n = blockIdx.y, q = C / 4;
+  const int gpb = 256 / G, cpk = 256 / K;              // cpk: chains of this CTA
+  const int k = threadIdx.x / cpk, ch = threadIdx.x % cpk;
+  const int grp = rank * (gpb / K) + ch / G, lg = ch % G;
+  const bool act = flags & TWG_FLAG_LRELU, pix = flags & TWG_FLAG_PIXNORM;
+  const float invC = 1.f / (float)C;
+  const int per = U * K, A = 8 * V * cpk;              // chain pixels of a batch; staged floats per chain pixel
+  const int batches = ((HW + gpb - 1) / gpb + per - 1) / per;   // chain 0 is the longest
+  float4 aa[V], bb[V], mm[V];
+#pragma unroll
+  for (int v = 0; v < V; ++v) {
+    const int64_t i = (int64_t)n * q + lg + v * 32;
+    aa[v] = ld4(a, i); bb[v] = ld4(b, i); mm[v] = ld4(mean, i);
+  }
+  // the adding side: tasks t = threadIdx.x + 256 i, i < 8 V / K, each one sum of one chain, multiplied in by w (1 for the
+  // sums of gu, r for the sums of gu yhat: fma(x, 1, acc) is acc + x)
+  float acc[4 * V], w[4 * V];
+  int len[4 * V];
+  const int tasks = 8 * V / K;
+#pragma unroll
+  for (int i = 0; i < 4 * V; ++i) {
+    acc[i] = 0.f; w[i] = 1.f; len[i] = 0;
+    if (i < tasks) {
+      const int t = threadIdx.x + 256 * i, q4 = t / (4 * cpk), tch = (t / 4) % cpk;
+      const int tgrp = rank * (gpb / K) + tch / G;
+      len[i] = tgrp < HW ? (HW - tgrp + gpb - 1) / gpb : 0;
+      if (q4 & 1) w[i] = rstd[(int64_t)n * C + (tch % G + q4 / 2 * 32) * 4 + t % 4];
+    }
+  }
+  float4 yy[U][V], gzv[U][V], gpv[U][V];
+  auto load = [&](int bt) {
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int p = grp + (bt * per + u * K + k) * gpb;
+      const int pp = p < HW ? p : 0;
+      const int64_t base = ((int64_t)n * HW + pp) * q + lg;
+      const int h = gpool ? pp / W : 0, ww = gpool ? pp - h * W : 0;
+      const int64_t pq = (((int64_t)n * (HW / max(W, 1) / 2) + (h >> 1)) * (W >> 1) + (ww >> 1)) * q + lg;
+#pragma unroll
+      for (int v = 0; v < V; ++v) {
+        yy[u][v] = ld4(y, base + v * 32);
+        if (gz) gzv[u][v] = ld4(gz, base + v * 32);
+        if (gpool) gpv[u][v] = ld4(gpool, pq + v * 32);
+      }
+    }
+  };
+  load(0);
+  for (int bt = 0; bt < batches; ++bt) {
+    float* buf = stage + (bt & 1) * kSplitWords;
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int p = grp + (bt * per + u * K + k) * gpb;
+      const bool valid = p < HW;
+      float4 g[V];
+#pragma unroll
+      for (int v = 0; v < V; ++v) {
+        g[v] = gz ? gzv[u][v] : make_float4(0, 0, 0, 0);
+        if (gpool) {
+          const float4 t = gpv[u][v];
+          g[v].x = fmaf(0.25f, t.x, g[v].x); g[v].y = fmaf(0.25f, t.y, g[v].y);
+          g[v].z = fmaf(0.25f, t.z, g[v].z); g[v].w = fmaf(0.25f, t.w, g[v].w);
+        }
+        if (!valid) g[v] = make_float4(0, 0, 0, 0);
+      }
+      bwd_gu_pixel<V>(yy[u], g, aa, bb, act, pix, G, invC, valid, gu, ((int64_t)n * HW + (valid ? p : 0)) * q + lg);
+      float* s = buf + (u * K + k) * A + ch * 4;
+#pragma unroll
+      for (int v = 0; v < V; ++v) {
+        *reinterpret_cast<float4*>(s + (2 * v) * 4 * cpk) = g[v];
+        *reinterpret_cast<float4*>(s + (2 * v + 1) * 4 * cpk) = yhat_num4(g[v], yy[u][v], mm[v]);
+      }
+    }
+    if (bt + 1 < batches) load(bt + 1);
+    __syncthreads();                                   // the batch is staged; the buffer written next was read before
+#pragma unroll
+    for (int i = 0; i < 4 * V; ++i) {
+      if (i >= tasks) break;
+      const float* s = buf + threadIdx.x + 256 * i;
+      const int cnt = min(per, len[i] - bt * per);
+      for (int j = 0; j < cnt; ++j) acc[i] = __fmaf_rn(s[j * A], w[i], acc[i]);
+    }
+  }
+  cl.sync();                                           // every CTA is done with its stage, rank 0's included
+  float* gather = cl.map_shared_rank(stage, 0);        // [8 V][256]: sum a of chain t at a * 256 + t
+#pragma unroll
+  for (int i = 0; i < 4 * V; ++i) {
+    if (i >= tasks) break;
+    const int t = threadIdx.x + 256 * i, q4 = t / (4 * cpk), tch = (t / 4) % cpk;
+    gather[(q4 * 4 + t % 4) * 256 + rank * cpk + tch] = acc[i];
+  }
+  cl.sync();
+  if (rank != 0) return;
+#pragma unroll
+  for (int kk = 0; kk < 8 * V; ++kk) {
+    const float s = block_tree_sum(stage[kk * 256 + threadIdx.x], G, sm);
+    if (threadIdx.x < G) {
+      int v = kk / 8, j = kk % 8;
+      int c = (threadIdx.x + v * 32) * 4 + (j & 3);
       red[((int64_t)n * C + c) * 2 + (j >> 2)] = s;
     }
   }
@@ -780,6 +930,72 @@ static int launch_bwd_reduce_stream(const float* y, const float* a, const float*
   return 0;
 }
 
+// The split reduce: clusters of K CTAs, one per sample.  split_clusters<V>()[i] is how many clusters of 2 << i CTAs
+// (K = 2, 4, 8) the device runs at once, queried once per instantiation; 0 if the query failed.
+template <int V>
+static cudaLaunchConfig_t split_config(int K, int N, cudaLaunchAttribute* attr, cudaStream_t st) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)K, (unsigned)N);
+  cfg.blockDim = dim3(256);
+  cfg.dynamicSmemBytes = kSplitBytes;
+  cfg.stream = st;
+  attr->id = cudaLaunchAttributeClusterDimension;
+  attr->val.clusterDim.x = (unsigned)K;
+  attr->val.clusterDim.y = 1;
+  attr->val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  return cfg;
+}
+
+template <int V>
+static const int* split_clusters() {
+  static std::once_flag once;
+  static int clusters[3] = {0, 0, 0};
+  std::call_once(once, [] {
+    if (cudaFuncSetAttribute(k_norm_act_bwd_reduce_split<V>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSplitBytes) !=
+        cudaSuccess) {
+      cudaGetLastError();
+      return;
+    }
+    for (int i = 0; i < 3; ++i) {
+      cudaLaunchAttribute attr;
+      const cudaLaunchConfig_t cfg = split_config<V>(2 << i, 1, &attr, nullptr);
+      if (cudaOccupancyMaxActiveClusters(&clusters[i], k_norm_act_bwd_reduce_split<V>, &cfg) != cudaSuccess) {
+        cudaGetLastError();
+        clusters[i] = 0;
+      }
+    }
+  });
+  return clusters;
+}
+
+// K for N samples of gpb pixel groups: the largest of 8, 4, 2 that divides gpb and for which the N clusters run in one
+// wave; 1 (the one-block kernels) when none does, or when a sample is under kSplitMinBytes: there the cluster launch and
+// barriers cost more than the wider grid saves (on an H100, samples of 256 KB were up to 3 % faster at N = 32 and 12 %
+// slower at N = 64; of 64 KB, 25-30 % slower)
+constexpr int64_t kSplitMinBytes = 512 << 10;
+template <int V>
+static int split_k(int N, int gpb, int64_t sample_bytes) {
+  if (sample_bytes < kSplitMinBytes) return 1;
+  const int* clusters = split_clusters<V>();
+  for (int i = 2; i >= 0; --i)
+    if (gpb % (2 << i) == 0 && N <= clusters[i]) return 2 << i;
+  return 1;
+}
+
+template <int V>
+static int launch_bwd_reduce_split(const float* y, const float* a, const float* b, const float* mean, const float* rstd,
+                                   const float* gz, float* gu, float* red, int N, int HW, int C, int G, int flags,
+                                   const float* gpool, int W, int K, cudaStream_t st) {
+  cudaLaunchAttribute attr;
+  const cudaLaunchConfig_t cfg = split_config<V>(K, N, &attr, st);
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, k_norm_act_bwd_reduce_split<V>, y, a, b, mean, rstd, gz, gu, red, HW, C, G,
+                                           flags, gpool, W);
+  if (e != cudaSuccess) return fail(TWG_ERR_CUDA, "twg_norm_act_bwd_reduce: cluster launch: %s", cudaGetErrorString(e));
+  return 0;
+}
+
 extern "C" {
 
 int twg_moments(const float* y, float* sums, int N, int HW, int C, int pivot_group, twg_stream_t stream) {
@@ -875,9 +1091,19 @@ int twg_norm_act_bwd_reduce(const float* y, const float* a, const float* b, cons
   if (!y || !a || !b || !mean || !rstd || (!gz && !gpool) || !gu || !red) return fail(TWG_ERR_INVALID, "twg_norm_act_bwd_reduce: null");
   if (gpool && (W <= 0 || W % 2 || HW % W || (HW / W) % 2 || !vec_geom(C).ok))
     return fail(TWG_ERR_UNSUPPORTED, "twg_norm_act_bwd_reduce: the pool gradient needs even H, W and a vectorisable C");
-  const dim3 grid(1, N);                    // one block per sample writes all of its sums
+  const dim3 grid(1, N);                    // one block (or one cluster) per sample writes all of its sums
   VecGeom g = vec_geom(C);
-  if (g.ok && stream_fills((int64_t)HW * C * 4)) {
+  const bool streamed = g.ok && stream_fills((int64_t)HW * C * 4);
+  const int64_t bytes = (int64_t)HW * C * 4;
+  const int K = !streamed ? 1
+                : g.V == 1 ? split_k<1>(N, 256 / g.G, bytes)
+                : g.V == 2 ? split_k<2>(N, 256 / g.G, bytes) : split_k<4>(N, 256 / g.G, bytes);
+  if (K > 1) {
+    int rc = g.V == 1 ? launch_bwd_reduce_split<1>(y, a, b, mean, rstd, gz, gu, red, N, HW, C, g.G, flags, gpool, W, K, S(stream))
+             : g.V == 2 ? launch_bwd_reduce_split<2>(y, a, b, mean, rstd, gz, gu, red, N, HW, C, g.G, flags, gpool, W, K, S(stream))
+                        : launch_bwd_reduce_split<4>(y, a, b, mean, rstd, gz, gu, red, N, HW, C, g.G, flags, gpool, W, K, S(stream));
+    if (rc) return rc;
+  } else if (streamed) {
     int rc = g.V == 1 ? launch_bwd_reduce_stream<1>(y, a, b, mean, rstd, gz, gu, red, N, HW, C, g.G, flags, gpool, W, S(stream))
              : g.V == 2 ? launch_bwd_reduce_stream<2>(y, a, b, mean, rstd, gz, gu, red, N, HW, C, g.G, flags, gpool, W, S(stream))
                         : launch_bwd_reduce_stream<4>(y, a, b, mean, rstd, gz, gu, red, N, HW, C, g.G, flags, gpool, W, S(stream));
@@ -891,6 +1117,16 @@ int twg_norm_act_bwd_reduce(const float* y, const float* a, const float* b, cons
     k_norm_act_bwd_reduce_scalar<<<grid, 256, 0, S(stream)>>>(y, a, b, mean, rstd, gz, gu, red, HW, C, flags);
   }
   return check_launch("twg_norm_act_bwd_reduce");
+}
+
+// Outside include/twg.h, launches nothing: how many clusters of K CTAs (2, 4 or 8) of twg_norm_act_bwd_reduce's split
+// kernel for channel count C the device runs at once (0 when C has no channel-vector layout), so that tests can restate
+// the route's choice of K.
+int twg_norm_bwd_reduce_split_clusters(int C, int K) {
+  const VecGeom g = vec_geom(C);
+  const int i = K == 2 ? 0 : K == 4 ? 1 : K == 8 ? 2 : -1;
+  if (!g.ok || i < 0) return 0;
+  return (g.V == 1 ? split_clusters<1>() : g.V == 2 ? split_clusters<2>() : split_clusters<4>())[i];
 }
 
 int twg_norm_act_bwd_apply(const float* y, const float* a, const float* mean, const float* rstd, const float* gu,
