@@ -24,15 +24,21 @@ def shard_batch(global_batch: int, rank: int, world: int):
   return rank * per, (rank + 1) * per
 
 
-def selfcheck(device, group=None, hw: int = 16, batch: int = 2, max_channels: int = 32, norm: str = 'instance_norm'):
+def selfcheck(device, group=None, hw: int = 16, batch: int = 2, max_channels: int = 32, norm: str = 'instance_norm',
+              extra_flags=None, graphed: bool = False):
   """Data-parallel correctness of the PRODUCT on real ranks (deployment/model_deploy.py:265-267, 473-503): with
   num_clones = world, (1) the all-reduced flat gradient of the ranks' micro-batches equals the sum over the same
   micro-batches run one after the other on one GPU, (2) after a whole train_step (overlapped all-reduces + both Adam
-  applies) every rank holds bit-identical parameters.  Returns a dict of measured errors; raises on failure."""
+  applies) every rank holds bit-identical parameters, (3) with two ranks, whose sum g0 + g1 does not depend on the order
+  of the reduction, that step leaves parameters, Adam slots and normaliser state bit-identical to a model without a
+  process group that sums the two micro-batches' gradients itself.  `extra_flags`: further twingan.Flags fields;
+  `graphed`: the step is captured and replayed (train_step_graphed) instead of launched eagerly.  Returns a dict of
+  measured errors; raises on failure."""
   from . import twingan
   world = dist.get_world_size(group)
   rank = dist.get_rank(group)
-  flags = twingan.Flags(train_image_size=hw, pggan_max_num_channels=max_channels, generator_norm_type=norm, num_clones=world)
+  flags = twingan.Flags(train_image_size=hw, pggan_max_num_channels=max_channels, generator_norm_type=norm, num_clones=world,
+                        **(extra_flags or {}))
   model = twingan.GanModel(flags, device=device, seed=7, process_group=group if group is not None else dist.group.WORLD)
   micro = []
   for r in range(world):
@@ -54,7 +60,11 @@ def selfcheck(device, group=None, hw: int = 16, batch: int = 2, max_channels: in
   # a whole step through the public entry point, then compare parameters across ranks bit for bit
   step_model = twingan.GanModel(twingan.Flags(**{**flags.__dict__}), device=device, seed=7,
                                 process_group=group if group is not None else dist.group.WORLD)
-  step_model.train_step(*micro[rank])
+  if graphed:
+    step_model.capture(*micro[rank])
+    step_model.train_step_graphed(*micro[rank])
+  else:
+    step_model.train_step(*micro[rank])
   torch.cuda.synchronize(device)
   mine = step_model.variables.flat
   gathered = [torch.empty_like(mine) for _ in range(world)]
@@ -65,8 +75,25 @@ def selfcheck(device, group=None, hw: int = 16, batch: int = 2, max_channels: in
   moved = float((mine - ref.variables.flat).abs().max())
   if not moved > 0:
     raise AssertionError('parameters did not move')
-  return {'world': world, 'grad_rel_err_vs_sequential_sum': grad_err, 'params_identical_across_ranks': identical,
-          'max_param_update': moved}
+  out = {'world': world, 'grad_rel_err_vs_sequential_sum': grad_err, 'params_identical_across_ranks': identical,
+         'max_param_update': moved}
+  if world == 2:
+    twin = twingan.GanModel(twingan.Flags(**{**flags.__dict__}), device=device, seed=7, process_group=None)
+    twin.compute_gradients(*micro[1 - rank])
+    other = twin.flat_grad.clone()
+    _, _, _, stats = twin.compute_gradients(*micro[rank])     # this rank's batch statistics feed its EMA pushes
+    twin.flat_grad.add_(other)
+    twin.apply_gradients()
+    twin.apply_stat_updates(stats)
+    torch.cuda.synchronize(device)
+    sv, tv = step_model.variables, twin.variables
+    for name, a, b in (('parameters', sv.flat, tv.flat), ('adam_m', sv.adam_m, tv.adam_m), ('adam_v', sv.adam_v, tv.adam_v),
+                       ('normaliser state', sv.state, tv.state)):
+      if not torch.equal(a, b):
+        raise AssertionError('rank %d: %s after the overlapped step differ from the sequential-sum step (max |diff| %g)'
+                             % (rank, name, float((a - b).abs().max())))
+    out['equal_to_sequential_sum_step'] = True
+  return out
 
 
 def _main():
@@ -82,6 +109,9 @@ def _main():
     out = selfcheck(dev)
     for norm in ('batch_renorm',):
       out[norm] = selfcheck(dev, norm=norm)
+    for graphed in (False, True):
+      out['equalized_learning_rate' + (' graphed' if graphed else '')] = selfcheck(
+          dev, extra_flags={'equalized_learning_rate': True}, graphed=graphed)
     if dist.get_rank() == 0:
       print('ddp selfcheck ok', out, flush=True)
   finally:

@@ -379,14 +379,58 @@ def register_grad_sinks(mapping) -> None:
   _GRAD_SINKS.update({int(k): v for k, v in mapping.items()})
 
 
+# Autograd runs the ready nodes of a backward in an order it takes from per-thread node sequence numbers.  The nodes of a
+# double backward (the DRAGAN / WGAN-GP input gradient, built with create_graph=True) are created on autograd's CUDA
+# worker thread, the forward's on the main thread, and the two counters advance independently, so where both reach the
+# same weight -- a residual block's diamond under --use_res_block -- the order in which their weight gradients are added
+# into the sink depends on how many nodes the process created before.  Inside fixed_order_weight_grads(group) the conv
+# weight gradients of `group` are recorded instead, and flush_weight_grads() adds them into their sinks in the order
+# their conv nodes were created, which is the program's order and does not depend on that history.
+_CONV_SERIAL = [0]          # creation counter of the conv nodes (forward order; the first-order backward's are in order)
+_DEFER_GROUPS = set()
+_DEFERRED = []              # (serial, operands of _conv_wgrad, sink)
+
+
+def _next_serial() -> int:
+  _CONV_SERIAL[0] += 1
+  return _CONV_SERIAL[0]
+
+
+@contextlib.contextmanager
+def fixed_order_weight_grads(group: Optional[str]):
+  """Record the conv weight gradients of `group` (None: none) in the running backward for flush_weight_grads()."""
+  added = group is not None and group not in _DEFER_GROUPS
+  if added:
+    _DEFER_GROUPS.add(group)
+  try:
+    yield
+  finally:
+    if added:
+      _DEFER_GROUPS.discard(group)
+
+
+def flush_weight_grads() -> None:
+  """Add the recorded weight gradients into their sinks, in the creation order of their conv nodes."""
+  for _, (x, gy, k, pad, xp, gp), sink in sorted(_DEFERRED, key=lambda e: e[0]):
+    _conv_wgrad(x, gy, k, pad, xp, gp, out=sink)
+  _DEFERRED.clear()
+
+
+def drop_weight_grads() -> None:
+  _DEFERRED.clear()
+
+
 def _weight_grad(ctx, w, x, gy, xp=None, gp=None):
   """The weight gradient of the conv node `ctx` (inputs [x-like, w, ...]) from its operands: added into w's gradient sink
-  when one is registered, else returned for autograd; None when not wanted or sunk."""
+  when one is registered (or recorded for flush_weight_grads), else returned for autograd; None when not wanted or sunk."""
   if not (ctx.needs_input_grad[1] and ctx.group not in _SKIP_PARAM_GRADS):
     return None
   sink = _sink(w)
   if sink is not None:
-    _conv_wgrad(x, gy, ctx.k, ctx.pad, xp, gp, out=sink)
+    if ctx.group in _DEFER_GROUPS:
+      _DEFERRED.append((ctx.serial, (x, gy, ctx.k, ctx.pad, xp, gp), sink))
+    else:
+      _conv_wgrad(x, gy, ctx.k, ctx.pad, xp, gp, out=sink)
     return None
   return ConvWgradFn.apply(x, gy, ctx.k, ctx.pad, ctx.group, xp, gp)
 
@@ -398,6 +442,7 @@ class ConvFn(Function):
   @staticmethod
   def forward(ctx, x, w, k, pad, group):
     ctx.k, ctx.pad, ctx.group, ctx.xshape = k, pad, group, tuple(x.shape)
+    ctx.serial = _next_serial()
     y, xp = _conv_fwd(x, w, k, pad)
     ctx.save_for_backward(x if xp is None else None, xp, w)
     return y
@@ -416,6 +461,7 @@ class ConvDgradFn(Function):
   @staticmethod
   def forward(ctx, gy, w, x_shape, k, pad, group, gy_planes=None):
     ctx.k, ctx.pad, ctx.group = k, pad, group
+    ctx.serial = _next_serial()
     gx, gp = _conv_dgrad(gy, w, tuple(x_shape), k, pad, gy_planes)
     ctx.save_for_backward(gy if gp is None else None, gp, w)
     return gx
@@ -470,6 +516,7 @@ class ConvBiasActFn(Function):
     ctx.set_materialize_grads(False)
     ctx.k, ctx.pad, ctx.group, ctx.act = k, pad, group, act
     ctx.xshape = tuple(x.shape)
+    ctx.serial = _next_serial()
     zp = _new_planes((N, H, W_, Cout), x.device) if emit_planes else None
     mask = None
     if act and ACT_SIGN_MASK and _epilogue_slots(N, H, W_, Cin, Cout, k, pad):
@@ -732,6 +779,7 @@ class GenLayerFn(Function):
     ctx.k, ctx.pad, ctx.kind, ctx.flags, ctx.group = k, pad, kind, flags, group
     ctx.gs, ctx.dom_mask = gs, int(dom_mask)
     ctx.xshape = (N, H, W_, Cin)
+    ctx.serial = _next_serial()
     ctx.pool = pool is not None
     if pool is None:
       return z
@@ -1143,15 +1191,20 @@ def tc_channel_pad(c: int) -> int:
 # count).  The padded tensor is a per-step temporary, so its weight gradient goes to a temporary sink of the padded
 # shape; flush_padded_sinks() adds the real rows into the variable's own sink.
 # The same mechanism serves weights scaled by the equalized-learning-rate constant (ScaleWeightFn): scratch * scale is
-# added to the variable's sink.  A padded scaled weight chains: its sink is the scaled weight's scratch.
-_PADDED_SINKS = {}   # temporary weight data_ptr -> (temporary (kept alive), scratch gradient, target sink, scale)
+# added to the variable's sink.  A padded scaled weight chains: its sink is the scaled weight's scratch.  Each entry
+# also keeps the variable's own sink at the end of the chain, so that one gradient set can be flushed on its own.
+_PADDED_SINKS = {}   # temporary weight data_ptr -> (temporary (kept alive), scratch gradient, target sink, scale, variable sink)
 
 
 def _sink_target(w):
+  """(sink the gradient of `w` goes to, the variable's own sink at the end of the chain), or (None, None)."""
   s = _GRAD_SINKS.get(w.data_ptr())
-  if s is None and w.data_ptr() in _PADDED_SINKS:
-    s = _PADDED_SINKS[w.data_ptr()][1]
-  return s
+  if s is not None:
+    return s, s
+  if w.data_ptr() in _PADDED_SINKS:
+    e = _PADDED_SINKS[w.data_ptr()]
+    return e[1], e[4]
+  return None, None
 
 
 class PadCinFn(Function):
@@ -1162,9 +1215,9 @@ class PadCinFn(Function):
     out = torch.zeros((k, k, int(cpad), cout), device=w.device, dtype=torch.float32)
     lib().call('twg_copy_cols', _p(w), _p(out), k * k, cin * cout, 0, int(cpad) * cout, 0, cin * cout, _st())
     ctx.wshape = tuple(w.shape)
-    sink = _sink_target(w)
+    sink, root = _sink_target(w)
     if sink is not None:
-      _PADDED_SINKS[out.data_ptr()] = (out, torch.zeros_like(out), sink, 1.0)
+      _PADDED_SINKS[out.data_ptr()] = (out, torch.zeros_like(out), sink, 1.0, root)
     return out
 
   @staticmethod
@@ -1180,8 +1233,16 @@ def pad_cin(w, cpad):
   return PadCinFn.apply(w, int(cpad))
 
 
-def flush_padded_sinks() -> None:
-  for out, scratch, sink, scale in reversed(list(_PADDED_SINKS.values())):   # a padded scaled weight flushes first
+def flush_padded_sinks(within: Optional[torch.Tensor] = None) -> None:
+  """Add the scratch gradients into their sinks and forget them.  `within`: only the entries whose variable's sink lies in
+  this slice of the gradient buffer (one gradient set); the others stay for a later call."""
+  keys = list(_PADDED_SINKS)
+  if within is not None:
+    lo = within.data_ptr()
+    hi = lo + within.numel() * within.element_size()
+    keys = [k for k in keys if lo <= _PADDED_SINKS[k][4].data_ptr() < hi]
+  for key in reversed(keys):                    # a padded scaled weight flushes first
+    out, scratch, sink, scale, _ = _PADDED_SINKS.pop(key)
     if out.numel() == sink.numel():             # a scaled weight (the fc weight is a [1,1,C,1] view of its [C,1] variable)
       tmp = scratch
     else:
@@ -1190,7 +1251,6 @@ def flush_padded_sinks() -> None:
       tmp = torch.empty_like(sink)
       lib().call('twg_copy_cols', _p(scratch), _p(tmp), k * k, cpad * cout, 0, cin * cout, 0, cin * cout, _st())
     lib().call('twg_axpby', _p(tmp), _p(sink), _p(sink), float(scale), 1.0, sink.numel(), _st())
-  _PADDED_SINKS.clear()
 
 
 class ScaleWeightFn(Function):
@@ -1205,9 +1265,9 @@ class ScaleWeightFn(Function):
     ctx.c = float(c)
     out = torch.empty_like(w)
     lib().call('twg_axpby', _p(w), None, _p(out), float(c), 0.0, w.numel(), _st())
-    sink = _sink_target(w)
+    sink, root = _sink_target(w)
     if sink is not None:
-      _PADDED_SINKS[out.data_ptr()] = (out, torch.zeros_like(out), sink, float(c))
+      _PADDED_SINKS[out.data_ptr()] = (out, torch.zeros_like(out), sink, float(c), root)
     return out
 
   @staticmethod

@@ -367,7 +367,8 @@ class GanModel:
     """Both gradient sets of one step into the flat gradient buffer.  Every parameter gradient is accumulated straight
     into its slice of that buffer by the kernel that produces it ("sinks": wgrad atomics, normaliser / bias column
     sums), so autograd neither sums per-use gradients of a shared variable nor packs them afterwards.
-    `after_generator_backward`: callback run between the two backward passes (gradient all-reduce overlap)."""
+    `after_generator_backward`: callback run between the two backward passes, once the generator-set slice of the buffer
+    is final (gradient all-reduce overlap)."""
     v = self.variables
     ops.begin_step()
     self._sync_counters()
@@ -386,12 +387,19 @@ class GanModel:
       # accumulators were created on, which a CUDA-graph capture of the step does not survive.
       with ops.skip_param_grads('D'):
         torch.autograd.grad(g_loss, self._g_cut, retain_graph=True, allow_unused=True)
+      # the scratch gradients of the generator set's scaled weights (--equalized_learning_rate) go into their sinks now,
+      # so the generator-set slice of the buffer is final from here on: the discriminator backward adds nothing to it
+      ops.flush_padded_sinks(v.group_slice(self.flat_grad, 'G'))
       if after_generator_backward is not None:
-        after_generator_backward()       # the generator-set slice of the buffer is final from here on
-      with ops.skip_param_grads('G'):
+        after_generator_backward()
+      # with residual blocks the discriminator's weights are reached through diamonds in both the forward and the penalty's
+      # double backward: their gradients are added in the order of the conv nodes, not in the order autograd runs them
+      with ops.skip_param_grads('G'), ops.fixed_order_weight_grads('D' if self.flags.use_res_block else None):
         torch.autograd.grad(d_loss, self._d_cut, allow_unused=True)
+      ops.flush_weight_grads()
       ops.flush_padded_sinks()
     finally:
+      ops.drop_weight_grads()
       ops.drop_padded_sinks()
       ops.require_sinks(False)
       ops.register_grad_sinks({})      # sinks are only valid while this model's step is being differentiated
