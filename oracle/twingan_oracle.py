@@ -746,17 +746,62 @@ def apply_stat_updates(cfg: Config, norm_state: Dict[str, Tensor], nets: Nets) -
     norm_state[base + 'moving_variance' + d] = norm_state[base + 'moving_variance' + d] * decay + mv * (1 - decay)
 
 
+def adam_applies(cfg: Config, params, adam_m, adam_v, grads, adam_t: int, groups) -> int:
+  """The Adam applies of one run, in order, each on one list of variable names: one optimizer => shared beta powers,
+  t advances per apply (model/model_inheritor.py:537-542).  Updates params / adam_m / adam_v in place; returns t."""
+  t = adam_t
+  for names in groups:
+    t += 1
+    for k in names:
+      params[k], adam_m[k], adam_v[k] = adam_apply(cfg, params[k], grads[k], adam_m[k], adam_v[k], t)
+  return t
+
+
+def step_update(cfg: Config, params, adam_m, adam_v, norm_state, nets: Nets, grads, adam_t: int) -> int:
+  """What a mode-B step does after its gradients: the generator apply, then the discriminator apply
+  (image_generation.py:640), then the EMA pushes.  global_step advances by one.  Returns Adam's t."""
+  t = adam_applies(cfg, params, adam_m, adam_v, grads, adam_t,
+                   (generator_variable_names(params), discriminator_variable_names(params)))
+  apply_stat_updates(cfg, norm_state, nets)
+  return t
+
+
 def train_step(cfg: Config, params, adam_m, adam_v, norm_state, sources, targets, dragan_rand, adam_t: int):
   """One 'simultaneous' step (SURVEY 8d mode B): both gradient sets on one batch, then BOTH Adam applies
   (G first: image_generation.py:640; one optimizer => shared beta powers, t advances per apply)."""
   g_loss, d_loss, named, grads, ends, nets = step_gradients(cfg, params, norm_state, sources, targets, dragan_rand)
-  t = adam_t
-  for names in (generator_variable_names(params), discriminator_variable_names(params)):
-    t += 1
-    for k in names:
-      params[k], adam_m[k], adam_v[k] = adam_apply(cfg, params[k], grads[k], adam_m[k], adam_v[k], t)
-  apply_stat_updates(cfg, norm_state, nets)
+  t = step_update(cfg, params, adam_m, adam_v, norm_state, nets, grads, adam_t)
   return g_loss, d_loss, named, grads, t
+
+
+def alternating_turn(n_critic_counter: int, n_critic: int) -> str:
+  """image_generation.py:640-646: the generator set is applied when n_critic_counter % n_critic == 0, else the
+  discriminator set."""
+  return 'G' if n_critic_counter % n_critic == 0 else 'D'
+
+
+def alternating_update(cfg: Config, params, adam_m, adam_v, norm_state, nets: Nets, grads, adam_t: int,
+                       n_critic_counter: int, n_critic: int):
+  """What a mode-A run does after its gradients (image_generation.py:622-651): ONE Adam apply, at t + 1, on the turn's
+  variables (tf.cond of :640-646; the single optimizer's beta powers advance on every apply); the EMA pushes, which are
+  created outside the tf.cond branches and run on every turn; n_critic_counter + 1 (apply_gradients' `step`, :641-645);
+  global_step + 1 on generator turns only (:648-651).  Returns (turn, t, n_critic_counter, global_step increment)."""
+  turn = alternating_turn(n_critic_counter, n_critic)
+  names = generator_variable_names(params) if turn == 'G' else discriminator_variable_names(params)
+  t = adam_applies(cfg, params, adam_m, adam_v, grads, adam_t, (names,))
+  apply_stat_updates(cfg, norm_state, nets)
+  return turn, t, n_critic_counter + 1, 1 if turn == 'G' else 0
+
+
+def train_step_alternating(cfg: Config, params, adam_m, adam_v, norm_state, sources, targets, dragan_rand, adam_t: int,
+                           n_critic_counter: int, n_critic: int = 2):
+  """One mode-A run (image_generation.py:599-655): both gradient sets on one batch, then alternating_update.
+  cfg.global_step (renorm clipping) and cfg.alpha_grow are the run's, i.e. those before its increment.
+  Returns (g_loss, d_loss, named, grads, turn, t, n_critic_counter, global_step increment)."""
+  g_loss, d_loss, named, grads, ends, nets = step_gradients(cfg, params, norm_state, sources, targets, dragan_rand)
+  turn, t, counter, dgs = alternating_update(cfg, params, adam_m, adam_v, norm_state, nets, grads, adam_t,
+                                             n_critic_counter, n_critic)
+  return g_loss, d_loss, named, grads, turn, t, counter, dgs
 
 
 def inference(cfg: Config, params, norm_state, sources: Tensor, target_domain: str = 't') -> Tensor:

@@ -5,6 +5,7 @@ from __future__ import annotations
 import math
 import os
 import sys
+from dataclasses import dataclass, replace
 
 import torch
 
@@ -227,55 +228,127 @@ def oracle_config(hw, is_growing, alpha, mc, norm, num_clones=1, global_step=0, 
                   num_clones=num_clones, global_step=global_step, **kw)
 
 
-def run_step_parity(hw=8, batch=4, max_num_channels=32, norm='instance_norm', is_growing=False, alpha=0.5, seed=0,
-                    prec=None, check_adam=True, verbose=False, tol=REL_TOL, global_step=0, batch_passes=True,
-                    extra_flags=None, weight_scale=1.0, grad_floor=0.0, loose=None):
-  """One TwinGAN G+D step on the device vs the fp64 oracle on identical seeded inputs.
+@dataclass
+class RefCounters:
+  """The reference's counters, kept by its rules and never read back from the model: Adam's t advances per apply
+  (model/model_inheritor.py:537-542), n_critic_counter per mode-A run (image_generation.py:622, 641-645), global_step per
+  mode-B step and per mode-A generator turn (:648-651)."""
+  adam_t: int = 0
+  global_step: int = 0
+  n_critic_counter: int = 0
+
+
+def _by_name(v, flat):
+  return {n: flat[o:o + math.prod(s)].view(s).detach().cpu().double() for n, (o, s) in v.offsets.items()}
+
+
+def entry_state(model, renorm=True):
+  """What a step starts from, read off the device in fp64: parameters, Adam slots and normaliser state under the
+  reference's names (`renorm`: with the renorm_* entries, which only batch_renorm has), and the device step counters."""
+  v = model.variables
+  return {'params': _by_name(v, v.flat), 'adam_m': _by_name(v, v.adam_m), 'adam_v': _by_name(v, v.adam_v),
+          'state': {k: t.detach().cpu().double() for k, t in v.state_to_dict(renorm).items()},
+          'counters': model._counters.tolist()}
+
+
+def _f32(x):
+  return float(torch.tensor(float(x), dtype=torch.float32))
+
+
+# c of the Adam kernel's m and v: a few roundings each, relative to the magnitudes of their two terms
+ADAM_C = 8 * U32
+# twg_step_schedule's lr_t (fp64 arithmetic on the fp32 flags, rounded to fp32) against lr_t of the exact flags
+LR_REL = 1e-6
+
+
+def adam_ref(cfg, p, g, m0, v0, t):
+  """One apply of the fp32 Adam kernel at time t from the fp32 entry values p, m0, v0 and the gradient g (fp64 tensors):
+  O.adam_apply on the flags as the kernel receives them (fp32), and bounds in the way of the Adam stage test's, for one
+  apply from nonzero slots: m within ADAM_C of Ma = |b1 m0| + |(1 - b1) g|, v within ADAM_C of v (no cancellation), sqrt
+  halves that; the quotient and the product add a few roundings, p's rounding one of |p'|, lr_t's rounding to fp32 one of
+  the update.  Returns (update p' - p, m', v', bound on the update, Ma)."""
+  c32 = replace(cfg, learning_rate=_f32(cfg.learning_rate), adam_beta1=_f32(cfg.adam_beta1),
+                adam_beta2=_f32(cfg.adam_beta2), adam_eps=_f32(cfg.adam_eps))
+  p1, m1, v1 = O.adam_apply(c32, p, g, m0, v0, t)
+  b1, b2 = c32.adam_beta1, c32.adam_beta2
+  lr_t = c32.learning_rate * math.sqrt(1 - b2 ** t) / (1 - b1 ** t)
+  Ma = b1 * m0.abs() + (1 - b1) * g.abs()
+  den = v1.sqrt() + c32.adam_eps
+  upd = (p1 - p).abs()
+  pe = lr_t * (ADAM_C * Ma / den + m1.abs() / den * (0.5 * ADAM_C + 4 * U32)) + 2 * U32 * (p1.abs() + upd)
+  return p1 - p, m1, v1, pe, Ma
+
+
+def lr_t(cfg, t):
+  return cfg.learning_rate * math.sqrt(1 - cfg.adam_beta2 ** t) / (1 - cfg.adam_beta1 ** t)
+
+
+class _Captured(object):
+  """Runs `run()` with ops.ACTIVE_SET_TRACE on, keeping what the model's compute_gradients returned (the forward end points
+  the entry points do not return)."""
+
+  def __init__(self, model, run):
+    from twingan_b200 import ops
+    self.calls = []
+    orig = model.compute_gradients
+
+    def spy(*a, **k):
+      out = orig(*a, **k)
+      self.calls.append(out)
+      return out
+    model.compute_gradients = spy                # instance attribute: train_step's self.compute_gradients finds it
+    ops.ACTIVE_SET_TRACE = {'lrelu': [], 'l1': []}
+    try:
+      self.result = run()
+      torch.cuda.synchronize()
+      self.trace = ops.ACTIVE_SET_TRACE
+    finally:
+      ops.ACTIVE_SET_TRACE = None
+      del model.compute_gradients
+    assert len(self.calls) == 1, 'the step computed its gradients %d times' % len(self.calls)
+
+
+def check_step(model, run, cfg, sources, targets, rand, ref, alternating=False, n_critic=2, tol=REL_TOL, grad_floor=0.0,
+               loose=None):
+  """Run one real training step of `model` (`run()`: train_step, train_step_alternating, or whatever calls one of them)
+  and hold it to the fp64 oracle evaluated once from the device's own entry state (teacher forcing: errors do not
+  compound over steps, and any state the device carries from step to step and gets wrong shows on that step).
+
+  `cfg`: the oracle configuration of the step, its global_step and alpha_grow those of the reference's counters `ref`
+  (RefCounters at entry), which this advances by the reference's rules: a mode-B step applies the generator set at t + 1,
+  the discriminator set at t + 2, global_step + 1; a mode-A run (`alternating`) applies the set of its turn
+  (n_critic_counter % n_critic) at t + 1, n_critic_counter + 1, global_step + 1 on generator turns.
 
   Gradients of a leaky-ReLU / L1 network are discontinuous where a pre-activation (pixel difference) crosses
   zero, and an element within rounding noise of the kink takes either slope in ANY finite-precision evaluation.
   Parity is therefore defined modulo the sub-gradient choice at the kink: the device run exports its active set
   (sign masks, test hook ops.ACTIVE_SET_TRACE) and the oracle is evaluated on the same side of every kink, after
-  verifying that the two active sets differ only on elements within O.KINK_AMBIGUITY (1e-3 rms, the forward tolerance) of the kink.
-  Every forward value, loss and gradient tensor must then agree within `tol` (1e-3, north_star)."""
-  from twingan_b200 import ops, twingan
-  if prec is not None:
-    ops.set_precision(prec)
-  # `extra_flags`: optional reference flags (SURVEY 8f-4) under the names both Flags and the oracle's Config use;
-  # `weight_scale` multiplies the N(0, 0.02) conv / fc weights (equalized lr expects N(0, 1) weights)
-  extra_flags = dict(extra_flags or {})
-  cfg = oracle_config(hw, is_growing, alpha, max_num_channels, norm, global_step=global_step, **extra_flags)
-  params = O.init_params(cfg, seed=1234 + seed, randomize_affine=True)
-  if weight_scale != 1.0:
-    params = {k: (v * weight_scale if k.endswith('/weights') else v) for k, v in params.items()}
-  state = O.init_norm_state(cfg, seed=77 + seed)
-  src, tgt, rand = O.make_inputs(cfg, batch, seed=seed)
-
-  flags = twingan.Flags(train_image_size=hw, is_growing=is_growing, alpha_grow=alpha,
-                        pggan_max_num_channels=max_num_channels, generator_norm_type=norm, global_step=global_step,
-                        batch_passes=batch_passes, **extra_flags)
-  model = twingan.GanModel(flags, device='cuda:0')
-  model.variables.load_dict(params, state if state else None)
-  dev = model.device
-  f32 = lambda t: t.to(device=dev, dtype=torch.float32).contiguous()
-  rand_d = {k: f32(v) for k, v in rand.items()}
-  ops.ACTIVE_SET_TRACE = {'lrelu': [], 'l1': []}
-  try:
-    gl, dl, ends_d, stats = model.compute_gradients(f32(src), f32(tgt), rand_d)
-    torch.cuda.synchronize()
-    trace = ops.ACTIVE_SET_TRACE
-  finally:
-    ops.ACTIVE_SET_TRACE = None
-  trace = twingan.GanModel.trace_in_reference_order(trace, batch)
+  verifying that the two active sets differ only on elements within O.KINK_AMBIGUITY (1e-3 rms, the forward tolerance) of
+  the kink.  Every forward value, loss and gradient tensor must then agree within `tol` (1e-3, north_star), and so must
+  the normaliser state after the EMA pushes.  Adam is compared on the device's own gradients (m / (sqrt(v) + eps) is
+  sign-like on a fresh slot, so each side's own gradient would turn 1e-7 noise into +-lr_t differences): the update
+  p' - p, m and v of each applying group against adam_ref's bounds; a group that does not apply keeps p, m and v bit for
+  bit.  Counters: the device's {adam_t, global_step} equal the reference's after the step, lr_t of the step's applies
+  matches the reference's t within LR_REL, and the renorm clipping is that of the reference's global_step.
+  Returns {'ok', 'worst', 'bad', 'details', 'kink_flips', 'turn', 'result': what run() returned}."""
+  from twingan_b200 import twingan
+  renorm = cfg.generator_norm_type == O.BATCH_RENORM_TYPE
+  entry = entry_state(model, renorm)
+  cap = _Captured(model, run)
+  _, _, ends_d, _ = cap.calls[0]
+  B = int(sources.shape[0])
+  d64 = lambda t: t.detach().cpu().double()
+  src, tgt, rnd = d64(sources), d64(targets), {k: d64(t) for k, t in rand.items()}
+  trace = twingan.GanModel.trace_in_reference_order(cap.trace, B)
   O.ACTIVE_SET = {'lrelu': iter(trace['lrelu']), 'l1': iter(trace['l1']), 'flips': [0, 0]}
   try:
-    g_loss, d_loss, named, grads, ends, nets = O.step_gradients(cfg, params, state, src, tgt, rand)
+    g_loss, d_loss, named, grads, ends, nets = O.step_gradients(cfg, entry['params'], entry['state'], src, tgt, rnd)
     flips = tuple(O.ACTIVE_SET['flips'])
     assert next(O.ACTIVE_SET['lrelu'], None) is None and next(O.ACTIVE_SET['l1'], None) is None, 'call-order mismatch'
   finally:
     O.ACTIVE_SET = None
 
-  details = {}
+  details, bounds, exact = {}, {}, []
   worst = 0.0
 
   def add(name, e):
@@ -283,69 +356,112 @@ def run_step_parity(hw=8, batch=4, max_num_channels=32, norm='instance_norm', is
     details[name] = e
     worst = max(worst, e)
 
-  add('generator_loss', abs(gl.item() - g_loss.item()) / abs(g_loss.item()))
-  add('discriminator_loss', abs(dl.item() - d_loss.item()) / abs(d_loss.item()))
-  for k, v in named.items():
-    add('loss/' + k, abs(model.last_losses[k].item() - v.item()) / max(abs(v.item()), 1e-12))
+  # losses, forward end points, both gradient sets
+  for k, ref_loss in (('generator_loss', g_loss), ('discriminator_loss', d_loss)):
+    add(k, abs(model.last_losses[k].item() - ref_loss.item()) / abs(ref_loss.item()))
+  for k, val in named.items():
+    add('loss/' + k, abs(model.last_losses[k].item() - val.item()) / max(abs(val.item()), 1e-12))
   for k in ('s_prime', 't_prime', 's_cycle', 't_cycle', 'enc_s', 'enc_t_prime', 'pred_real_s', 'pred_t_prime'):
     add('fwd/' + k, rel_err(ends_d[k], ends[k]))
   v = model.variables
+  gdev = _by_name(v, model.flat_grad)
+  group_of = lambda name: 'D' if name.startswith('discriminator') else 'G'
   # `grad_floor` > 0: a gradient tensor is compared on the scale max(its own max, grad_floor * the largest gradient of
   # its optimiser group).  Needed where a gradient is an (almost) exact cancellation -- e.g. the critic loss
   # mean D(G) - mean D(x) w.r.t. a bias, or a residual shortcut's bias in front of a normalised toRGB (exactly zero) --
   # so that fp32 rounding residue of the cancelling sums is not divided by ~0.
   gmax = {}
   for name in v.offsets:
-    grp = 'D' if name.startswith('discriminator') else 'G'
-    gmax[grp] = max(gmax.get(grp, 0.0), float(grads[name].abs().max()))
-  for name, (o, shape) in v.offsets.items():
-    n = 1
-    for s in shape:
-      n *= s
-    got = model.flat_grad[o:o + n].view(shape)
-    ref = grads[name]
-    floor = grad_floor * gmax['D' if name.startswith('discriminator') else 'G']
-    if grad_floor > 0.0 and float(ref.abs().max()) < floor:
-      add('grad/' + name, float((got.detach().double().cpu() - ref.double()).abs().max()) / floor)
+    gmax[group_of(name)] = max(gmax.get(group_of(name), 0.0), float(grads[name].abs().max()))
+  for name in v.offsets:
+    got, want = gdev[name], grads[name]
+    floor = grad_floor * gmax[group_of(name)]
+    if grad_floor > 0.0 and float(want.abs().max()) < floor:
+      add('grad/' + name, float((got - want).abs().max()) / floor)
     else:
-      add('grad/' + name, rel_err(got, ref))
-  if check_adam:
-    # Adam kernel parity on IDENTICAL gradients (the device's own): m/(sqrt(v)+eps) is sign-like at step 1, so
-    # feeding each side its own gradient would turn 1e-7 gradient noise into +-lr parameter differences.
-    gdev = {}
-    for name, (o, shape) in v.offsets.items():
-      n = 1
-      for s_ in shape:
-        n *= s_
-      gdev[name] = model.flat_grad[o:o + n].view(shape).detach().cpu().double()
-    m = {k: torch.zeros_like(p) for k, p in params.items()}
-    vv = {k: torch.zeros_like(p) for k, p in params.items()}
-    t = 0
-    p2 = {k: p.float().double() for k, p in params.items()}
-    for names in (O.generator_variable_names(params), O.discriminator_variable_names(params)):
-      t += 1
-      for k in names:
-        p2[k], m[k], vv[k] = O.adam_apply(cfg, p2[k], gdev[k], m[k], vv[k], t)
-    model.apply_gradients()
-    got = model.variables.to_dict()
-    upd_err = 0.0
-    for k in p2:
-      upd_err = max(upd_err, rel_err(got[k], p2[k]))
-    add('adam/params', upd_err)
-    if state:
-      O.apply_stat_updates(cfg, state, nets)
-      model.apply_stat_updates(stats)
-      got_state = model.variables.state_to_dict()
-      for k, val in state.items():
-        add('state/' + k, rel_err(got_state[k], val))
-  torch.cuda.synchronize()
-  # `loose`: {substring of a detail name: tolerance} for entries known to be ill-conditioned in fp32 (documented at the caller)
+      add('grad/' + name, rel_err(got, want))
+
+  # Adam, on the device's gradients from the device's entry slots, at the reference's t of each apply
+  t0 = ref.adam_t
+  if alternating:
+    turn = O.alternating_turn(ref.n_critic_counter, n_critic)
+    applies = {turn: t0 + 1}
+    ref.adam_t, ref.n_critic_counter = t0 + 1, ref.n_critic_counter + 1
+    ref.global_step += 1 if turn == 'G' else 0
+    if isinstance(cap.result, tuple) and len(cap.result) == 3 and cap.result[2] != turn:
+      exact.append('turn: the device applied %s, the reference %s' % (cap.result[2], turn))
+  else:
+    turn = None
+    applies = {'G': t0 + 1, 'D': t0 + 2}
+    ref.adam_t, ref.global_step = t0 + 2, ref.global_step + 1
+  after = {'params': _by_name(v, v.flat), 'adam_m': _by_name(v, v.adam_m), 'adam_v': _by_name(v, v.adam_v)}
+  for name in v.offsets:
+    p0, m0, v0 = entry['params'][name], entry['adam_m'][name], entry['adam_v'][name]
+    p1, m1, v1 = after['params'][name], after['adam_m'][name], after['adam_v'][name]
+    grp = group_of(name)
+    if grp not in applies:
+      if not (torch.equal(p0, p1) and torch.equal(m0, m1) and torch.equal(v0, v1)):
+        exact.append('%s moved on a %s turn' % (name, turn))
+      continue
+    dp, m_ref, v_ref, pe, Ma = adam_ref(cfg, p0, gdev[name], m0, v0, applies[grp])
+    for k, r in (('adam/update/' + grp, conv_error_ratio(p1 - p0, dp, pe, 1.0)),
+                 ('adam/m/' + grp, conv_error_ratio(m1, m_ref, Ma, ADAM_C)),
+                 ('adam/v/' + grp, conv_error_ratio(v1, v_ref, v_ref, ADAM_C))):
+      bounds[k] = max(bounds.get(k, 0.0), r)
+
+  # normaliser state after the EMA pushes
+  state_ref = dict(entry['state'])
+  O.apply_stat_updates(cfg, state_ref, nets)
+  got_state = v.state_to_dict(renorm)
+  for k, val in state_ref.items():
+    add('state/' + k, rel_err(got_state[k], val))
+
+  # counters
+  counters = model._counters.tolist()
+  if counters != [ref.adam_t, ref.global_step]:
+    exact.append('device counters %s, reference (adam_t, global_step) %s' % (counters, [ref.adam_t, ref.global_step]))
+  if alternating and model.n_critic_counter != ref.n_critic_counter:
+    exact.append('n_critic_counter %d, reference %d' % (model.n_critic_counter, ref.n_critic_counter))
+  for i, lr_dev in enumerate(model._lr_dev.tolist()):
+    want = lr_t(cfg, t0 + 1 + i)
+    bounds['lr_t/%d' % i] = abs(lr_dev - want) / (LR_REL * want)
+  clip = O.renorm_clipping(cfg.global_step)
+  want_clip = [_f32(clip['rmin']), _f32(clip['rmax']), _f32(clip['dmax'])]
+  if model._clip_dev.tolist() != want_clip:
+    exact.append('renorm clipping %s, reference %s at global_step %d' % (model._clip_dev.tolist(), want_clip,
+                                                                          cfg.global_step))
+
   def tol_for(k):
+    # `loose`: {substring of a detail name: tolerance} for entries known to be ill-conditioned in fp32 (documented at the caller)
     for sub, t in (loose or {}).items():
       if sub in k:
         return max(t, tol)
     return tol
   bad = {k: e for k, e in details.items() if not (e <= tol_for(k))}
+  bad.update({k: r for k, r in bounds.items() if not (r <= 1.0)})
+  bad.update({'exact/%d' % i: msg for i, msg in enumerate(exact)})
+  details.update(bounds)
+  return {'ok': not bad, 'worst': worst, 'bad': bad, 'details': details, 'kink_flips': flips, 'turn': turn,
+          'result': cap.result}
+
+
+def run_step_parity(hw=8, batch=4, max_num_channels=32, norm='instance_norm', is_growing=False, alpha=0.5, seed=0,
+                    prec=None, verbose=False, tol=REL_TOL, global_step=0, batch_passes=True, extra_flags=None,
+                    weight_scale=1.0, grad_floor=0.0, loose=None):
+  """One TwinGAN G+D step (GanModel.train_step) on the device from seeded parameters and normaliser state vs the fp64
+  oracle on identical seeded inputs: check_step's comparison of losses, forward values, gradients, Adam applies,
+  normaliser state and counters."""
+  from twingan_b200 import ops, twingan
+  if prec is not None:
+    ops.set_precision(prec)
+  # `extra_flags`: optional reference flags (SURVEY 8f-4) under the names both Flags and the oracle's Config use;
+  # `weight_scale` multiplies the N(0, 0.02) conv / fc weights (equalized lr expects N(0, 1) weights)
+  extra_flags = dict(extra_flags or {})
+  cfg = oracle_config(hw, is_growing, alpha, max_num_channels, norm, global_step=global_step, **extra_flags)
+  model, (src, tgt, rand) = seeded_model(cfg, batch, seed, weight_scale, batch_passes=batch_passes)
+  res = check_step(model, lambda: model.train_step(src, tgt, rand), cfg, src, tgt, rand,
+                   RefCounters(global_step=global_step), tol=tol, grad_floor=grad_floor, loose=loose)
+  worst, details, flips = res['worst'], res['details'], res['kink_flips']
   _log_result(dict(hw=hw, batch=batch, mc=max_num_channels, norm=norm, growing=is_growing, prec=ops.get_precision(),
                    batched=batch_passes, worst=worst, flips=flips, top=sorted(details.items(), key=lambda kv: -kv[1])[:5]))
   if verbose:
@@ -354,4 +470,26 @@ def run_step_parity(hw=8, batch=4, max_num_channels=32, norm='instance_norm', is
           (hw, batch, max_num_channels, norm, is_growing, ops.get_precision(), seed, flips[0], flips[1], worst))
     for k, e in top:
       print('   %-70s %.3e' % (k, e))
-  return {'ok': not bad, 'worst': worst, 'bad': bad, 'details': details, 'seed': seed, 'kink_flips': flips}
+  res['seed'] = seed
+  return res
+
+
+def seeded_model(cfg, batch, seed=0, weight_scale=1.0, **flags):
+  """A GanModel of `cfg` on cuda:0 loaded with seeded parameters (gamma / beta / biases randomised too) and normaliser
+  state, and a seeded batch with its DRAGAN draws on the device.  `flags`: further twingan.Flags fields."""
+  from twingan_b200 import twingan
+  params = O.init_params(cfg, seed=1234 + seed, randomize_affine=True)
+  if weight_scale != 1.0:
+    params = {k: (v * weight_scale if k.endswith('/weights') else v) for k, v in params.items()}
+  state = O.init_norm_state(cfg, seed=77 + seed)
+  src, tgt, rand = O.make_inputs(cfg, batch, seed=seed)
+  opt = {k: getattr(cfg, k) for k in ('equalized_learning_rate', 'wgan_drift_loss_weight', 'use_res_block',
+                                      'loss_architecture', 'gradient_penalty_lambda', 'gan_weight', 'l_cyc_weight',
+                                      'do_l_cyc_gan', 'l_content_weight', 'learning_rate', 'adam_beta1', 'adam_beta2')}
+  f = twingan.Flags(train_image_size=cfg.hw, is_growing=cfg.is_growing, alpha_grow=cfg.alpha_grow,
+                    pggan_max_num_channels=cfg.max_num_channels, generator_norm_type=cfg.generator_norm_type,
+                    global_step=cfg.global_step, opt_epsilon=cfg.adam_eps, **opt, **flags)
+  model = twingan.GanModel(f, device='cuda:0')
+  model.variables.load_dict(params, state if state else None)
+  f32 = lambda t: t.to(device=model.device, dtype=torch.float32).contiguous()
+  return model, (f32(src), f32(tgt), {k: f32(v) for k, v in rand.items()})

@@ -97,3 +97,65 @@ def test_checkpoint_round_trip_and_growing_hand_off(tmp_path):
   bad['variables'][n0] = torch.zeros(3)
   with pytest.raises(ValueError):
     R.warm_start(m16, bad, ignore_missing_vars=True)
+
+
+class _AlternatingStub(object):
+  """The part of GanModel that run_stage(alternating=True) drives: flags, device and a train_step_alternating that records
+  what each run was given and keeps the model's counters (turn by n_critic_counter; global_step + 1 on generator turns)."""
+
+  def __init__(self, n_critic_counter=0, global_step=0):
+    self.flags = twingan.Flags(train_image_size=8, is_growing=True, global_step=global_step)
+    self.device = torch.device('cpu')
+    self.n_critic_counter = n_critic_counter
+    self.runs = []                       # (batch index, global_step, alpha, turn) of each run
+
+  def train_step_alternating(self, sources, targets, rand):
+    turn = 'G' if self.n_critic_counter % self.flags.n_critic == 0 else 'D'
+    self.runs.append((int(sources[0, 0, 0, 0]), self.flags.global_step, self.flags.alpha_grow, turn))
+    self.n_critic_counter += 1
+    if turn == 'G':
+      self.flags.global_step += 1
+    return torch.zeros(()), torch.zeros(()), turn
+
+
+def test_alternating_stage_counts_generator_turns_as_global_steps(monkeypatch):
+  """image_generation.py:622-651: n_critic_counter counts runs and picks the turn; global_step advances on generator turns
+  only, and it is what alpha (twingan.py:834-835), slim's number_of_steps stop (model/model_inheritor.py:1116-1123),
+  save_every and the checkpoint names count.  With n_critic = 2 a 4-step growing stage is 7 runs: G D G D G D G."""
+  saved = []
+  monkeypatch.setattr(R, 'save_checkpoint', lambda m, d, step: saved.append((step, m.flags.global_step, m.n_critic_counter)))
+  batch_fn = lambda st, i: (torch.full((st.batch_size, st.hw, st.hw, 3), float(i)),) * 2
+  stage = R.Stage(8, True, 2, 4, '4to8')
+  m = _AlternatingStub()
+  log = []
+  assert R.run_stage(m, stage, batch_fn, 'unused', save_every=2, alternating=True, log_fn=lambda s, l: log.append(s)) == 4
+  assert [r[0] for r in m.runs] == list(range(7))                    # batch_fn gets the run index
+  assert [r[3] for r in m.runs] == ['G', 'D'] * 3 + ['G']
+  assert [r[1] for r in m.runs] == [0, 1, 1, 2, 2, 3, 3]              # the global_step each run computes with
+  assert [r[2] for r in m.runs] == [g / 4.0 for g in (0, 1, 1, 2, 2, 3, 3)]
+  assert log == [1, 1, 2, 2, 3, 3, 4]
+  assert m.flags.global_step == 4 and m.n_critic_counter == 7
+  assert saved == [(2, 2, 3), (4, 4, 7), (4, 4, 7)]                  # save_every, then the stage's last checkpoint
+
+  # resumed after an odd number of runs (checkpoint of global step 2 at run 3): the next run is a discriminator turn on
+  # batch 3, and the stage stops at the same run as the uninterrupted one
+  saved.clear()
+  r = _AlternatingStub(n_critic_counter=3, global_step=2)
+  assert R.run_stage(r, stage, batch_fn, 'unused', start_step=2, save_every=2, alternating=True) == 4
+  assert r.runs == m.runs[3:] and saved == [(4, 4, 7), (4, 4, 7)]
+  assert R.runs_to_reach(3, 2, 2) == 4 and R.runs_to_reach(0, 2, 4) == 7 and R.runs_to_reach(5, 3, 0) == 0
+
+
+def test_checkpoint_carries_the_alternating_counter(tmp_path):
+  """n_critic_counter is a variable of the reference's checkpoint (image_generation.py:622): a resume restores it, a new
+  stage starts it at 0 like global_step."""
+  m = _model(8, False, seed=1)
+  m.n_critic_counter, m.flags.global_step = 5, 2
+  ck = R.load_checkpoint(R.save_checkpoint(m, str(tmp_path), 2))
+  assert ck['n_critic_counter'] == 5
+  resumed = _model(8, False, seed=2)
+  R.warm_start(resumed, ck, restore_step=True)
+  assert resumed.n_critic_counter == 5 and resumed.flags.global_step == 2
+  fresh = _model(8, False, seed=3)
+  R.warm_start(fresh, ck, restore_optimizer=False)
+  assert fresh.n_critic_counter == 0 and fresh.flags.global_step == 0

@@ -875,16 +875,15 @@ def test_elementwise_stage_against_fp64(built_lib, key):
 
 def _owners():
   """{suite: the entry points it checks}: the conv suite (every conv entry, and the split kernels it checks bit for bit),
-  the normaliser suite, this file, the step test that replays a captured step across the counters' boundaries, the SWD
-  stage suite, and the translate tests that hold the uint8 front end to the fp64 restatement and the quantisation bit
+  the normaliser suite, this file, the trajectory suite that holds the step counters and the lr_t / renorm clipping
+  derived from them to the reference's after every step of a run, the SWD stage suite, and the translate tests that hold the uint8 front end to the fp64 restatement and the quantisation bit
   for bit."""
   from tests.test_gpu_norm_conformance import _RUNNERS as NORM_RUNNERS
   from tests.test_gpu_swd_conformance import _RUNNERS as SWD_RUNNERS
   return {'test_gpu_conv_conformance': set(_GEOM_AT) | {'twg_split_act', 'twg_split_weights', 'twg_split_weights_table'},
           'test_gpu_norm_conformance': set(NORM_RUNNERS),
           'test_gpu_elementwise_conformance': set(_RUNNERS),
-          'test_gpu_step::test_graph_replay_follows_the_renorm_schedule_and_adam_time': {'twg_step_schedule',
-                                                                                         'twg_step_advance'},
+          'test_gpu_trajectory': {'twg_step_schedule', 'twg_step_advance'},
           'test_gpu_swd_conformance': set(SWD_RUNNERS),
           'test_gpu_translate': {'twg_images_u8_to_batch', 'twg_batch_to_u8'}}
 

@@ -9,14 +9,16 @@ loop here drives `twingan.GanModel`:
   * `alpha_grow(...)`            fade-in coefficient from the global step (twingan.py:834-835)
   * `save_checkpoint / load_checkpoint / latest_checkpoint`
                                  `<train_dir>/model.ckpt-<step>.pt` holding the variables under their TF names
-                                 (SURVEY 8a.4-11), the normaliser state, both Adam slots and the Adam time
+                                 (SURVEY 8a.4-11), the normaliser state, both Adam slots, the Adam time and the
+                                 step counters (global_step, mode A's n_critic_counter)
   * `warm_start(model, ckpt, ignore_missing_vars)`
                                  restore-by-name; a growing stage adds from_rgb/to_rgb/block variables that the
                                  previous stage does not have (pggan_runner.py:143; model_inheritor init_fn)
   * `run_stage / run`            the training loop; fixed stages replay the captured CUDA graphs, growing stages run
                                  eagerly because alpha changes every step
 
-Nothing here touches the data path: batches come from a `batch_fn(stage, step) -> (sources, targets)` callable.
+Nothing here touches the data path: batches come from a `batch_fn(stage, index) -> (sources, targets)` callable, the
+index being the step (mode B) or the run (mode A, run_stage).
 """
 from __future__ import annotations
 
@@ -120,6 +122,7 @@ def model_state(model) -> Dict[str, object]:
       'norm_state': {n: t.cpu() for n, t in v.state_to_dict().items()},
       'adam_m': adam_m, 'adam_v': adam_v, 'adam_t': int(v.adam_t),
       'global_step': int(model.flags.global_step),
+      'n_critic_counter': int(model.n_critic_counter),     # a tf.get_variable of the reference (image_generation.py:622)
       'train_image_size': int(model.flags.train_image_size), 'is_growing': bool(model.flags.is_growing),
   }
 
@@ -178,6 +181,7 @@ def warm_start(model, ckpt: Dict[str, object], ignore_missing_vars: bool = False
     v.adam_t = int(ckpt.get('adam_t', 0))     # one beta-power pair per optimizer (SURVEY 8a.4-5)
   if restore_step:
     model.flags.global_step = int(ckpt.get('global_step', 0))
+    model.n_critic_counter = int(ckpt.get('n_critic_counter', 0))
   from . import ops
   ops.invalidate_weight_cache()
   return missing
@@ -252,6 +256,15 @@ def load_for_inference(path: str, flags, device='cuda'):
 
 
 # -- the loop ----------------------------------------------------------------------------------------------
+def runs_to_reach(n_critic_counter: int, n_critic: int, generator_turns: int) -> int:
+  """Mode-A runs, from run `n_critic_counter` on, up to and including the `generator_turns`-th generator turn (runs whose
+  counter is a multiple of n_critic, image_generation.py:640-646)."""
+  if generator_turns <= 0:
+    return 0
+  first_g = -(-n_critic_counter // n_critic) * n_critic
+  return first_g + (generator_turns - 1) * n_critic + 1 - n_critic_counter
+
+
 BatchFn = Callable[[Stage, int], Tuple[torch.Tensor, torch.Tensor]]
 EvalFn = Callable[[object, int], object]
 
@@ -261,11 +274,15 @@ def run_stage(model, stage: Stage, batch_fn: BatchFn, train_dir: Optional[str] =
               grow_start_number_of_steps: int = 0, dragan_generator: Optional[torch.Generator] = None,
               log_fn: Optional[Callable[[int, Dict[str, float]], None]] = None, alternating: bool = False,
               prefetch: int = 0, eval_every_n_iter_in_training: int = 0, eval_fn: Optional[EvalFn] = None) -> int:
-  """Train `model` for one stage, from `start_step` to min(stage.max_number_of_steps, start_step + max_steps).
+  """Train `model` for one stage, from global step `start_step` to min(stage.max_number_of_steps, start_step + max_steps).
   Returns the step reached.  Growing stages recompute alpha every step (twingan.py:834-835) and therefore run the
   eager step; stable stages capture the step once and replay it.  `alternating`: the reference's own schedule
   (GanModel.train_step_alternating: one Adam apply per run, generator and discriminator turns alternate) instead of
-  the simultaneous mode-B step; `step` then counts runs, like the reference's n_critic_counter.
+  the simultaneous mode-B step.  Steps, and with them alpha, the renorm clipping, the stop, `save_every`, evaluations and
+  checkpoint names, then count generator turns -- global_step advances on those only (image_generation.py:648-651) and
+  slim's number_of_steps stops on it (model/model_inheritor.py:1116-1123) -- while the runs are counted by
+  model.n_critic_counter (:622, 641-645), which `batch_fn` receives as its index so that a resume replays the same
+  batches; `log_fn` is called after every run.
   `prefetch` > 0: `batch_fn` returns HOST tensors; a background thread keeps that many batches ready in pinned memory and
   the host->device copy of batch k+1 runs on a side stream while step k computes (prefetch.py; the reference's
   slim.prefetch_queue, model/model_inheritor.py:425-470).
@@ -276,18 +293,20 @@ def run_stage(model, stage: Stage, batch_fn: BatchFn, train_dir: Optional[str] =
   graphed = False
   step = start_step
   feed = host_feed = None
+  first = model.n_critic_counter if alternating else start_step     # index of the first batch
   if prefetch > 0 and end > start_step:
     from .prefetch import DevicePrefetcher, HostPrefetcher
-    host_feed = HostPrefetcher(lambda i: tuple(batch_fn(stage, start_step + i)), capacity=prefetch, num_batches=end - start_step)
+    num = runs_to_reach(first, model.flags.n_critic, end - start_step) if alternating else end - start_step
+    host_feed = HostPrefetcher(lambda i: tuple(batch_fn(stage, first + i)), capacity=prefetch, num_batches=num)
     feed = DevicePrefetcher(host_feed, model.device)
   while step < end:
-    sources, targets = next(feed) if feed is not None else batch_fn(stage, step)
+    sources, targets = next(feed) if feed is not None else batch_fn(stage, model.n_critic_counter if alternating else step)
     rand = twingan.make_dragan_rand(sources.shape[0], stage.hw, model.device, dragan_generator)
     model.flags.global_step = step
     if stage.is_growing:
       model.flags.alpha_grow = alpha_grow(step, stage.max_number_of_steps, grow_start_number_of_steps)
     if alternating:
-      g, d, _ = model.train_step_alternating(sources, targets, rand)
+      g, d, turn = model.train_step_alternating(sources, targets, rand)
     elif stage.is_growing:
       g, d = model.train_step(sources, targets, rand)
     elif use_graph and model.device.type == 'cuda':
@@ -299,6 +318,10 @@ def run_stage(model, stage: Stage, batch_fn: BatchFn, train_dir: Optional[str] =
       g, d = model.train_step(sources, targets, rand)
     if feed is not None:
       feed.release()
+    if alternating and turn != 'G':      # a discriminator turn leaves global_step where it was
+      if log_fn is not None:
+        log_fn(step, {'generator_loss': float(g), 'discriminator_loss': float(d)})
+      continue
     step += 1
     if log_fn is not None:
       log_fn(step, {'generator_loss': float(g), 'discriminator_loss': float(d)})
@@ -317,15 +340,17 @@ def run_stage(model, stage: Stage, batch_fn: BatchFn, train_dir: Optional[str] =
 def run(base_flags, base_dir: str, batch_fn: BatchFn, stages: Optional[Iterable[Stage]] = None,
         max_steps_per_stage: Optional[int] = None, device='cuda', seed: int = 1234, process_group=None,
         save_every: int = 0, use_graph: bool = True, log_fn=None, tf_checkpoint_prefix: Optional[str] = None,
-        prefetch: int = 0, eval_every_n_iter_in_training: int = 0, eval_fn: Optional[EvalFn] = None):
+        prefetch: int = 0, eval_every_n_iter_in_training: int = 0, eval_fn: Optional[EvalFn] = None,
+        alternating: bool = False, dragan_generator: Optional[torch.Generator] = None):
   """pggan_runner.py main(): walk the stage plan; skip stages whose checkpoint already reached the stage's step count
   (:117-121); resume a partially trained stage from its own directory; otherwise warm-start from the previous
   stage's directory with ignore_missing_vars = is_growing (:137-146).  `tf_checkpoint_prefix`: a TensorFlow V2
   checkpoint of the reference (e.g. its pretrained models) that seeds the first stage that has nothing to start
   from (twingan_b200/tf_checkpoint.py).  `prefetch` > 0: `batch_fn` returns host tensors that are produced on a background
   thread and copied ahead of the step (run_stage).  `eval_every_n_iter_in_training` / `eval_fn`: periodic evaluation as in
-  run_stage, for the stages of 16 x 16 and up (the reference skips SWD below 16, image_generation.py:869-871).  Returns the
-  last model."""
+  run_stage, for the stages of 16 x 16 and up (the reference skips SWD below 16, image_generation.py:869-871).
+  `alternating` / `dragan_generator`: as in run_stage; a resumed stage restores global_step and n_critic_counter from its
+  checkpoint, a new stage starts both at 0.  Returns the last model."""
   from . import twingan
   last_train_dir = None
   model = None
@@ -354,7 +379,8 @@ def run(base_flags, base_dir: str, batch_fn: BatchFn, stages: Optional[Iterable[
       tf_checkpoint.import_into(model, tf_checkpoint_prefix, ignore_missing_vars=True)
     run_stage(model, st, batch_fn, train_dir, start_step=start,
               max_steps=None if max_steps_per_stage is None else target - start, save_every=save_every,
-              use_graph=use_graph, log_fn=log_fn, prefetch=prefetch,
+              use_graph=use_graph, log_fn=log_fn, prefetch=prefetch, alternating=alternating,
+              dragan_generator=dragan_generator,
               eval_every_n_iter_in_training=eval_every_n_iter_in_training if st.hw >= 16 else 0, eval_fn=eval_fn)
     last_train_dir = train_dir
   return model

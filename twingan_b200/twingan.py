@@ -478,8 +478,10 @@ class GanModel:
     applies only one -- the generator set when n_critic_counter % n_critic == 0 (so the very first run is a generator
     turn), the discriminator set otherwise; the counter advances on every apply, global_step only on generator turns,
     and the single Adam object's beta powers advance on every apply.  The normalisers' moving-average pushes are
-    created outside the tf.cond branches and attached as control dependencies, so they run on every turn.
+    created outside the tf.cond branches and attached as control dependencies, so they run on every turn.  The device
+    counters advance with their host mirrors, as they do in the mode-B step.
     Returns (generator_loss, discriminator_loss, 'G' | 'D')."""
+    from ._lib import lib
     f, v = self.flags, self.variables
     g_loss, d_loss, ends, stats = self.compute_gradients(sources, targets, dragan_rand)
     self.allreduce_gradients()
@@ -493,8 +495,10 @@ class GanModel:
       v.weight_table.refresh()
     self.apply_stat_updates(stats)
     self.n_critic_counter += 1
-    if turn == 'G':
-      f.global_step += 1
+    dgs = 1 if turn == 'G' else 0
+    f.global_step += dgs
+    lib().call('twg_step_advance', self._counters.data_ptr(), 1, dgs, ops._st())
+    self._counters_mirror = (self._counters_mirror[0] + 1, self._counters_mirror[1] + dgs)
     return g_loss, d_loss, turn
 
   # -- CUDA-graph replay of the whole step -------------------------------------------------------------
