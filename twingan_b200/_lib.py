@@ -1,4 +1,4 @@
-"""ctypes binding of libtwg.so (the C-ABI declared in include/twg.h).
+"""ctypes binding of libtwg.so (the C-ABI declared in include/twg.h, and the JPEG decoder's in include/twgjpeg.h).
 
 The prototypes are parsed from the header itself so the Python side can never drift from the ABI.
 There is no CPU fallback: if the library is missing, or a kernel entry point is called without a CUDA
@@ -13,6 +13,8 @@ from typing import Dict, List, Tuple
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'twg.h')
+JPEG_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'twgjpeg.h')
+JPEG_PREFIX = 'twgjpeg_'
 LIB_PATH = os.environ.get('TWG_LIB') or os.path.join(_HERE, 'libtwg.so')   # TWG_LIB: A/B builds of the same ABI
 
 _CTYPES = {
@@ -23,14 +25,14 @@ _CTYPES = {
 }
 
 
-def parse_header(path: str = HEADER) -> Dict[str, Tuple[str, List[str]]]:
-  """Returns {symbol: (return type, [arg types])} for every function declared in twg.h."""
+def parse_header(path: str = HEADER, prefix: str = 'twg_') -> Dict[str, Tuple[str, List[str]]]:
+  """Returns {symbol: (return type, [arg types])} for every function named `prefix`* declared in the header (twg.h)."""
   src = open(path).read()
   src = re.sub(r'/\*.*?\*/', '', src, flags=re.S)
   src = re.sub(r'//[^\n]*', '', src)
   src = '\n'.join(l for l in src.splitlines() if not l.strip().startswith('#'))
   protos = {}
-  for m in re.finditer(r'(const char\*|int64_t|int|void)\s+(twg_\w+)\s*\(([^)]*)\)\s*;', src):
+  for m in re.finditer(r'(const char\*|int64_t|int|void)\s+(' + re.escape(prefix) + r'\w+)\s*\(([^)]*)\)\s*;', src):
     ret, name, args = m.group(1), m.group(2), m.group(3).strip()
     types: List[str] = []
     if args and args != 'void':
@@ -54,7 +56,8 @@ class _Lib:
                      '(there is no CPU fallback)')
     self.cdll = ctypes.CDLL(LIB_PATH)
     self.protos = parse_header()
-    for name, (ret, args) in self.protos.items():
+    self.jpeg_protos = parse_header(JPEG_HEADER, JPEG_PREFIX)
+    for name, (ret, args) in list(self.protos.items()) + list(self.jpeg_protos.items()):
       fn = getattr(self.cdll, name)  # raises AttributeError if the symbol is not exported
       fn.restype = _CTYPES[ret]
       fn.argtypes = [_CTYPES[a] for a in args]

@@ -1,0 +1,324 @@
+"""Host side of the device JPEG decoder (csrc/twg_jpeg.cu): read a file's headers, decide whether the device decodes it,
+and pack the descriptors of a batch.
+
+A file goes to the device only if libjpeg (as PIL calls it) would decode it through the path the kernels restate:
+  * baseline sequential Huffman: SOF0, or SOF1 with 8-bit samples; one scan (Ss 0, Se 63, Ah 0, Al 0) holding every
+    component in frame order, ended by EOI;
+  * 1 component, or 3 that libjpeg reads as YCbCr: a JFIF APP0, or an Adobe APP14 with transform 1, or neither marker
+    and component ids 1, 2, 3 (jdapimin.c default_decompress_parms, nothing looser);
+  * 4:4:4, 4:2:2 (luma 2x1) or 4:2:0 (luma 2x2), chroma 1x1;
+  * every Huffman and quantisation table it uses defined before the scan, and every Huffman table valid as libjpeg's
+    jpeg_make_d_derived_tbl checks it.
+DQT (8- or 16-bit), DHT, DRI, any size and APPn / COM segments in any order are accepted.  Everything else -- progressive,
+arithmetic, lossless, 12-bit, CMYK / YCCK, Adobe transform 0, other sampling, DNL, several scans, a scan not ended by EOI,
+anything the parser does not recognise -- is left to PIL: `parse` raises `Unsupported` with the reason.
+
+The segments of a scan (restart intervals when DRI is set, else the whole scan) are found here by their RSTn markers; the
+device checks that each one ends in the marker it should (RSTn in sequence, EOI after the last).
+"""
+from __future__ import annotations
+
+from typing import List, NamedTuple, Sequence, Tuple
+
+import numpy as np
+
+# descriptor row layouts (int64), shared with include/twgjpeg.h
+SEG_FIELDS = 6      # {byte start, byte end, image, first MCU, MCUs, segment index in its image}
+COMP_FIELDS = 10    # {block base, blocks wide, blocks high, plane offset, quant row, DC table, AC table, h, v, image}
+IMAGE_FIELDS = 12   # {first comp, comps, MCUs wide, H, W, payload offset, first pixel, segments, hmax, vmax, 0, 0}
+HUFF_LUT_BITS = 9
+HUFF_WORDS = 1024   # int32 per table: lut[512] | maxcode[18] | valoff[18] | vals[256] | pad
+
+# device status bits (TWG_JPEG_* of include/twgjpeg.h)
+STATUS_BAD_CODE = 1
+STATUS_MARKER = 2
+STATUS_TRUNCATED = 4
+STATUS_RESTART = 8
+STATUS_COEF_RANGE = 16
+STATUS_IDCT_RANGE = 32
+
+
+class Unsupported(ValueError):
+  """The file is not in the subset the device decodes (the reason is the message); PIL decodes it."""
+
+
+class Component(NamedTuple):
+  id: int
+  h: int
+  v: int
+  tq: int
+
+
+class JpegInfo(NamedTuple):
+  H: int
+  W: int
+  comps: Tuple[Component, ...]
+  qt: Tuple[np.ndarray, ...]          # per component: int32 [64], zig-zag order
+  dc: Tuple[Tuple[bytes, bytes], ...]  # per component: (BITS[16], HUFFVAL)
+  ac: Tuple[Tuple[bytes, bytes], ...]
+  restart_interval: int
+  mcux: int
+  mcuy: int
+  segments: Tuple[Tuple[int, int], ...]   # [start, end) byte ranges of the entropy-coded segments in the file
+  scan_start: int
+  eoi: int                             # offset of the FF D9 that ends the scan
+
+  @property
+  def hmax(self):
+    return max(c.h for c in self.comps)
+
+  @property
+  def vmax(self):
+    return max(c.v for c in self.comps)
+
+  @property
+  def mcus(self):
+    return self.mcux * self.mcuy
+
+  def block_dims(self):
+    """(blocks wide, blocks high) of each component as coded."""
+    if len(self.comps) == 1:
+      return [(self.mcux, self.mcuy)]
+    return [(self.mcux * c.h, self.mcuy * c.v) for c in self.comps]
+
+
+def _u16(b, i):
+  return (b[i] << 8) | b[i + 1]
+
+
+def _huff_ok(bits: bytes, vals: bytes, is_dc: bool) -> bool:
+  """jpeg_make_d_derived_tbl's checks: no code runs out of its length, DC symbols <= 15."""
+  code = 0
+  for l in range(1, 17):
+    code += bits[l - 1]
+    if code >= (1 << l):
+      return False
+    code <<= 1
+  return not (is_dc and any(v > 15 for v in vals))
+
+
+def parse(data: bytes) -> JpegInfo:
+  """The header and segment layout of a JPEG file the device decodes; `Unsupported` otherwise."""
+  b = memoryview(data).cast('B') if not isinstance(data, (bytes, bytearray)) else data
+  n = len(b)
+  if n < 4 or b[0] != 0xFF or b[1] != 0xD8:
+    raise Unsupported('not a JPEG stream (no SOI)')
+  pos = 2
+  qt = {}
+  huff = {}
+  ri = 0
+  frame = None
+  jfif = adobe = False
+  transform = None
+  while True:
+    if pos >= n or b[pos] != 0xFF:
+      raise Unsupported('no marker at byte %d' % pos)
+    while pos < n and b[pos] == 0xFF:
+      pos += 1
+    if pos >= n:
+      raise Unsupported('truncated before the scan')
+    m = b[pos]
+    pos += 1
+    if m == 0xD8 or m == 0xD9 or m == 0x01 or 0xD0 <= m <= 0xD7:
+      raise Unsupported('marker %02X before the scan' % m)
+    if pos + 2 > n:
+      raise Unsupported('truncated marker segment')
+    L = _u16(b, pos)
+    if L < 2 or pos + L > n:
+      raise Unsupported('marker %02X: bad length %d' % (m, L))
+    seg = bytes(b[pos + 2:pos + L])
+    pos += L
+    if m in (0xC0, 0xC1):
+      if frame is not None:
+        raise Unsupported('two frame headers')
+      if len(seg) < 6 or seg[0] != 8:
+        raise Unsupported('SOF%d with %d-bit samples' % (m - 0xC0, seg[0] if seg else -1))
+      H, W, nf = _u16(seg, 1), _u16(seg, 3), seg[5]
+      if H == 0 or W == 0:
+        raise Unsupported('image size %dx%d (DNL)' % (H, W))
+      if nf not in (1, 3) or len(seg) != 6 + 3 * nf:
+        raise Unsupported('%d components' % nf)
+      comps = tuple(Component(seg[6 + 3 * i], seg[7 + 3 * i] >> 4, seg[7 + 3 * i] & 15, seg[8 + 3 * i]) for i in range(nf))
+      frame = (H, W, comps)
+    elif 0xC2 <= m <= 0xCF and m not in (0xC4, 0xC8, 0xCC):
+      raise Unsupported('SOF%d (progressive, lossless or arithmetic)' % (m - 0xC0))
+    elif m == 0xCC:
+      raise Unsupported('arithmetic coding (DAC)')
+    elif m == 0xC4:
+      i = 0
+      while i < len(seg):
+        if i + 17 > len(seg):
+          raise Unsupported('bad DHT')
+        tc, th = seg[i] >> 4, seg[i] & 15
+        bits = bytes(seg[i + 1:i + 17])
+        cnt = sum(bits)
+        if tc > 1 or th > 3 or cnt > 256 or i + 17 + cnt > len(seg):
+          raise Unsupported('bad DHT')
+        vals = bytes(seg[i + 17:i + 17 + cnt])
+        if not _huff_ok(bits, vals, tc == 0):
+          raise Unsupported('invalid Huffman table')
+        huff[(tc, th)] = (bits, vals)
+        i += 17 + cnt
+    elif m == 0xDB:
+      i = 0
+      while i < len(seg):
+        pq, tq = seg[i] >> 4, seg[i] & 15
+        size = 64 * (pq + 1)
+        if pq > 1 or tq > 3 or i + 1 + size > len(seg):
+          raise Unsupported('bad DQT')
+        raw = np.frombuffer(seg[i + 1:i + 1 + size], dtype='>u2' if pq else np.uint8)
+        qt[tq] = raw.astype(np.int32)
+        i += 1 + size
+    elif m == 0xDD:
+      if len(seg) != 2:
+        raise Unsupported('bad DRI')
+      ri = _u16(seg, 0)
+    elif m == 0xE0:
+      if len(seg) >= 14 and seg[:5] == b'JFIF\0':
+        jfif = True
+    elif m == 0xEE:
+      if len(seg) >= 12 and seg[:5] == b'Adobe':
+        adobe, transform = True, seg[11]
+    elif 0xE1 <= m <= 0xEF or m == 0xFE:
+      pass
+    elif m == 0xDA:
+      break
+    else:
+      raise Unsupported('marker %02X' % m)
+  if frame is None:
+    raise Unsupported('scan before the frame header')
+  H, W, comps = frame
+  # the scan header
+  ns = seg[0] if seg else 0
+  if ns != len(comps) or len(seg) != 4 + 2 * ns:
+    raise Unsupported('a scan of %d of %d components' % (ns, len(comps)))
+  if [seg[1 + 2 * i] for i in range(ns)] != [c.id for c in comps]:
+    raise Unsupported('scan components not in frame order')
+  if len({c.id for c in comps}) != len(comps):
+    raise Unsupported('duplicate component ids')
+  ss, se, ahal = seg[1 + 2 * ns], seg[2 + 2 * ns], seg[3 + 2 * ns]
+  if ss != 0 or se != 63 or ahal != 0:
+    raise Unsupported('not a sequential scan (Ss %d, Se %d, AhAl %02X)' % (ss, se, ahal))
+  tables = [(seg[2 + 2 * i] >> 4, seg[2 + 2 * i] & 15) for i in range(ns)]
+  # colour space and sampling
+  if len(comps) == 3:
+    if not jfif:
+      if adobe and transform != 1:
+        raise Unsupported('Adobe transform %d' % transform)
+      if not adobe and [c.id for c in comps] != [1, 2, 3]:
+        raise Unsupported('component ids %s without JFIF or Adobe marker' % [c.id for c in comps])
+    y, cb, cr = comps
+    if (cb.h, cb.v, cr.h, cr.v) != (1, 1, 1, 1) or (y.h, y.v) not in ((1, 1), (2, 1), (2, 2)):
+      raise Unsupported('sampling %s' % ['%dx%d' % (c.h, c.v) for c in comps])
+  else:
+    comps = (comps[0]._replace(h=1, v=1),)      # a lone component is coded one block per MCU whatever its factors
+  for c in comps:
+    if c.tq not in qt:
+      raise Unsupported('quantisation table %d undefined' % c.tq)
+  for td, ta in tables:
+    if (0, td) not in huff or (1, ta) not in huff:
+      raise Unsupported('Huffman table undefined')
+  hmax, vmax = max(c.h for c in comps), max(c.v for c in comps)
+  mcux, mcuy = -(-W // (8 * hmax)), -(-H // (8 * vmax))
+  # the entropy-coded data: RSTn split it, the first other marker ends it
+  scan_start = pos
+  arr = np.frombuffer(bytes(b[scan_start:]), dtype=np.uint8)
+  ff = np.flatnonzero(arr[:-1] == 0xFF)
+  nxt = arr[ff + 1]
+  is_marker = (nxt != 0) & (nxt != 0xFF)
+  rst = (nxt >= 0xD0) & (nxt <= 0xD7)
+  ends = np.flatnonzero(is_marker & ~rst)
+  if not len(ends):
+    raise Unsupported('the scan is not ended by a marker')
+  eoi = int(ff[ends[0]])
+  if nxt[ends[0]] != 0xD9:
+    raise Unsupported('marker %02X after the scan (several scans or DNL)' % nxt[ends[0]])
+  cuts = ff[is_marker & rst & (ff < eoi)].tolist()
+  starts = [0] + [c + 2 for c in cuts]
+  stops = cuts + [eoi]
+  segments = tuple((scan_start + s, scan_start + e) for s, e in zip(starts, stops))
+  return JpegInfo(H, W, comps, tuple(qt[c.tq] for c in comps), tuple(huff[(0, t[0])] for t in tables),
+                  tuple(huff[(1, t[1])] for t in tables), ri, mcux, mcuy, segments, scan_start, scan_start + eoi)
+
+
+def probe(data: bytes):
+  """JpegInfo for a file the device decodes, else None."""
+  try:
+    return parse(data)
+  except Unsupported:
+    return None
+
+
+def huff_table(bits: bytes, vals: bytes) -> np.ndarray:
+  """The device form of one Huffman table, int32 [HUFF_WORDS]: lut[2^9] = (length << 8 | symbol) of every code of at most
+  9 bits indexed by the next 9 bits of the stream (0: longer code), maxcode[l] (l = 1..16; -1 when no code has length l,
+  maxcode[17] = INT_MAX), valoff[l] (symbol = vals[code + valoff[l]]), vals[256]."""
+  t = np.zeros(HUFF_WORDS, np.int32)
+  lut, maxcode, valoff, v = t[:512], t[512:530], t[530:548], t[548:804]
+  v[:len(vals)] = np.frombuffer(vals, np.uint8)
+  code = k = 0
+  maxcode[:] = -1
+  for l in range(1, 17):
+    cnt = bits[l - 1]
+    if cnt:
+      valoff[l] = k - code
+      for j in range(cnt):
+        if l <= HUFF_LUT_BITS:
+          lo = (code + j) << (HUFF_LUT_BITS - l)
+          lut[lo:lo + (1 << (HUFF_LUT_BITS - l))] = (l << 8) | vals[k + j]
+      code += cnt
+      k += cnt
+      maxcode[l] = code - 1
+    code <<= 1
+  maxcode[17] = 0x7FFFFFFF
+  return t
+
+
+class Batch(NamedTuple):
+  """Descriptors of the JPEG images of one batch (host int tensors as numpy arrays; see include/twgjpeg.h)."""
+  data: np.ndarray     # uint8: the scans, each through its EOI
+  segs: np.ndarray     # int64 [S, SEG_FIELDS]
+  comps: np.ndarray    # int64 [C, COMP_FIELDS]
+  images: np.ndarray   # int64 [n, IMAGE_FIELDS]
+  qt: np.ndarray       # int32 [Q, 64]
+  huff: np.ndarray     # int32 [T, HUFF_WORDS]
+  blocks: int          # coefficient blocks (scratch: 128 bytes each)
+  plane_bytes: int     # sample planes (scratch)
+  pixels: int
+
+
+def pack(files: Sequence[bytes], infos: Sequence[JpegInfo], payload_offsets: Sequence[int]) -> Batch:
+  """Descriptors for decoding files[i] (described by infos[i]) into a payload at byte payload_offsets[i]."""
+  chunks, segs, comps, images, qts = [], [], [], [], []
+  tables, table_rows = {}, []
+  at = blocks = planes = pixels = 0
+
+  def table(bv):
+    if bv not in tables:
+      tables[bv] = len(table_rows)
+      table_rows.append(huff_table(*bv))
+    return tables[bv]
+
+  for i, (f, info, off) in enumerate(zip(files, infos, payload_offsets)):
+    chunk = f[info.scan_start:info.eoi + 2]
+    base = at - info.scan_start
+    nseg = 1 if info.restart_interval == 0 else -(-info.mcus // info.restart_interval)
+    per = info.mcus if info.restart_interval == 0 else info.restart_interval
+    for s in range(nseg):
+      a, e = info.segments[s] if s < len(info.segments) else (info.eoi, info.eoi)
+      segs.append((a + base, e + base, i, s * per, min(per, info.mcus - s * per), s))
+    first = len(comps)
+    for c, (comp, (bw, bh)) in enumerate(zip(info.comps, info.block_dims())):
+      comps.append((blocks, bw, bh, planes, len(qts), table(info.dc[c]), table(info.ac[c]), comp.h, comp.v, i))
+      qts.append(info.qt[c])
+      blocks += bw * bh
+      planes += bw * bh * 64
+    images.append((first, len(info.comps), info.mcux, info.H, info.W, off, pixels, nseg, info.hmax, info.vmax, 0, 0))
+    pixels += info.H * info.W
+    chunks.append(np.frombuffer(chunk, np.uint8))
+    at += len(chunk)
+  i64 = lambda rows, k: np.asarray(rows, np.int64).reshape(-1, k)
+  return Batch(np.concatenate(chunks) if chunks else np.zeros(0, np.uint8), i64(segs, SEG_FIELDS),
+               i64(comps, COMP_FIELDS), i64(images, IMAGE_FIELDS),
+               np.asarray(qts, np.int32).reshape(-1, 64), np.asarray(table_rows, np.int32).reshape(-1, HUFF_WORDS),
+               blocks, planes, pixels)

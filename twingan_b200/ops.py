@@ -1611,6 +1611,39 @@ def images_u8_to_batch(payload: torch.Tensor, table: torch.Tensor, hw: int, out:
   return out
 
 
+JPEG_STAGES = ('twgjpeg_entropy', 'twgjpeg_idct', 'twgjpeg_color')
+
+
+def jpeg_decode(payload: torch.Tensor, data: torch.Tensor, segs: torch.Tensor, comps: torch.Tensor, images: torch.Tensor,
+                qt: torch.Tensor, huff: torch.Tensor, blocks: int, plane_bytes: int, pixels: int, stage_hook=None
+                ) -> torch.Tensor:
+  """Decode the JPEG scans of one batch into their regions of a uint8 CUDA payload (twgjpeg_entropy, twgjpeg_idct,
+  twgjpeg_color): the descriptors are a jpeg.Batch on the device, `blocks`, `plane_bytes` and `pixels` its host sizes.
+  Returns the int32 [images] device status without waiting for it: 0 for an image decoded bit for bit as libjpeg-turbo,
+  else the TWG_JPEG_* bits of what made the device stop (jpeg.STATUS_*); such an image's region is undefined.
+  `stage_hook(name)`, when given, is called after each stage is enqueued (timing)."""
+  if not payload.is_cuda or payload.dtype != torch.uint8:
+    raise TwgError('jpeg_decode: payload must be a uint8 CUDA tensor (no CPU fallback)')
+  dev = payload.device
+  n = int(images.shape[0])
+  status = torch.empty(n, device=dev, dtype=torch.int32)
+  coefs = torch.empty(blocks * 64, device=dev, dtype=torch.int16)
+  planes = torch.empty(plane_bytes, device=dev, dtype=torch.uint8)
+  L = lib()
+  L.call('twgjpeg_entropy', data.data_ptr(), segs.data_ptr(), int(segs.shape[0]), images.data_ptr(), n,
+         comps.data_ptr(), huff.data_ptr(), coefs.data_ptr(), status.data_ptr(), _st())
+  if stage_hook:
+    stage_hook(JPEG_STAGES[0])
+  L.call('twgjpeg_idct', coefs.data_ptr(), comps.data_ptr(), int(comps.shape[0]), blocks, qt.data_ptr(),
+         planes.data_ptr(), status.data_ptr(), _st())
+  if stage_hook:
+    stage_hook(JPEG_STAGES[1])
+  L.call('twgjpeg_color', planes.data_ptr(), images.data_ptr(), n, comps.data_ptr(), pixels, payload.data_ptr(), _st())
+  if stage_hook:
+    stage_hook(JPEG_STAGES[2])
+  return status
+
+
 def batch_to_u8(x: torch.Tensor) -> torch.Tensor:
   """uint8 image of the model output, clip(x * 255, 0, 255) truncated (util_io.imsave; twg_batch_to_u8)."""
   x = _check(x)

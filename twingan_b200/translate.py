@@ -4,10 +4,16 @@ inference/image_translation_infer.py (docs/infer_and_eval.md), with its flag nam
   python -m twingan_b200.translate --model_path=<train_dir>/256 --image_hw=256 \\
       --input_image_path=<file or directory> --output_image_path=<file or directory>
 
-Decoding and encoding run on the host (PIL, as util_io.imread / imsave); everything between runs on the device.  Per batch:
-  * a background thread decodes the files of batch k+1 on a pool of `--num_decode_threads` threads and packs them into
-    one uint8 payload + a table of {offset, H, W} (HostPrefetcher, pinned memory) while batch k computes;
-  * the payload and table are copied to the device on a side stream (DevicePrefetcher);
+Encoding runs on the host (PIL, as util_io.imsave); decoding runs on the device for baseline JPEG files and on the host
+(PIL, as util_io.imread) for every other file; everything between runs on the device.  Per batch:
+  * a background thread reads the files of batch k+1 on a pool of `--num_decode_threads` threads.  A JPEG that
+    twingan_b200/jpeg.py accepts (baseline Huffman, grey or YCbCr, 4:4:4 / 4:2:2 / 4:2:0) travels compressed, with its
+    descriptors; PIL decodes every other file into its region of one uint8 payload + a table of {offset, H, W}
+    (HostPrefetcher, pinned memory; the JPEG headers give their rows before any decoding) while batch k computes;
+  * the payload, table and compressed scans are copied to the device on a side stream (DevicePrefetcher);
+  * three kernels decode the JPEG scans into their regions of the payload, bit for bit as PIL does (ops.jpeg_decode);
+    the batch's status is read once, and an image the device could not decode exactly is decoded by PIL and written
+    into its region instead (a file PIL refuses fails as before);
   * one kernel converts and resizes the ragged batch to the model input (ops.images_u8_to_batch: convert_image_dtype +
     TF-1 bilinear resize_images), the model translates it (InferencePipeline._infer: a CUDA graph per batch shape), one
     kernel quantises the result (ops.batch_to_u8: util_io.imsave's clip(x * 255).astype(uint8));
@@ -86,6 +92,75 @@ def decode(path: str) -> np.ndarray:
     raise ValueError('cannot decode %s: %s' % (path, e)) from e
 
 
+class _DeviceJpegs(object):
+  """The JPEG files of a batch the device decodes: their paths, their table rows {offset, H, W}, and the host sizes of
+  their jpeg.Batch.  (Not a tuple: the prefetcher maps over tuples.)"""
+
+  def __init__(self, paths, rows, blocks, plane_bytes, pixels):
+    self.paths, self.rows, self.blocks, self.plane_bytes, self.pixels = paths, rows, blocks, plane_bytes, pixels
+
+
+def _read(path: str) -> Optional[bytes]:
+  """The file's bytes, or None when it cannot be read (decode() then raises its usual error)."""
+  try:
+    with open(path, 'rb') as f:
+      return f.read()
+  except OSError:
+    return None
+
+
+def _device_jpeg(data: Optional[bytes]):
+  """jpeg.JpegInfo when the device decodes this file, else None.  Images above PIL's decompression-bomb limit stay with
+  PIL, which warns or refuses as before."""
+  from PIL import Image
+  from . import jpeg
+  info = jpeg.probe(data) if data else None
+  if info is not None and Image.MAX_IMAGE_PIXELS and info.H * info.W > Image.MAX_IMAGE_PIXELS:
+    return None
+  return info
+
+
+def _decode_jpegs(payload: torch.Tensor, descriptors, jpegs: '_DeviceJpegs') -> None:
+  """Decode a batch's JPEG files into their regions of the device payload; an image the device flags is decoded by PIL
+  (decode(), so a file PIL refuses raises as before) and copied into its region."""
+  from . import ops
+  status = ops.jpeg_decode(payload, *descriptors, jpegs.blocks, jpegs.plane_bytes, jpegs.pixels).cpu()
+  for i in torch.nonzero(status).flatten().tolist():
+    off, h, w = jpegs.rows[i]
+    arr = decode(jpegs.paths[i])
+    if arr.shape != (h, w, 3):
+      raise ValueError('cannot decode %s: PIL reads %s, the header says %dx%d' % (jpegs.paths[i], arr.shape[:2], h, w))
+    payload[off:off + arr.size].copy_(torch.from_numpy(arr.reshape(-1).copy()))
+
+
+def _produce_batch(paths: Sequence[str], batch_size: int, pool: ThreadPoolExecutor):
+  """(tensors, (count, jpegs)) of one batch for Translator.run: PIL decodes the files the device does not."""
+  from . import jpeg, ops
+  blobs = list(pool.map(_read, paths))
+  infos = list(pool.map(_device_jpeg, blobs))
+  host = [i for i, info in enumerate(infos) if info is None]
+  arrays = dict(zip(host, pool.map(decode, [paths[i] for i in host])))
+  shapes = [(info.H, info.W) if info is not None else arrays[i].shape[:2] for i, info in enumerate(infos)]
+  table = np.zeros((batch_size, 3), np.int64)
+  off = 0
+  for i, (h, w) in enumerate(shapes):
+    table[i] = (off, h, w)
+    off += h * w * 3
+  table[len(paths):] = table[len(paths) - 1]
+  payload = np.empty(off, np.uint8)
+  for i, a in arrays.items():
+    payload[table[i, 0]:table[i, 0] + a.size] = a.reshape(-1)
+  payload, table_t = torch.from_numpy(payload), torch.from_numpy(table)
+  ops.check_table(table_t, payload.numel())
+  dev = [i for i, info in enumerate(infos) if info is not None]
+  if not dev:
+    return (payload, table_t), (len(paths), None)
+  b = jpeg.pack([blobs[i] for i in dev], [infos[i] for i in dev], [int(table[i, 0]) for i in dev])
+  tensors = (payload, table_t) + tuple(torch.from_numpy(a) for a in (b.data, b.segs, b.comps, b.images, b.qt, b.huff))
+  rows = [tuple(int(v) for v in table[i]) for i in dev]
+  return tensors, (len(paths), _DeviceJpegs([paths[i] for i in dev], rows, b.blocks, b.plane_bytes, b.pixels))
+
+
 def save(arr: np.ndarray, path: str) -> None:
   """PIL's defaults for the format the extension implies, as scipy.misc.imsave did."""
   from PIL import Image
@@ -100,7 +175,7 @@ def _padded_batches(images: Sequence[np.ndarray], batch_size: int):
     payload, table = ops.pack_images(chunk)
     if len(chunk) < batch_size:
       table = torch.cat([table, table[-1:].expand(batch_size - len(chunk), 3)], 0)
-    yield (payload, table), len(chunk)
+    yield (payload, table), (len(chunk), None)
 
 
 class Translator(object):
@@ -117,23 +192,29 @@ class Translator(object):
     self.depth = depth
 
   def run(self, host_batches):
-    """host_batches: iterable of ((payload, table), count).  Yields the first `count` translated images of each batch."""
+    """host_batches: iterable of (tensors, (count, jpegs)): tensors = (payload, table) host tensors, followed by the six
+    descriptor tensors of a jpeg.Batch when `jpegs` (a _DeviceJpegs) names images the device decodes.  Yields the first
+    `count` translated images of each batch."""
     from . import ops
     from .prefetch import DevicePrefetcher
     counts = collections.deque()
 
     def tensors():
-      for pair, n in host_batches:
-        counts.append(n)
-        yield pair
+      for t, info in host_batches:
+        counts.append(info)
+        yield t
 
     feed = DevicePrefetcher(tensors(), self.model.device, self.depth)
     pending = None
-    for payload, table in feed:
+    for batch in feed:
+      payload, table = batch[0], batch[1]
+      n, jpegs = counts.popleft()
+      if jpegs is not None:
+        _decode_jpegs(payload, batch[2:], jpegs)
       x = ops.images_u8_to_batch(payload, table, self.hw)
       y = ops.batch_to_u8(self.pipe._infer(x))
       feed.release()
-      done = self.back.put(y) + (counts.popleft(),)
+      done = self.back.put(y) + (n,)
       if pending is not None:
         yield self._finish(pending)
       pending = done
@@ -165,7 +246,6 @@ def translate_arrays(model, images: Sequence[np.ndarray], target_domain: str = '
 def translate_files(model, input_paths: Sequence[str], output_paths: Sequence[str], target_domain: str = 't',
                     batch_size: int = 64, num_decode_threads: int = 8, use_graph: bool = True) -> int:
   """Translate input_paths[i] into output_paths[i] (created directories included); returns the number written."""
-  from . import ops
   from .prefetch import HostPrefetcher
   if len(input_paths) != len(output_paths):
     raise ValueError('%d inputs but %d outputs' % (len(input_paths), len(output_paths)))
@@ -179,19 +259,14 @@ def translate_files(model, input_paths: Sequence[str], output_paths: Sequence[st
   writers = ThreadPoolExecutor(num_decode_threads, thread_name_prefix='twg-encode')
 
   def produce(k):
-    paths = input_paths[k * batch_size:(k + 1) * batch_size]
-    payload, table = ops.pack_images(list(decoders.map(decode, paths)))
-    if len(paths) < batch_size:
-      table = torch.cat([table, table[-1:].expand(batch_size - len(paths), 3)], 0)
-    return payload, table, torch.tensor(len(paths))
+    return _produce_batch(input_paths[k * batch_size:(k + 1) * batch_size], batch_size, decoders)
 
   host = HostPrefetcher(produce, capacity=2, num_batches=nb)
   for d in sorted({os.path.dirname(os.path.abspath(p)) for p in output_paths}):
     os.makedirs(d, exist_ok=True)
   written, in_flight = 0, collections.deque()
   try:
-    batches = (((p, t), int(c)) for p, t, c in host)
-    for k, arr in enumerate(Translator(model, target_domain, use_graph).run(batches)):
+    for k, arr in enumerate(Translator(model, target_domain, use_graph).run(host)):
       outs = output_paths[k * batch_size:k * batch_size + len(arr)]
       in_flight.append([writers.submit(save, a, p) for a, p in zip(arr, outs)])
       while len(in_flight) > 2:                 # bound the images waiting to be encoded

@@ -637,7 +637,8 @@ class InferencePipeline(object):
         for _ in range(2):                              # warm-up on the capture stream (lazy one-time set-up, allocator)
           self.model.infer(static_in, self.target_domain)
         graph = torch.cuda.CUDAGraph()
-        graph.capture_begin()
+        # thread-local: the file reader of translate pins host memory on its own thread while a batch is captured
+        graph.capture_begin(capture_error_mode='thread_local')
         static_out = self.model.infer(static_in, self.target_domain)
         graph.capture_end()
       torch.cuda.current_stream(dev).wait_stream(side)
