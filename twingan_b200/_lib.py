@@ -1,4 +1,5 @@
-"""ctypes binding of libtwg.so (the C-ABI declared in include/twg.h, and the JPEG decoder's in include/twgjpeg.h).
+"""ctypes binding of libtwg.so (the C-ABI declared in include/twg.h, the JPEG decoder's in include/twgjpeg.h and the
+JPEG encoder's in include/twgjenc.h).
 
 The prototypes are parsed from the header itself so the Python side can never drift from the ABI.
 There is no CPU fallback: if the library is missing, or a kernel entry point is called without a CUDA
@@ -15,6 +16,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'twg.h')
 JPEG_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'twgjpeg.h')
 JPEG_PREFIX = 'twgjpeg_'
+JENC_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'twgjenc.h')
+JENC_PREFIX = 'twgjenc_'
 LIB_PATH = os.environ.get('TWG_LIB') or os.path.join(_HERE, 'libtwg.so')   # TWG_LIB: A/B builds of the same ABI
 
 _CTYPES = {
@@ -57,7 +60,8 @@ class _Lib:
     self.cdll = ctypes.CDLL(LIB_PATH)
     self.protos = parse_header()
     self.jpeg_protos = parse_header(JPEG_HEADER, JPEG_PREFIX)
-    for name, (ret, args) in list(self.protos.items()) + list(self.jpeg_protos.items()):
+    self.jenc_protos = parse_header(JENC_HEADER, JENC_PREFIX)
+    for name, (ret, args) in list(self.protos.items()) + list(self.jpeg_protos.items()) + list(self.jenc_protos.items()):
       fn = getattr(self.cdll, name)  # raises AttributeError if the symbol is not exported
       fn.restype = _CTYPES[ret]
       fn.argtypes = [_CTYPES[a] for a in args]

@@ -1,5 +1,6 @@
 """Host side of the device JPEG decoder (csrc/twg_jpeg.cu): read a file's headers, decide whether the device decodes it,
-and pack the descriptors of a batch.
+and pack the descriptors of a batch; and of the device JPEG encoder (csrc/twg_jenc.cu): the header PIL writes before
+the scan the device encodes.
 
 A file goes to the device only if libjpeg (as PIL calls it) would decode it through the path the kernels restate:
   * baseline sequential Huffman: SOF0, or SOF1 with 8-bit samples; one scan (Ss 0, Se 63, Ah 0, Al 0) holding every
@@ -322,3 +323,70 @@ def pack(files: Sequence[bytes], infos: Sequence[JpegInfo], payload_offsets: Seq
                i64(comps, COMP_FIELDS), i64(images, IMAGE_FIELDS),
                np.asarray(qts, np.int32).reshape(-1, 64), np.asarray(table_rows, np.int32).reshape(-1, HUFF_WORDS),
                blocks, planes, pixels)
+
+
+# ---- encoding (csrc/twg_jenc.cu): the file PIL writes for Image.fromarray(rgb).save(f, 'JPEG') ----------------------
+#
+# PIL's defaults are libjpeg's: baseline, quality 75, 4:2:0 (Y 2x2, Cb and Cr 1x1), the Annex K Huffman tables without
+# optimisation, no restart markers, a JFIF 1.01 APP0 without units at density 1x1.  Only the frame size varies between
+# files, so the header is assembled here and the device writes the entropy-coded scan that follows it.
+
+# T.81 Annex K.1, tables K.1 and K.2 (natural order): the basis libjpeg's jpeg_set_quality scales
+_STD_LUMA_QT = (16, 11, 10, 16, 24, 40, 51, 61, 12, 12, 14, 19, 26, 58, 60, 55, 14, 13, 16, 24, 40, 57, 69, 56,
+                14, 17, 22, 29, 51, 87, 80, 62, 18, 22, 37, 56, 68, 109, 103, 77, 24, 35, 55, 64, 81, 104, 113, 92,
+                49, 64, 78, 87, 103, 121, 120, 101, 72, 92, 95, 98, 112, 100, 103, 99)
+_STD_CHROMA_QT = (17, 18, 24, 47, 99, 99, 99, 99, 18, 21, 26, 66, 99, 99, 99, 99, 24, 26, 56, 99, 99, 99, 99, 99,
+                  47, 66, 99, 99, 99, 99, 99, 99) + (99,) * 32
+# natural index of the k-th coefficient in zig-zag order
+ZIGZAG = (0, 1, 8, 16, 9, 2, 3, 10, 17, 24, 32, 25, 18, 11, 4, 5, 12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13, 6,
+          7, 14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51, 58, 59, 52, 45, 38, 31,
+          39, 46, 53, 60, 61, 54, 47, 55, 62, 63)
+# T.81 Annex K.3 (tables K.3 - K.6): (BITS[16], HUFFVAL) of DC luma, AC luma, DC chroma, AC chroma
+_AC_LUMA_VALS = bytes.fromhex(
+    '01020300041105122131410613516107227114328191a1082342b1c11552d1f02433627282090a161718191a25262728292a3435363738'
+    '393a434445464748494a535455565758595a636465666768696a737475767778797a838485868788898a92939495969798999aa2a3a4a5'
+    'a6a7a8a9aab2b3b4b5b6b7b8b9bac2c3c4c5c6c7c8c9cad2d3d4d5d6d7d8d9dae1e2e3e4e5e6e7e8e9eaf1f2f3f4f5f6f7f8f9fa')
+_AC_CHROMA_VALS = bytes.fromhex(
+    '000102031104052131061241510761711322328108144291a1b1c109233352f0156272d10a162434e125f11718191a262728292a353637'
+    '38393a434445464748494a535455565758595a636465666768696a737475767778797a82838485868788898a92939495969798999aa2a3'
+    'a4a5a6a7a8a9aab2b3b4b5b6b7b8b9bac2c3c4c5c6c7c8c9cad2d3d4d5d6d7d8d9dae2e3e4e5e6e7e8e9eaf2f3f4f5f6f7f8f9fa')
+STD_HUFF = (
+    (bytes([0, 1, 5, 1, 1, 1, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0]), bytes(range(12))),
+    (bytes([0, 2, 1, 3, 3, 2, 4, 3, 5, 5, 4, 4, 0, 0, 1, 0x7D]), _AC_LUMA_VALS),
+    (bytes([0, 3, 1, 1, 1, 1, 1, 1, 1, 1, 1, 0, 0, 0, 0, 0]), bytes(range(12))),
+    (bytes([0, 2, 1, 2, 4, 4, 3, 4, 7, 5, 4, 4, 0, 1, 2, 0x77]), _AC_CHROMA_VALS),
+)
+ENCODE_QUALITY = 75
+
+
+def encoder_qt(quality: int = ENCODE_QUALITY) -> np.ndarray:
+  """int32 [2, 64] (luma, chroma) in zig-zag order: jcparam.c jpeg_set_quality's scaling of Annex K with baseline
+  limits, (basis * s + 50) // 100 clamped to [1, 255], s = 5000 / q below 50, else 200 - 2 q."""
+  s = 5000 // quality if quality < 50 else 200 - 2 * quality
+  out = np.empty((2, 64), np.int32)
+  for t, basis in enumerate((_STD_LUMA_QT, _STD_CHROMA_QT)):
+    nat = np.clip((np.asarray(basis, np.int64) * s + 50) // 100, 1, 255)
+    out[t] = nat[list(ZIGZAG)]
+  return out
+
+
+def _segment(marker: int, body: bytes) -> bytes:
+  return bytes([0xFF, marker]) + (len(body) + 2).to_bytes(2, 'big') + body
+
+
+def encoder_header(H: int, W: int) -> bytes:
+  """The bytes PIL writes before the scan of an H x W RGB image: SOI, JFIF APP0, DQT luma and chroma, SOF0 (Y 2x2 on
+  table 0, Cb and Cr 1x1 on table 1), DHT DC0 AC0 DC1 AC1, SOS of the three components."""
+  if not (1 <= H <= 65535 and 1 <= W <= 65535):
+    raise ValueError('a JPEG frame is 1..65535 pixels a side (got %dx%d)' % (H, W))
+  qt = encoder_qt()
+  out = [b'\xff\xd8', _segment(0xE0, b'JFIF\x00\x01\x01\x00\x00\x01\x00\x01\x00\x00')]
+  out += [_segment(0xDB, bytes([t]) + bytes(qt[t].astype(np.uint8))) for t in (0, 1)]
+  out.append(_segment(0xC0, bytes([8]) + H.to_bytes(2, 'big') + W.to_bytes(2, 'big')
+                      + bytes([3, 1, 0x22, 0, 2, 0x11, 1, 3, 0x11, 1])))
+  out += [_segment(0xC4, bytes([cls]) + bits + vals) for cls, (bits, vals) in zip((0x00, 0x10, 0x01, 0x11), STD_HUFF)]
+  out.append(_segment(0xDA, bytes([3, 1, 0x00, 2, 0x11, 3, 0x11, 0, 63, 0])))
+  return b''.join(out)
+
+
+EOI = b'\xff\xd9'

@@ -1644,6 +1644,41 @@ def jpeg_decode(payload: torch.Tensor, data: torch.Tensor, segs: torch.Tensor, c
   return status
 
 
+_JENC_QT = {}
+
+
+def jpeg_encode(rgb: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+  """The entropy-coded scans of uint8 [n, h, w, 3] RGB CUDA images, byte for byte what PIL writes between
+  jpeg.encoder_header(h, w) and EOI for Image.fromarray(rgb[i]).save(f, 'JPEG') (twgjenc_dct, twgjenc_bits,
+  twgjenc_pack).  Returns (uint8 device buffer, int64 [n + 1] device offsets) without waiting: image i's scan is
+  buffer[offsets[i]:offsets[i + 1]]."""
+  from . import jpeg
+  if not rgb.is_cuda or rgb.dtype != torch.uint8 or rgb.dim() != 4 or rgb.shape[3] != 3:
+    raise TwgError('jpeg_encode: want a uint8 [n, h, w, 3] CUDA tensor (no CPU fallback), got %s %s %s'
+                   % (rgb.device, rgb.dtype, tuple(rgb.shape)))
+  rgb = rgb.contiguous()
+  n, h, w = (int(s) for s in rgb.shape[:3])
+  dev = rgb.device
+  if dev not in _JENC_QT:
+    _JENC_QT[dev] = torch.from_numpy(jpeg.encoder_qt()).to(dev)
+  qt = _JENC_QT[dev]
+  L = lib()
+  ws, cap = L.cdll.twgjenc_workspace_bytes(n, h, w), L.cdll.twgjenc_scan_capacity(n, h, w)
+  if ws < 0 or cap < 0:
+    raise TwgError('jpeg_encode: %s' % L.last_error())
+  blocks = 6 * ((h + 15) // 16) * ((w + 15) // 16)
+  coefs = torch.empty(n * blocks * 64, device=dev, dtype=torch.int16)
+  bitpos = torch.empty(n * (blocks + 1), device=dev, dtype=torch.int32)
+  work = torch.empty(ws, device=dev, dtype=torch.uint8)
+  out = torch.empty(cap, device=dev, dtype=torch.uint8)
+  offsets = torch.empty(n + 1, device=dev, dtype=torch.int64)
+  L.call('twgjenc_dct', rgb.data_ptr(), n, h, w, qt.data_ptr(), coefs.data_ptr(), _st())
+  L.call('twgjenc_bits', coefs.data_ptr(), n, h, w, bitpos.data_ptr(), _st())
+  L.call('twgjenc_pack', coefs.data_ptr(), bitpos.data_ptr(), n, h, w, work.data_ptr(), out.data_ptr(),
+         offsets.data_ptr(), _st())
+  return out, offsets
+
+
 def batch_to_u8(x: torch.Tensor) -> torch.Tensor:
   """uint8 image of the model output, clip(x * 255, 0, 255) truncated (util_io.imsave; twg_batch_to_u8)."""
   x = _check(x)

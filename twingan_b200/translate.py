@@ -4,8 +4,8 @@ inference/image_translation_infer.py (docs/infer_and_eval.md), with its flag nam
   python -m twingan_b200.translate --model_path=<train_dir>/256 --image_hw=256 \\
       --input_image_path=<file or directory> --output_image_path=<file or directory>
 
-Encoding runs on the host (PIL, as util_io.imsave); decoding runs on the device for baseline JPEG files and on the host
-(PIL, as util_io.imread) for every other file; everything between runs on the device.  Per batch:
+JPEG files are decoded and encoded on the device, byte for byte as PIL does; PIL decodes every other input (as
+util_io.imread) and encodes every other output (as util_io.imsave); everything between runs on the device.  Per batch:
   * a background thread reads the files of batch k+1 on a pool of `--num_decode_threads` threads.  A JPEG that
     twingan_b200/jpeg.py accepts (baseline Huffman, grey or YCbCr, 4:4:4 / 4:2:2 / 4:2:0) travels compressed, with its
     descriptors; PIL decodes every other file into its region of one uint8 payload + a table of {offset, H, W}
@@ -17,7 +17,11 @@ Encoding runs on the host (PIL, as util_io.imsave); decoding runs on the device 
   * one kernel converts and resizes the ragged batch to the model input (ops.images_u8_to_batch: convert_image_dtype +
     TF-1 bilinear resize_images), the model translates it (InferencePipeline._infer: a CUDA graph per batch shape), one
     kernel quantises the result (ops.batch_to_u8: util_io.imsave's clip(x * 255).astype(uint8));
-  * the uint8 images come back on a side stream (HostReturner) and are encoded and written on a thread pool.
+  * the outputs PIL would save as JPEG (their extension maps to 'JPEG' in Image.registered_extensions()) are encoded on
+    the device (ops.jpeg_encode: the entropy-coded scans packed back to back, jpeg.py writes the header PIL writes);
+    their offsets come back on a side stream; a batch later, when the host waits for that batch anyway, exactly their
+    bytes follow on a stream that holds nothing of the batch computing meanwhile (ScanReturner).  A batch with any other
+    output returns its uint8 images (HostReturner) for PIL to encode.  A thread pool writes the files.
 A short last batch is padded with repeats of its last image, so one graph serves the whole run; the padded outputs are
 dropped.  The outputs are image_hw x image_hw: like the reference, nothing resizes them back to the input's size.
 """
@@ -167,6 +171,81 @@ def save(arr: np.ndarray, path: str) -> None:
   Image.fromarray(arr).save(path)
 
 
+def saves_as_jpeg(path: str) -> bool:
+  """Whether `save` writes this path as a JPEG file: PIL picks the format from the lower-cased extension."""
+  from PIL import Image
+  return Image.registered_extensions().get(os.path.splitext(path)[1].lower()) == 'JPEG'
+
+
+def _write(data: bytes, path: str) -> None:
+  with open(path, 'wb') as f:
+    f.write(data)
+
+
+class ScanReturner(object):
+  """The JPEG scans of ops.jpeg_encode device -> host, only the bytes of the rows asked for.  `put` enqueues the copy of
+  the offsets on a side stream behind the main stream's work.  `fetch` waits for that copy, which already implies the
+  batch's encode is done, then copies the rows' bytes on a second stream that holds nothing else, so the host waits for
+  that batch alone and not for the batch queued after it.  Pinned buffers are reused, growing only when a batch needs
+  more."""
+
+  def __init__(self, device, depth: int = 2):
+    self.device = torch.device(device)
+    self.depth = max(2, int(depth))
+    self._stream = torch.cuda.Stream(device=self.device)
+    self._copy = torch.cuda.Stream(device=self.device)
+    self._offsets = [None] * self.depth
+    self._bytes = None
+    self._n = 0
+    self.d2h_bytes = 0
+
+  def put(self, scans: torch.Tensor, offsets: torch.Tensor):
+    slot = self._n % self.depth                # fetch runs in order and is synchronous: the slot's last use is over
+    self._n += 1
+    k = int(offsets.numel())
+    if self._offsets[slot] is None or self._offsets[slot].numel() < k:
+      self._offsets[slot] = torch.empty(k, dtype=torch.int64).pin_memory()
+    ready = torch.cuda.Event()
+    ready.record(torch.cuda.current_stream(self.device))
+    with torch.cuda.stream(self._stream):
+      self._stream.wait_event(ready)
+      self._offsets[slot][:k].copy_(offsets, non_blocking=True)
+      ev = torch.cuda.Event()
+      ev.record(self._stream)
+    self.d2h_bytes += k * 8
+    return slot, k, scans, offsets, ev
+
+  def fetch(self, handle, rows: Sequence[int]) -> List[bytes]:
+    """The scans of `rows` (ascending) of a batch `put` returned `handle` for."""
+    slot, k, scans, _, ev = handle
+    ev.synchronize()
+    off = self._offsets[slot][:k].numpy().copy()
+    runs = []                                  # [first row, last row] of each run of consecutive rows
+    for r in rows:
+      if runs and runs[-1][1] == r - 1:
+        runs[-1][1] = r
+      else:
+        runs.append([r, r])
+    total = int(sum(off[b + 1] - off[a] for a, b in runs))
+    if self._bytes is None or self._bytes.numel() < total:
+      size = max(total, 2 * (self._bytes.numel() if self._bytes is not None else 0))
+      self._bytes = torch.empty(size, dtype=torch.uint8).pin_memory()
+    at, where = 0, {}
+    with torch.cuda.stream(self._copy):        # the batch's encode is done: nothing to wait for on the device
+      for a, b in runs:
+        m = int(off[b + 1] - off[a])
+        self._bytes[at:at + m].copy_(scans[int(off[a]):int(off[b + 1])], non_blocking=True)
+        for r in range(a, b + 1):
+          where[r] = at + int(off[r] - off[a])
+        at += m
+      done = torch.cuda.Event()
+      done.record(self._copy)
+    done.synchronize()
+    self.d2h_bytes += total
+    data = self._bytes[:total].numpy()
+    return [data[where[r]:where[r] + int(off[r + 1] - off[r])].tobytes() for r in rows]
+
+
 def _padded_batches(images: Sequence[np.ndarray], batch_size: int):
   """(payload, table) of consecutive batches; the last one padded to batch_size rows with its last row."""
   from . import ops
@@ -189,12 +268,15 @@ class Translator(object):
     self.hw = int(model.flags.train_image_size)
     self.pipe = twingan.InferencePipeline(model, depth, use_graph=use_graph, target_domain=target_domain)
     self.back = HostReturner(model.device, depth)
+    self.scans = ScanReturner(model.device, depth) if self.back.cuda else None
     self.depth = depth
 
-  def run(self, host_batches):
+  def run(self, host_batches, jpeg_rows=None):
     """host_batches: iterable of (tensors, (count, jpegs)): tensors = (payload, table) host tensors, followed by the six
     descriptor tensors of a jpeg.Batch when `jpegs` (a _DeviceJpegs) names images the device decodes.  Yields the first
-    `count` translated images of each batch."""
+    `count` translated images of each batch.  With `jpeg_rows` (per batch, `count` booleans), yields (images or None,
+    {row: JPEG scan bytes}) instead: the marked rows are encoded on the device, and the images come back only when
+    some row is not marked."""
     from . import ops
     from .prefetch import DevicePrefetcher
     counts = collections.deque()
@@ -206,7 +288,7 @@ class Translator(object):
 
     feed = DevicePrefetcher(tensors(), self.model.device, self.depth)
     pending = None
-    for batch in feed:
+    for k, batch in enumerate(feed):
       payload, table = batch[0], batch[1]
       n, jpegs = counts.popleft()
       if jpegs is not None:
@@ -214,19 +296,28 @@ class Translator(object):
       x = ops.images_u8_to_batch(payload, table, self.hw)
       y = ops.batch_to_u8(self.pipe._infer(x))
       feed.release()
-      done = self.back.put(y) + (n,)
+      rows = None if jpeg_rows is None else [i for i, j in enumerate(jpeg_rows[k]) if j]
+      scans = None
+      if rows:                                  # every row is encoded; only the marked rows' bytes come back
+        scans = self.scans.put(*ops.jpeg_encode(y[:n])), rows
+      raw = self.back.put(y) if rows is None or len(rows) < n else None
       if pending is not None:
         yield self._finish(pending)
-      pending = done
+      pending = (raw, scans, n, jpeg_rows is not None)
     if pending is not None:
       yield self._finish(pending)
 
-  @staticmethod
-  def _finish(pending):
-    out, ev, n = pending
-    if ev is not None:
-      ev.synchronize()
-    return out[:n].numpy().copy()             # the pinned slot is reused two batches later
+  def _finish(self, pending):
+    raw, scans, n, files = pending
+    arrays = None
+    if raw is not None:
+      out, ev = raw
+      if ev is not None:
+        ev.synchronize()
+      arrays = out[:n].numpy().copy()           # the pinned slot is reused two batches later
+    if not files:
+      return arrays
+    return arrays, (dict(zip(scans[1], self.scans.fetch(*scans))) if scans is not None else {})
 
 
 def translate_arrays(model, images: Sequence[np.ndarray], target_domain: str = 't', batch_size: int = 64,
@@ -246,6 +337,7 @@ def translate_arrays(model, images: Sequence[np.ndarray], target_domain: str = '
 def translate_files(model, input_paths: Sequence[str], output_paths: Sequence[str], target_domain: str = 't',
                     batch_size: int = 64, num_decode_threads: int = 8, use_graph: bool = True) -> int:
   """Translate input_paths[i] into output_paths[i] (created directories included); returns the number written."""
+  from . import jpeg
   from .prefetch import HostPrefetcher
   if len(input_paths) != len(output_paths):
     raise ValueError('%d inputs but %d outputs' % (len(input_paths), len(output_paths)))
@@ -256,7 +348,7 @@ def translate_files(model, input_paths: Sequence[str], output_paths: Sequence[st
     return 0
   nb = (n + batch_size - 1) // batch_size
   decoders = ThreadPoolExecutor(num_decode_threads, thread_name_prefix='twg-decode')
-  writers = ThreadPoolExecutor(num_decode_threads, thread_name_prefix='twg-encode')
+  writers = ThreadPoolExecutor(num_decode_threads, thread_name_prefix='twg-encode')   # PIL encodes non-JPEG outputs
 
   def produce(k):
     return _produce_batch(input_paths[k * batch_size:(k + 1) * batch_size], batch_size, decoders)
@@ -265,10 +357,15 @@ def translate_files(model, input_paths: Sequence[str], output_paths: Sequence[st
   for d in sorted({os.path.dirname(os.path.abspath(p)) for p in output_paths}):
     os.makedirs(d, exist_ok=True)
   written, in_flight = 0, collections.deque()
+  as_jpeg = [saves_as_jpeg(p) for p in output_paths]
+  jpeg_rows = [as_jpeg[k * batch_size:(k + 1) * batch_size] for k in range(nb)]
   try:
-    for k, arr in enumerate(Translator(model, target_domain, use_graph).run(host)):
-      outs = output_paths[k * batch_size:k * batch_size + len(arr)]
-      in_flight.append([writers.submit(save, a, p) for a, p in zip(arr, outs)])
+    translator = Translator(model, target_domain, use_graph)
+    header = jpeg.encoder_header(translator.hw, translator.hw) if any(as_jpeg) else b''
+    for k, (arr, scans) in enumerate(translator.run(host, jpeg_rows)):
+      outs = output_paths[k * batch_size:(k + 1) * batch_size]
+      in_flight.append([writers.submit(_write, header + scans[i] + jpeg.EOI, p) if i in scans else
+                        writers.submit(save, arr[i], p) for i, p in enumerate(outs)])
       while len(in_flight) > 2:                 # bound the images waiting to be encoded
         for f in in_flight.popleft():
           f.result()
