@@ -1,5 +1,5 @@
-"""ctypes binding of libtwg.so (the C-ABI declared in include/twg.h, the JPEG decoder's in include/twgjpeg.h and the
-JPEG encoder's in include/twgjenc.h).
+"""ctypes binding of libtwg.so (the C-ABI declared in include/twg.h, the JPEG decoder's in include/twgjpeg.h, the
+JPEG encoder's in include/twgjenc.h and the PNG decoder's in include/twgpng.h).
 
 The prototypes are parsed from the header itself so the Python side can never drift from the ABI.
 There is no CPU fallback: if the library is missing, or a kernel entry point is called without a CUDA
@@ -18,6 +18,8 @@ JPEG_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'twgjpeg.h')
 JPEG_PREFIX = 'twgjpeg_'
 JENC_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'twgjenc.h')
 JENC_PREFIX = 'twgjenc_'
+PNG_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'twgpng.h')
+PNG_PREFIX = 'twgpng_'
 LIB_PATH = os.environ.get('TWG_LIB') or os.path.join(_HERE, 'libtwg.so')   # TWG_LIB: A/B builds of the same ABI
 
 _CTYPES = {
@@ -61,7 +63,9 @@ class _Lib:
     self.protos = parse_header()
     self.jpeg_protos = parse_header(JPEG_HEADER, JPEG_PREFIX)
     self.jenc_protos = parse_header(JENC_HEADER, JENC_PREFIX)
-    for name, (ret, args) in list(self.protos.items()) + list(self.jpeg_protos.items()) + list(self.jenc_protos.items()):
+    self.png_protos = parse_header(PNG_HEADER, PNG_PREFIX)
+    for name, (ret, args) in (list(self.protos.items()) + list(self.jpeg_protos.items()) + list(self.jenc_protos.items())
+                              + list(self.png_protos.items())):
       fn = getattr(self.cdll, name)  # raises AttributeError if the symbol is not exported
       fn.restype = _CTYPES[ret]
       fn.argtypes = [_CTYPES[a] for a in args]

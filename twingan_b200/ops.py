@@ -1644,6 +1644,39 @@ def jpeg_decode(payload: torch.Tensor, data: torch.Tensor, segs: torch.Tensor, c
   return status
 
 
+PNG_STAGES = ('twgpng_inflate', 'twgpng_unfilter', 'twgpng_rgb')
+
+
+def png_decode(payload: torch.Tensor, data: torch.Tensor, images: torch.Tensor, palettes: torch.Tensor, raw_bytes: int,
+               pixels: int, stage_hook=None) -> torch.Tensor:
+  """Decode the PNG streams of one batch into their regions of a uint8 CUDA payload (twgpng_inflate, twgpng_unfilter,
+  twgpng_rgb): the descriptors are a png.Batch on the device, `raw_bytes` and `pixels` its host sizes.  Returns the
+  int32 [images] device status without waiting for it: 0 for an image decoded exactly (PIL's pixels), else the TWG_PNG_*
+  bits of what made the device stop (png.STATUS_*); such an image's region is undefined.  The inflated scratch comes
+  from the caching allocator on the current stream, so calls on several streams may run at once and, after warm-up,
+  none reaches cudaMalloc.  `stage_hook(name)`, when given, is called after each stage is enqueued (timing)."""
+  if not payload.is_cuda or payload.dtype != torch.uint8:
+    raise TwgError('png_decode: payload must be a uint8 CUDA tensor (no CPU fallback)')
+  dev = payload.device
+  n = int(images.shape[0])
+  if data.numel() < 1 or raw_bytes < 1:
+    raise ValueError('png_decode: an empty stream or image (png.parse declines them)')
+  raw = torch.empty(raw_bytes, device=dev, dtype=torch.uint8)
+  status = torch.empty(n, device=dev, dtype=torch.int32)
+  L = lib()
+  L.call('twgpng_inflate', data.data_ptr(), images.data_ptr(), n, raw.data_ptr(), status.data_ptr(), _st())
+  if stage_hook:
+    stage_hook(PNG_STAGES[0])
+  L.call('twgpng_unfilter', raw.data_ptr(), images.data_ptr(), n, status.data_ptr(), _st())
+  if stage_hook:
+    stage_hook(PNG_STAGES[1])
+  L.call('twgpng_rgb', raw.data_ptr(), images.data_ptr(), n, palettes.data_ptr(), pixels, status.data_ptr(),
+         payload.data_ptr(), _st())
+  if stage_hook:
+    stage_hook(PNG_STAGES[2])
+  return status
+
+
 _JENC_QT = {}
 
 

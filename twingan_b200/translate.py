@@ -4,16 +4,21 @@ inference/image_translation_infer.py (docs/infer_and_eval.md), with its flag nam
   python -m twingan_b200.translate --model_path=<train_dir>/256 --image_hw=256 \\
       --input_image_path=<file or directory> --output_image_path=<file or directory>
 
-JPEG files are decoded and encoded on the device, byte for byte as PIL does; PIL decodes every other input (as
-util_io.imread) and encodes every other output (as util_io.imsave); everything between runs on the device.  Per batch:
+JPEG and PNG files are decoded on the device, pixel for pixel as PIL decodes them, and JPEG outputs are encoded there,
+byte for byte as PIL does; PIL decodes every other input (as util_io.imread) and encodes every other output (as
+util_io.imsave); everything between runs on the device.  Per batch:
   * a background thread reads the files of batch k+1 on a pool of `--num_decode_threads` threads.  A JPEG that
-    twingan_b200/jpeg.py accepts (baseline Huffman, grey or YCbCr, 4:4:4 / 4:2:2 / 4:2:0) travels compressed, with its
-    descriptors; PIL decodes every other file into its region of one uint8 payload + a table of {offset, H, W}
-    (HostPrefetcher, pinned memory; the JPEG headers give their rows before any decoding) while batch k computes;
-  * the payload, table and compressed scans are copied to the device on a side stream (DevicePrefetcher);
-  * three kernels decode the JPEG scans into their regions of the payload, bit for bit as PIL does (ops.jpeg_decode);
-    the batch's status is read once, and an image the device could not decode exactly is decoded by PIL and written
-    into its region instead (a file PIL refuses fails as before);
+    twingan_b200/jpeg.py accepts (baseline Huffman, grey or YCbCr, 4:4:4 / 4:2:2 / 4:2:0) or a PNG that
+    twingan_b200/png.py accepts (not interlaced, not animated, no palette transparency, known chunks, every CRC right)
+    travels compressed, with its descriptors; PIL decodes every other file into its region of one uint8 payload + a
+    table of {offset, H, W} (HostPrefetcher, pinned memory; the headers give the device files' rows before any
+    decoding) while batch k computes;
+  * the payload, table and compressed data are copied to the device on a side stream (DevicePrefetcher);
+  * three kernels decode the JPEG scans (ops.jpeg_decode) and three the PNG streams (ops.png_decode) into their regions
+    of a copy of the payload, on a stream of the batch's own, up to Translator.DECODE_AHEAD batches ahead of the one
+    translated (_DeviceDecoder: the decoders are serial within a file, so batches decode side by side); the batch's
+    status is read once, when it is translated, and an image the device could not decode exactly is decoded by PIL and
+    written into its region instead (a file PIL refuses fails as before);
   * one kernel converts and resizes the ragged batch to the model input (ops.images_u8_to_batch: convert_image_dtype +
     TF-1 bilinear resize_images), the model translates it (InferencePipeline._infer: a CUDA graph per batch shape), one
     kernel quantises the result (ops.batch_to_u8: util_io.imsave's clip(x * 255).astype(uint8));
@@ -96,12 +101,12 @@ def decode(path: str) -> np.ndarray:
     raise ValueError('cannot decode %s: %s' % (path, e)) from e
 
 
-class _DeviceJpegs(object):
-  """The JPEG files of a batch the device decodes: their paths, their table rows {offset, H, W}, and the host sizes of
-  their jpeg.Batch.  (Not a tuple: the prefetcher maps over tuples.)"""
+class _DeviceFiles(object):
+  """The files of a batch one device decoder decodes: their paths, their table rows {offset, H, W}, and the host sizes
+  its ops call takes after the descriptor tensors.  (Not a tuple: the prefetcher maps over tuples.)"""
 
-  def __init__(self, paths, rows, blocks, plane_bytes, pixels):
-    self.paths, self.rows, self.blocks, self.plane_bytes, self.pixels = paths, rows, blocks, plane_bytes, pixels
+  def __init__(self, paths, rows, sizes):
+    self.paths, self.rows, self.sizes = paths, rows, sizes
 
 
 def _read(path: str) -> Optional[bytes]:
@@ -124,27 +129,104 @@ def _device_jpeg(data: Optional[bytes]):
   return info
 
 
-def _decode_jpegs(payload: torch.Tensor, descriptors, jpegs: '_DeviceJpegs') -> None:
-  """Decode a batch's JPEG files into their regions of the device payload; an image the device flags is decoded by PIL
-  (decode(), so a file PIL refuses raises as before) and copied into its region."""
-  from . import ops
-  status = ops.jpeg_decode(payload, *descriptors, jpegs.blocks, jpegs.plane_bytes, jpegs.pixels).cpu()
+def _device_png(data: Optional[bytes]):
+  """png.PngInfo when the device decodes this file, else None; as _device_jpeg, above PIL's decompression-bomb limit
+  PIL decides."""
+  from PIL import Image
+  from . import png
+  info = png.probe(data) if data and data[:8] == png.SIGNATURE else None
+  if info is not None and Image.MAX_IMAGE_PIXELS and info.H * info.W > Image.MAX_IMAGE_PIXELS:
+    return None
+  return info
+
+
+def _device_file(data: Optional[bytes]):
+  """('jpeg' or 'png', its info) when the device decodes this file, else None."""
+  info = _device_jpeg(data)
+  if info is not None:
+    return 'jpeg', info
+  info = _device_png(data)
+  return ('png', info) if info is not None else None
+
+
+def _redecode(payload: torch.Tensor, status: torch.Tensor, files: '_DeviceFiles') -> None:
+  """PIL decodes (decode(), so a file PIL refuses raises as before) each image whose status is not 0 into its region of
+  the device payload."""
   for i in torch.nonzero(status).flatten().tolist():
-    off, h, w = jpegs.rows[i]
-    arr = decode(jpegs.paths[i])
+    off, h, w = files.rows[i]
+    arr = decode(files.paths[i])
     if arr.shape != (h, w, 3):
-      raise ValueError('cannot decode %s: PIL reads %s, the header says %dx%d' % (jpegs.paths[i], arr.shape[:2], h, w))
+      raise ValueError('cannot decode %s: PIL reads %s, the header says %dx%d' % (files.paths[i], arr.shape[:2], h, w))
     payload[off:off + arr.size].copy_(torch.from_numpy(arr.reshape(-1).copy()))
 
 
+class _DeviceDecoder(object):
+  """Decodes batches' JPEG and PNG files on the device with `ahead` batches in flight behind the one being translated.
+
+  Entropy decoding and inflate are serial within a file (a thread or a warp each), so one batch keeps a few SMs busy
+  for as long as its largest file takes.  Each batch therefore decodes on a stream of its own, concurrently with the
+  batches around it and with the model, and the host reads its status only when the batch is translated.  `start`
+  copies the batch out of the prefetcher's staging slot (on the main stream, so the slot can be refilled at once) and
+  enqueues the decoders on that batch's stream; `finish` waits for the status, lets PIL decode the images the device
+  flagged, and orders the main stream after the decoding."""
+
+  def __init__(self, device, ahead: int):
+    self.device = torch.device(device)
+    self.streams = [torch.cuda.Stream(device=self.device) for _ in range(ahead + 1)]
+    self._n = 0
+
+  def start(self, payload: torch.Tensor, table: torch.Tensor, descriptors, jpegs: Optional['_DeviceFiles'],
+            pngs: Optional['_DeviceFiles']):
+    """(payload, table, handle) of a batch (the six tensors of a jpeg.Batch, then the three of a png.Batch, each present
+    when its files are), the first two copies owned by the caller from now on."""
+    from . import ops
+    payload, table = payload.clone(), table.clone()
+    descriptors = [d.clone() for d in descriptors]
+    copied = torch.cuda.Event()
+    copied.record(torch.cuda.current_stream(self.device))
+    stream = self.streams[self._n % len(self.streams)]   # its last batch was finished before this one started
+    self._n += 1
+    if jpegs is None and pngs is None:
+      return payload, table, None
+    stream.wait_event(copied)
+    for t in [payload] + descriptors:
+      t.record_stream(stream)
+    with torch.cuda.stream(stream):
+      status = []
+      if jpegs is not None:
+        status.append(ops.jpeg_decode(payload, *descriptors[:6], *jpegs.sizes))
+        descriptors = descriptors[6:]
+      if pngs is not None:
+        status.append(ops.png_decode(payload, *descriptors[:3], *pngs.sizes))
+      status = torch.cat(status) if len(status) > 1 else status[0]
+      host = torch.empty(status.numel(), dtype=torch.int32).pin_memory()
+      host.copy_(status, non_blocking=True)
+      done = torch.cuda.Event()
+      done.record(stream)
+    return payload, table, (host, done, jpegs, pngs)
+
+  def finish(self, payload: torch.Tensor, handle) -> None:
+    if handle is None:
+      return
+    host, done, jpegs, pngs = handle
+    done.synchronize()
+    torch.cuda.current_stream(self.device).wait_event(done)
+    status = host.clone()
+    nj = len(jpegs.paths) if jpegs is not None else 0
+    if jpegs is not None:
+      _redecode(payload, status[:nj], jpegs)
+    if pngs is not None:
+      _redecode(payload, status[nj:], pngs)
+
+
 def _produce_batch(paths: Sequence[str], batch_size: int, pool: ThreadPoolExecutor):
-  """(tensors, (count, jpegs)) of one batch for Translator.run: PIL decodes the files the device does not."""
-  from . import jpeg, ops
+  """(tensors, (count, jpegs, pngs)) of one batch for Translator.run: PIL decodes the files the device does not."""
+  from . import jpeg, ops, png
   blobs = list(pool.map(_read, paths))
-  infos = list(pool.map(_device_jpeg, blobs))
-  host = [i for i, info in enumerate(infos) if info is None]
+  kinds = list(pool.map(_device_file, blobs))
+  host = [i for i, k in enumerate(kinds) if k is None]
   arrays = dict(zip(host, pool.map(decode, [paths[i] for i in host])))
-  shapes = [(info.H, info.W) if info is not None else arrays[i].shape[:2] for i, info in enumerate(infos)]
+  shapes = [(k[1].H, k[1].W) if k is not None else arrays[i].shape[:2] for i, k in enumerate(kinds)]
   table = np.zeros((batch_size, 3), np.int64)
   off = 0
   for i, (h, w) in enumerate(shapes):
@@ -156,13 +238,23 @@ def _produce_batch(paths: Sequence[str], batch_size: int, pool: ThreadPoolExecut
     payload[table[i, 0]:table[i, 0] + a.size] = a.reshape(-1)
   payload, table_t = torch.from_numpy(payload), torch.from_numpy(table)
   ops.check_table(table_t, payload.numel())
-  dev = [i for i, info in enumerate(infos) if info is not None]
-  if not dev:
-    return (payload, table_t), (len(paths), None)
-  b = jpeg.pack([blobs[i] for i in dev], [infos[i] for i in dev], [int(table[i, 0]) for i in dev])
-  tensors = (payload, table_t) + tuple(torch.from_numpy(a) for a in (b.data, b.segs, b.comps, b.images, b.qt, b.huff))
-  rows = [tuple(int(v) for v in table[i]) for i in dev]
-  return tensors, (len(paths), _DeviceJpegs([paths[i] for i in dev], rows, b.blocks, b.plane_bytes, b.pixels))
+  tensors, files = (payload, table_t), []
+  for kind in ('jpeg', 'png'):
+    dev = [i for i, k in enumerate(kinds) if k is not None and k[0] == kind]
+    if not dev:
+      files.append(None)
+      continue
+    args = [blobs[i] for i in dev], [kinds[i][1] for i in dev], [int(table[i, 0]) for i in dev]
+    if kind == 'jpeg':
+      b = jpeg.pack(*args)
+      tensors += tuple(torch.from_numpy(a) for a in (b.data, b.segs, b.comps, b.images, b.qt, b.huff))
+      sizes = (b.blocks, b.plane_bytes, b.pixels)
+    else:
+      b = png.pack(*args)
+      tensors += tuple(torch.from_numpy(a) for a in (b.data, b.images, b.palettes))
+      sizes = (b.raw_bytes, b.pixels)
+    files.append(_DeviceFiles([paths[i] for i in dev], [tuple(int(v) for v in table[i]) for i in dev], sizes))
+  return tensors, (len(paths),) + tuple(files)
 
 
 def save(arr: np.ndarray, path: str) -> None:
@@ -254,12 +346,16 @@ def _padded_batches(images: Sequence[np.ndarray], batch_size: int):
     payload, table = ops.pack_images(chunk)
     if len(chunk) < batch_size:
       table = torch.cat([table, table[-1:].expand(batch_size - len(chunk), 3)], 0)
-    yield (payload, table), (len(chunk), None)
+    yield (payload, table), (len(chunk), None, None)
 
 
 class Translator(object):
   """The device path of a run: payload/table batches in, uint8 [n, hw, hw, 3] host arrays out, in order.  The staging
   buffers, result slots and CUDA graphs persist across `run` calls."""
+
+  # batches whose device decoding runs behind the one being translated: enough that the serial decoders of several
+  # batches share the GPU (tools/png_decode_bench.py)
+  DECODE_AHEAD = 3
 
   def __init__(self, model, target_domain: str = 't', use_graph: bool = True, depth: int = 2):
     from . import twingan
@@ -270,13 +366,16 @@ class Translator(object):
     self.back = HostReturner(model.device, depth)
     self.scans = ScanReturner(model.device, depth) if self.back.cuda else None
     self.depth = depth
+    self.decoder = _DeviceDecoder(model.device, self.DECODE_AHEAD) if self.back.cuda else None
 
   def run(self, host_batches, jpeg_rows=None):
-    """host_batches: iterable of (tensors, (count, jpegs)): tensors = (payload, table) host tensors, followed by the six
-    descriptor tensors of a jpeg.Batch when `jpegs` (a _DeviceJpegs) names images the device decodes.  Yields the first
+    """host_batches: iterable of (tensors, (count, jpegs, pngs)): tensors = (payload, table) host tensors, followed by
+    the six descriptor tensors of a jpeg.Batch when `jpegs` (a _DeviceFiles) names JPEG images the device decodes, then
+    the three of a png.Batch when `pngs` names PNG images.  Yields the first
     `count` translated images of each batch.  With `jpeg_rows` (per batch, `count` booleans), yields (images or None,
     {row: JPEG scan bytes}) instead: the marked rows are encoded on the device, and the images come back only when
-    some row is not marked."""
+    some row is not marked.  From the first batch with files the device decodes, the batches go through the decoder
+    in order, up to DECODE_AHEAD of them decoding behind the one translated."""
     from . import ops
     from .prefetch import DevicePrefetcher
     counts = collections.deque()
@@ -287,15 +386,33 @@ class Translator(object):
         yield t
 
     feed = DevicePrefetcher(tensors(), self.model.device, self.depth)
+    decoding = collections.deque()               # (k, n, payload, table, handle) in order
+
+    def ready():
+      """(k, n, payload, table, staged): the batches in order, each once its images are in its payload; `staged`: the
+      payload is the prefetcher's slot, to be released once the batch has been enqueued."""
+      for k, batch in enumerate(feed):
+        n, jpegs, pngs = counts.popleft()
+        if jpegs is None and pngs is None and not decoding:
+          yield k, n, batch[0], batch[1], True
+          continue
+        decoding.append((k, n) + self.decoder.start(batch[0], batch[1], batch[2:], jpegs, pngs))
+        feed.release()                           # start copied the batch out of its slot
+        while len(decoding) > self.DECODE_AHEAD:
+          k0, n0, payload, table, handle = decoding.popleft()
+          self.decoder.finish(payload, handle)
+          yield k0, n0, payload, table, False
+      while decoding:
+        k0, n0, payload, table, handle = decoding.popleft()
+        self.decoder.finish(payload, handle)
+        yield k0, n0, payload, table, False
+
     pending = None
-    for k, batch in enumerate(feed):
-      payload, table = batch[0], batch[1]
-      n, jpegs = counts.popleft()
-      if jpegs is not None:
-        _decode_jpegs(payload, batch[2:], jpegs)
+    for k, n, payload, table, staged in ready():
       x = ops.images_u8_to_batch(payload, table, self.hw)
       y = ops.batch_to_u8(self.pipe._infer(x))
-      feed.release()
+      if staged:
+        feed.release()
       rows = None if jpeg_rows is None else [i for i, j in enumerate(jpeg_rows[k]) if j]
       scans = None
       if rows:                                  # every row is encoded; only the marked rows' bytes come back
