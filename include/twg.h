@@ -51,6 +51,21 @@ int twg_version(void);
 const char* twg_last_error(void);
 /* number of kernels launched by this library in the calling process since load (for bench gpu_launches) */
 int64_t twg_launch_count(void);
+/* The partial-sum scratch of the deterministic cross-block reductions: twg_partials_regions() fixed, disjoint regions of
+ * twg_partials_region_floats() floats each, on every device.  Region 0 serves every stream not bound to a region;
+ * twg_partials_bind gives one non-default stream a region 1.. of its own on the CURRENT device (bind with the stream's
+ * device current), so that two streams can run the reductions at once (the discriminator domains of the training step);
+ * region 0 gives the stream's region back.  Binding fails (TWG_ERR_INVALID) when the region belongs to another stream
+ * of that device or the stream already owns another region; binding a stream to its own region again is a no-op.
+ * twg_partials_region: the region a launch on that stream of the current device gets; twg_partials_region_uses: how
+ * many reductions each region has served in this process (all devices), -1 for a region that does not exist.
+ * stream_key is the cudaStream_t handle, compared and never launched on (these are host-only entries).  Call bind
+ * while no work that uses the regions is in flight. */
+int twg_partials_regions(void);
+int64_t twg_partials_region_floats(void);
+int twg_partials_region(const void* stream_key);
+int64_t twg_partials_region_uses(int region);
+int twg_partials_bind(const void* stream_key, int region);
 
 /* ---- convolution: replaces tf.contrib.layers.conv2d (nets/pggan_utils.py:316-320) and its
  *      tf.gradients-generated Conv2DBackpropInput / Conv2DBackpropFilter -------------------------------

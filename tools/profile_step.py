@@ -10,6 +10,13 @@ Prints and writes to DIR:
   * convs.json / the second table: every tensor-core conv launch of the step (entry point and geometry, recorded where
     twingan_b200.ops calls the library) matched to its kernel in the trace, with its time, FLOPs, algorithmic HBM bytes and
     the modelled L2 -> shared-memory operand bytes of the per-tap and the column-box kernels (conv_traffic);
+  * fill.json / the third table: how much of the GPU each launch fills (its grid against one wave, 132 SMs times the CTAs
+    one SM holds at the launch's registers, shared memory and block size), summed over the discriminator chains, which
+    run one domain after the other on one stream: D_s / D_t ('Ds', 'Dt') and their DRAGAN penalty chains ('DRs', 'DRt'),
+    forward and both backward passes (a backward node carries the chain of the forward call that made it).  For each
+    chain: the time of the launches below one wave, the time of the last partial wave of the others, the idle share of
+    the GPU over the chain's launches, and the upper bound of what running the two domains' chains side by side could
+    save (launch i of D_s beside launch i of D_t: their two durations against the longer one and their summed work);
   * trace.json, the profiler's Chrome trace.
 The card name and power limit are read in the same run.  TWG_LIB selects another build of the library.  Needs a GPU."""
 from __future__ import annotations
@@ -80,6 +87,43 @@ def conv_traffic(entry, N, H, W, Cin, Cout, k, pad):
           'l2_after': float(after), 'cols': cols}
 
 
+# ---- launch fill: CTAs one SM of an H100 (sm_90) holds, from the launch's resources (the CUDA occupancy rules) ----
+SMS = 132
+
+
+def resident_ctas(threads, regs, smem):
+  """CTAs of `threads` threads, `regs` registers per thread and `smem` bytes of shared memory one sm_90 SM holds."""
+  warps = -(-threads // 32)
+  by_warps = 64 // warps
+  by_blocks = 32
+  reg_warp = -(-max(regs, 1) * 32 // 256) * 256                # registers are allocated per warp in units of 256
+  by_regs = (65536 // reg_warp) // warps
+  by_smem = 233472 // (-(-(smem + 1024) // 128) * 128) if smem else by_blocks    # 1 KB per CTA is reserved
+  return max(0, min(by_warps, by_blocks, by_regs, by_smem))
+
+
+def launch_fill(grid, per_sm):
+  """(waves, the launch's average share of the GPU's CTA slots, the share of its time spent in a last partial wave),
+  every wave taken to last as long as the others."""
+  wave = SMS * max(per_sm, 1)
+  waves = -(-grid // wave)
+  util = grid / float(waves * wave)
+  tail = (1.0 / waves) if (grid % wave and waves > 1) else 0.0
+  return waves, util, tail
+
+
+def overlap_bound(a, b):
+  """Upper bound of the time saved by running launch list `a` beside `b` (pairs in order, (us, util) each): a pair takes
+  at least its longer launch and at least its summed work over the whole GPU."""
+  saved = 0.0
+  for (da, ua), (db, ub) in zip(a, b):
+    saved += da + db - max(da, db, da * ua + db * ub)
+  return saved
+
+
+CHAINS = ('Ds', 'Dt', 'DRs', 'DRt')
+
+
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--out', required=True)
@@ -90,7 +134,7 @@ def main():
   ap.add_argument('--warmup', type=int, default=2)
   args = ap.parse_args()
   import torch
-  from torch.profiler import ProfilerActivity, profile
+  from torch.profiler import ProfilerActivity, profile, record_function
   if not torch.cuda.is_available():
     raise SystemExit('profile_step.py needs a CUDA device')
   from bench import gpu_info
@@ -111,19 +155,42 @@ def main():
   L = lib()
   calls = []
   call = L.call
+  # the chain a launch belongs to: ops.trace_tag in the forward; in a backward, the tag its node was made under, which a
+  # node made during that backward (create_graph) inherits
+  chain = [None]
 
   def spy(name, *a):
     if name in _GEOM_AT:
       i = _GEOM_AT[name]
       calls.append((name,) + tuple(int(v) for v in a[i:i + 7]))
-    return call(name, *a)
+    with record_function('twg|%s|%s' % (chain[0] or ops.TRACE_TAG, name)):
+      return call(name, *a)
+
+  def tagged(fwd, bwd):
+    def forward(ctx, *a, **k):
+      ctx._twg_chain = chain[0] or ops.TRACE_TAG
+      return fwd(ctx, *a, **k)
+
+    def backward(ctx, *g):
+      prev, chain[0] = chain[0], getattr(ctx, '_twg_chain', None)
+      try:
+        return bwd(ctx, *g)
+      finally:
+        chain[0] = prev
+    return staticmethod(forward), staticmethod(backward)
+  saved = {c: (vars(c)['forward'], vars(c)['backward']) for c in vars(ops).values()
+           if isinstance(c, type) and issubclass(c, torch.autograd.Function) and 'forward' in vars(c)}
+  for c in saved:
+    c.forward, c.backward = tagged(c.forward, c.backward)
   L.call = spy
   try:
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
       model.train_step(s, t, r)
       torch.cuda.synchronize()
   finally:
     del L.call
+    for c, (forward, backward) in saved.items():
+      c.forward, c.backward = forward, backward
   os.makedirs(args.out, exist_ok=True)
   trace = os.path.join(args.out, 'trace.json')
   prof.export_chrome_trace(trace)
@@ -193,6 +260,58 @@ def main():
     json.dump({'gpu': gpu, 'library': LIB_PATH, 'kernel_us': total, 'span_us': span, 'kernels': table}, f, indent=1)
   with open(os.path.join(args.out, 'convs.json'), 'w') as f:
     json.dump({'gpu': gpu, 'library': LIB_PATH, 'groups': groups, 'launches': rows}, f, indent=1)
+
+  # each kernel -> the runtime call that launched it (correlation id) -> the library call around it (same thread, time)
+  notes = collections.defaultdict(list)
+  for e in events:
+    if e.get('ph') == 'X' and str(e.get('name', '')).startswith('twg|'):
+      notes[e['tid']].append(e)
+  launch_at = {}
+  for e in events:
+    if e.get('ph') == 'X' and e.get('cat') in ('cuda_runtime', 'cuda_driver') and 'correlation' in e.get('args', {}):
+      launch_at[e['args']['correlation']] = e
+  fill = []
+  for k in kernels:
+    a = k['args']
+    rt = launch_at.get(a.get('correlation'))
+    tag = 'torch'
+    if rt is not None:
+      for n in notes.get(rt['tid'], ()):
+        if n['ts'] <= rt['ts'] <= n['ts'] + n['dur']:
+          tag = n['name'].split('|')[1]
+    grid = int(a['grid'][0]) * int(a['grid'][1]) * int(a['grid'][2])
+    block = int(a['block'][0]) * int(a['block'][1]) * int(a['block'][2])
+    per_sm = resident_ctas(block, int(a.get('registers per thread', 0)), int(a.get('shared memory', 0)))
+    waves, util, tail = launch_fill(grid, per_sm)
+    fill.append({'kernel': short(k['name']), 'chain': tag, 'us': k['dur'], 'grid': grid, 'block': block,
+                 'ctas_per_sm': per_sm, 'waves': waves, 'util': util, 'tail_us': k['dur'] * tail})
+  summary = collections.OrderedDict()
+  for tag in CHAINS + ('other',):
+    rows_t = [f_ for f_ in fill if (f_['chain'] == tag if tag != 'other' else f_['chain'] not in CHAINS)]
+    sub = [f_ for f_ in rows_t if f_['waves'] == 1 and f_['util'] < 1.0]
+    summary[tag] = {'launches': len(rows_t), 'us': sum(f_['us'] for f_ in rows_t),
+                    'sub_wave_launches': len(sub), 'sub_wave_us': sum(f_['us'] for f_ in sub),
+                    'tail_us': sum(f_['tail_us'] for f_ in rows_t),
+                    'idle_us': sum(f_['us'] * (1.0 - f_['util']) for f_ in rows_t)}
+  pairs = {}
+  for a_tag, b_tag in (('Ds', 'Dt'), ('DRs', 'DRt')):
+    la = [(f_['us'], f_['util']) for f_ in fill if f_['chain'] == a_tag]
+    lb = [(f_['us'], f_['util']) for f_ in fill if f_['chain'] == b_tag]
+    ka = [(f_['kernel'], f_['grid']) for f_ in fill if f_['chain'] == a_tag]
+    kb = [(f_['kernel'], f_['grid']) for f_ in fill if f_['chain'] == b_tag]
+    pairs[a_tag + '|' + b_tag] = {'launches': [len(la), len(lb)], 'same_kernels_and_grids': ka == kb,
+                                  'overlap_bound_us': overlap_bound(la, lb)}
+  print('\n%-8s %8s %10s %9s %12s %10s %10s' % ('chain', 'launches', 'total us', 'sub-wave', 'sub-wave us', 'tail us',
+                                               'idle us'))
+  for tag, d in summary.items():
+    print('%-8s %8d %10.1f %9d %12.1f %10.1f %10.1f' % (tag, d['launches'], d['us'], d['sub_wave_launches'],
+                                                       d['sub_wave_us'], d['tail_us'], d['idle_us']))
+  for key, d in pairs.items():
+    print('%s side by side: %s launches, same kernels and grids in order: %s, at most %.1f us saved'
+          % (key.replace('|', ' / '), d['launches'], d['same_kernels_and_grids'], d['overlap_bound_us']))
+  with open(os.path.join(args.out, 'fill.json'), 'w') as f:
+    json.dump({'gpu': gpu, 'library': LIB_PATH, 'sms': SMS, 'chains': summary, 'pairs': pairs, 'launches': fill}, f,
+              indent=1)
 
 
 if __name__ == '__main__':

@@ -20,7 +20,9 @@ int check_launch(const char* what);
 // block b's partial of output i at parts[b * n + i] (parts = partials(nb * n), zeroed when `zero`), and add_partials then
 // adds them to out[i] in block order -- fp32 atomics would add them in whatever order the blocks finish, and the training
 // step amplifies that last-bit noise into visibly different results from run to run.  The buffer is owned by the library
-// (one per device), so kernels of this library must not run concurrently on two streams of one device.
+// and split into fixed regions (twg_runtime.cu): a stream bound to a region of its own on its device (twg_partials_bind)
+// gets that region, every other stream region 0.  So this library's kernels may run concurrently on two streams of one
+// device only when at most one of them is unbound.
 float* partials(int64_t n, bool zero, cudaStream_t st);
 int add_partials(float* out, const float* parts, int nb, int64_t n, cudaStream_t st);
 

@@ -3,6 +3,8 @@
 #include <stdarg.h>
 #include <string.h>
 
+#include <mutex>
+
 #include "twg_common.cuh"
 
 namespace twg {
@@ -26,14 +28,45 @@ int check_launch(const char* what) {
 }
 
 constexpr int64_t kPartialFloats = 8 << 20;        // 32 MB: the largest user is the tensor-core weight gradient (<= ~5 M)
-__device__ float g_partials[kPartialFloats];
+// One region per stream that may run library work concurrently with another: region 0 serves every stream not bound
+// to a region of its own, regions 1.. are bound one stream each per device (twg_partials_bind; the table is keyed on the
+// current device, which is the device of the stream a launch goes to).  Fixed and preallocated, so a launch captured into
+// a CUDA graph never allocates.
+constexpr int kPartialRegions = 2;
+constexpr int kMaxDevices = 64;
+__device__ float g_partials[kPartialRegions * kPartialFloats];
+
+std::mutex g_region_mu;
+cudaStream_t g_region_stream[kMaxDevices][kPartialRegions] = {};   // [d][0] unused: region 0 has no owner
+bool g_region_bound[kMaxDevices][kPartialRegions] = {};
+std::atomic<int64_t> g_region_uses[kPartialRegions] = {};           // partials() calls served, all devices
+
+int current_device() {
+  int d = 0;
+  if (cudaGetDevice(&d) != cudaSuccess) {     // no device (host-only use of the table): keep slot 0
+    cudaGetLastError();
+    d = 0;
+  }
+  return d;
+}
+
+int partials_region(int dev, cudaStream_t st) {
+  if (dev < 0 || dev >= kMaxDevices) return 0;
+  std::lock_guard<std::mutex> lock(g_region_mu);
+  for (int r = 1; r < kPartialRegions; ++r)
+    if (g_region_bound[dev][r] && g_region_stream[dev][r] == st) return r;
+  return 0;
+}
 
 float* partials(int64_t n, bool zero, cudaStream_t st) {
   if (n > kPartialFloats) return nullptr;
   void* p = nullptr;
   if (cudaGetSymbolAddress(&p, g_partials) != cudaSuccess) return nullptr;
-  if (zero) cudaMemsetAsync(p, 0, sizeof(float) * n, st);
-  return static_cast<float*>(p);
+  int r = partials_region(current_device(), st);
+  g_region_uses[r].fetch_add(1, std::memory_order_relaxed);
+  float* region = static_cast<float*>(p) + r * kPartialFloats;
+  if (zero) cudaMemsetAsync(region, 0, sizeof(float) * n, st);
+  return region;
 }
 
 __global__ void __launch_bounds__(256) k_add_partials(float* __restrict__ out, const float* __restrict__ parts, int nb,
@@ -75,6 +108,38 @@ extern "C" {
 int twg_version(void) { return 101; }
 const char* twg_last_error(void) { return g_err; }
 int64_t twg_launch_count(void) { return g_launches.load(); }
+
+int twg_partials_regions(void) { return kPartialRegions; }
+int64_t twg_partials_region_floats(void) { return kPartialFloats; }
+int twg_partials_region(const void* stream_key) { return partials_region(current_device(), (cudaStream_t)stream_key); }
+
+int64_t twg_partials_region_uses(int region) {
+  return (region >= 0 && region < kPartialRegions) ? g_region_uses[region].load() : -1;
+}
+
+int twg_partials_bind(const void* stream_key, int region) {
+  cudaStream_t st = (cudaStream_t)stream_key;
+  if (region < 0 || region >= kPartialRegions)
+    return fail(TWG_ERR_INVALID, "partials_bind: region %d is not one of 0..%d", region, kPartialRegions - 1);
+  if (st == nullptr) return fail(TWG_ERR_INVALID, "partials_bind: the default stream keeps region 0");
+  int dev = current_device();
+  if (dev >= kMaxDevices) return fail(TWG_ERR_INVALID, "partials_bind: device %d is beyond %d", dev, kMaxDevices);
+  std::lock_guard<std::mutex> lock(g_region_mu);
+  cudaStream_t* owner = g_region_stream[dev];
+  bool* bound = g_region_bound[dev];
+  for (int r = 1; r < kPartialRegions; ++r)
+    if (bound[r] && owner[r] == st && r != region) {
+      if (region != 0) return fail(TWG_ERR_INVALID, "partials_bind: the stream already owns region %d", r);
+      bound[r] = false;                               // region 0: the stream gives its region back
+      owner[r] = nullptr;
+    }
+  if (region == 0) return TWG_OK;
+  if (bound[region] && owner[region] != st)
+    return fail(TWG_ERR_INVALID, "partials_bind: region %d belongs to another stream", region);
+  owner[region] = st;
+  bound[region] = true;
+  return TWG_OK;
+}
 
 int64_t twg_crc32c(const void* data, int64_t n, int64_t crc) {
   static const Crc32cTable tables;        // built once, on first use; the initialisation is thread-safe

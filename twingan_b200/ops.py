@@ -71,6 +71,24 @@ def _st():
   return torch.cuda.current_stream().cuda_stream
 
 
+_DOMAIN_STREAMS = {}   # device index -> the stream the second discriminator domain runs on
+
+
+def domain_stream(device) -> torch.cuda.Stream:
+  """The stream of the training step's second discriminator domain on `device`: one per device for the process, bound to a
+  partial-sum region of its own in the library, so that its reductions never share scratch with the other domain's."""
+  idx = torch.device(device).index
+  idx = torch.cuda.current_device() if idx is None else idx
+  st = _DOMAIN_STREAMS.get(idx)
+  if st is None:
+    st = torch.cuda.Stream(device=idx)
+    with torch.cuda.device(idx):        # the library keys the binding on the current device
+      if lib().try_call('twg_partials_bind', st.cuda_stream, 1) != 0:     # binds, launches nothing
+        raise TwgError('twg_partials_bind: ' + lib().last_error())
+    _DOMAIN_STREAMS[idx] = st
+  return st
+
+
 # ------------------------------------------------------------------------------------------------
 # convolution (bilinear => closed under differentiation)
 # ------------------------------------------------------------------------------------------------
@@ -388,7 +406,7 @@ def register_grad_sinks(mapping) -> None:
 # their conv nodes were created, which is the program's order and does not depend on that history.
 _CONV_SERIAL = [0]          # creation counter of the conv nodes (forward order; the first-order backward's are in order)
 _DEFER_GROUPS = set()
-_DEFERRED = []              # (serial, operands of _conv_wgrad, sink)
+_DEFERRED = []              # (serial, operands of _conv_wgrad, sink, the stream the conv node's backward ran on)
 
 
 def _next_serial() -> int:
@@ -410,9 +428,11 @@ def fixed_order_weight_grads(group: Optional[str]):
 
 
 def flush_weight_grads() -> None:
-  """Add the recorded weight gradients into their sinks, in the creation order of their conv nodes."""
-  for _, (x, gy, k, pad, xp, gp), sink in sorted(_DEFERRED, key=lambda e: e[0]):
-    _conv_wgrad(x, gy, k, pad, xp, gp, out=sink)
+  """Add the recorded weight gradients into their sinks, in the creation order of their conv nodes, each on the stream its
+  node ran on (a discriminator domain's stream keeps that domain's adds in order after the operands it made)."""
+  for _, (x, gy, k, pad, xp, gp), sink, stream in sorted(_DEFERRED, key=lambda e: e[0]):
+    with torch.cuda.stream(stream):
+      _conv_wgrad(x, gy, k, pad, xp, gp, out=sink)
   _DEFERRED.clear()
 
 
@@ -428,7 +448,7 @@ def _weight_grad(ctx, w, x, gy, xp=None, gp=None):
   sink = _sink(w)
   if sink is not None:
     if ctx.group in _DEFER_GROUPS:
-      _DEFERRED.append((ctx.serial, (x, gy, ctx.k, ctx.pad, xp, gp), sink))
+      _DEFERRED.append((ctx.serial, (x, gy, ctx.k, ctx.pad, xp, gp), sink, torch.cuda.current_stream()))
     else:
       _conv_wgrad(x, gy, ctx.k, ctx.pad, xp, gp, out=sink)
     return None
@@ -881,14 +901,16 @@ def norm_update_stats(state_live, batch_stats, kind, C, decay=0.99, eps=1e-3):
 # discriminator arg scope: bias + leaky-ReLU, twice differentiable
 # ------------------------------------------------------------------------------------------------
 
-_DUMMY_COLSUM = {}
+_DUMMY_COLSUM = {}   # (device, stream) -> discarded column sums; per stream, so that a buffer outgrown and freed on
+                     # one stream is never one another stream is still writing into
 
 
 def _dummy_colsum(device, C):
-  t = _DUMMY_COLSUM.get(device)
+  key = (device, torch.cuda.current_stream(device).cuda_stream)
+  t = _DUMMY_COLSUM.get(key)
   if t is None or t.numel() < C:
     t = torch.zeros(max(C, 1024), device=device, dtype=torch.float32)
-    _DUMMY_COLSUM[device] = t
+    _DUMMY_COLSUM[key] = t
   return t
 
 

@@ -58,6 +58,13 @@ class Flags:
   # -> one 2B pass, the four G passes -> one 4B pass, E(t'),E(s') -> one 2B pass, D_x(real, cycle, prime) -> one 3B pass
   # per domain -- instead of 16 separate passes.  Same arithmetic per sample; batch statistics stay per original pass.
   batch_passes: bool = True
+  # Engine option: with batch_passes, run the domain-t discriminator chain (D_t's forward and GAN terms, the DRAGAN
+  # penalty's forward and input gradient on x_hat_t, and through autograd their backward nodes) on a second stream,
+  # beside the domain-s chain.  The domains share no variable, sink or partial-sum region, and each chain keeps its
+  # kernels and their order, so the results are the serial schedule's bit for bit; the under-filled launches of the
+  # discriminators' small layers and the tail waves of their large ones overlap the other domain's.  False: the serial
+  # schedule (the parity twin).
+  concurrent_domains: bool = True
 
 
 class GanModel:
@@ -163,37 +170,33 @@ class GanModel:
                                 stats=stats, tags=self._G_TAGS)
     d_s_in, d_t_in, e2_in, l_cyc_s, l_cyc_t = ops.FanoutFn.apply(gout, x, f.l_cyc_weight)
     self._d_cut += [d_s_in, d_t_in]
+    # the domain-t chain forks here, after twg_fanout_fwd made its batch; its backward nodes run on the stream it was built on
+    main = torch.cuda.current_stream(x.device)
+    side = ops.domain_stream(x.device) if f.concurrent_domains else main
+    if side is not main:
+      # ops._one is made lazily, by whichever chain needs it first (the WGAN-GP interpolate): made here, before the
+      # fork, neither chain can read it while the other stream is still filling it
+      ops._one(x.device)
+      side.wait_stream(main)
+      # made on the current stream and read on `side` until the discriminator-loss backward frees them: the allocator
+      # must not hand their memory to the current stream's work before `side` is done with them
+      d_t_in.record_stream(side)
+      x.record_stream(side)
     with ops.trace_tag('E2'):
       enc2, _ = self._encoder(e2_in, ('_t', '_s'), stats=stats, tags=self._E2_TAGS)
     with ops.trace_tag('Ds'):
       pred_s, _ = self._discriminator(d_s_in, DISCRIMINATOR_VAR_SCOPE_SOURCE, groups=3)
-    with ops.trace_tag('Dt'):
+    with ops.trace_tag('Dt'), torch.cuda.stream(side):
       pred_t, _ = self._discriminator(d_t_in, DISCRIMINATOR_VAR_SCOPE_TARGET, groups=3)
     gl, dl = {}, {}
     gl['l_cyc_s'], gl['l_cyc_t'] = l_cyc_s, l_cyc_t
     cyc = f.train_image_size >= 64 and f.do_l_cyc_gan       # twingan.py:466
-    for dom, pred, dscope in (('s', pred_s, DISCRIMINATOR_VAR_SCOPE_SOURCE), ('t', pred_t, DISCRIMINATOR_VAR_SCOPE_TARGET)):
-      original = x.detach()[0:B] if dom == 's' else x.detach()[B:2 * B]
-      if f.loss_architecture in ('gan', 'dragan'):
-        fool_c, fool_p, fake_c, real_c, fake_p, real_p = ops.GanLossesFn.apply(pred, f.gan_weight)
-        if cyc:
-          gl['generator_fool_loss_cycle_' + dom] = fool_c
-          dl['discriminator_fake_loss_cycle_' + dom] = fake_c
-          dl['discriminator_real_loss_cycle_' + dom] = real_c
-        gl['generator_fool_loss_prime_' + dom] = fool_p
-        dl['discriminator_fake_loss_prime_' + dom] = fake_p
-        dl['discriminator_real_loss_prime_' + dom] = real_p
-        if f.loss_architecture == 'dragan':
-          with ops.trace_tag('DR' + dom):
-            dl['discriminator_gradient_penalty_prime_' + dom] = self._add_dragan_loss(
-                original, dscope, dragan_rand['alpha_' + dom], dragan_rand['noise_' + dom])
-      else:
-        # wgan / wgan_gp / hinge (SURVEY 8f-4): the terms of add_gan_loss on the blocks [real | cycle | prime] of the batch
-        real_pred = pred[0:B]
-        for post, fake_pred in ((('cycle', pred[B:2 * B]),) if cyc else ()) + (('prime', pred[2 * B:3 * B]),):
-          fake_img = gout[3 * B:4 * B] if dom == 's' else gout[2 * B:3 * B]     # s_prime / t_prime (only used for 'prime')
-          with ops.trace_tag('DR' + dom):
-            self._add_gan_loss_optional(gl, dl, dom, post, fake_pred, real_pred, fake_img, original, dscope, dragan_rand)
+    for dom, pred, dscope, stream in (('s', pred_s, DISCRIMINATOR_VAR_SCOPE_SOURCE, main),
+                                      ('t', pred_t, DISCRIMINATOR_VAR_SCOPE_TARGET, side)):
+      with torch.cuda.stream(stream):
+        self._add_domain_gan_losses(gl, dl, dom, pred, dscope, x, gout, B, cyc, dragan_rand)
+    if side is not main:
+      main.wait_stream(side)
     if f.l_content_weight:
       # l_content_s = |enc_s - enc_t_prime|, l_content_t = |enc_t - enc_s_prime| (twingan.py:485-505): block g of enc vs enc2
       gl['l_content_s'], gl['l_content_t'] = ops.L1GroupsFn.apply(enc2, enc, f.l_content_weight)
@@ -210,6 +213,31 @@ class GanModel:
               'pred_real_t': pred_t[0:B], 'pred_t_cycle': pred_t[B:2 * B], 'pred_t_prime': pred_t[2 * B:3 * B]}
     stats.sort(key=lambda e: e[4])     # EMA pushes in the reference's program order (stable: layers stay in order)
     return g_loss, d_loss, named, ends, stats
+
+  def _add_domain_gan_losses(self, gl, dl, dom, pred, dscope, x, gout, B, cyc, dragan_rand):
+    """The GAN terms of one discriminator batch [real | cycle | prime] and, with DRAGAN / WGAN-GP, its penalty chain."""
+    f = self.flags
+    original = x.detach()[0:B] if dom == 's' else x.detach()[B:2 * B]
+    if f.loss_architecture in ('gan', 'dragan'):
+      fool_c, fool_p, fake_c, real_c, fake_p, real_p = ops.GanLossesFn.apply(pred, f.gan_weight)
+      if cyc:
+        gl['generator_fool_loss_cycle_' + dom] = fool_c
+        dl['discriminator_fake_loss_cycle_' + dom] = fake_c
+        dl['discriminator_real_loss_cycle_' + dom] = real_c
+      gl['generator_fool_loss_prime_' + dom] = fool_p
+      dl['discriminator_fake_loss_prime_' + dom] = fake_p
+      dl['discriminator_real_loss_prime_' + dom] = real_p
+      if f.loss_architecture == 'dragan':
+        with ops.trace_tag('DR' + dom):
+          dl['discriminator_gradient_penalty_prime_' + dom] = self._add_dragan_loss(
+              original, dscope, dragan_rand['alpha_' + dom], dragan_rand['noise_' + dom])
+    else:
+      # wgan / wgan_gp / hinge (SURVEY 8f-4): the terms of add_gan_loss on the blocks [real | cycle | prime] of the batch
+      real_pred = pred[0:B]
+      for post, fake_pred in ((('cycle', pred[B:2 * B]),) if cyc else ()) + (('prime', pred[2 * B:3 * B]),):
+        fake_img = gout[3 * B:4 * B] if dom == 's' else gout[2 * B:3 * B]     # s_prime / t_prime (only used for 'prime')
+        with ops.trace_tag('DR' + dom):
+          self._add_gan_loss_optional(gl, dl, dom, post, fake_pred, real_pred, fake_img, original, dscope, dragan_rand)
 
   @staticmethod
   def trace_in_reference_order(trace, batch):
@@ -387,6 +415,7 @@ class GanModel:
       # accumulators were created on, which a CUDA-graph capture of the step does not survive.
       with ops.skip_param_grads('D'):
         torch.autograd.grad(g_loss, self._g_cut, retain_graph=True, allow_unused=True)
+      self._join_domains()
       # the scratch gradients of the generator set's scaled weights (--equalized_learning_rate) go into their sinks now,
       # so the generator-set slice of the buffer is final from here on: the discriminator backward adds nothing to it
       ops.flush_padded_sinks(v.group_slice(self.flat_grad, 'G'))
@@ -397,6 +426,7 @@ class GanModel:
       with ops.skip_param_grads('G'), ops.fixed_order_weight_grads('D' if self.flags.use_res_block else None):
         torch.autograd.grad(d_loss, self._d_cut, allow_unused=True)
       ops.flush_weight_grads()
+      self._join_domains()
       ops.flush_padded_sinks()
     finally:
       ops.drop_weight_grads()
@@ -407,6 +437,12 @@ class GanModel:
     self.last_losses = {'generator_loss': g_loss.detach(), 'discriminator_loss': d_loss.detach()}
     self.last_losses.update({k: t.detach() for k, t in named.items()})
     return g_loss.detach(), d_loss.detach(), ends, stats
+
+  def _join_domains(self):
+    """Make the current stream wait for the domain-t discriminator chain (Flags.concurrent_domains): autograd joins what
+    a later node consumes, not the gradient sinks and scratch sinks that chain wrote."""
+    if self.flags.batch_passes and self.flags.concurrent_domains:
+      torch.cuda.current_stream(self.device).wait_stream(ops.domain_stream(self.device))
 
   def allreduce_gradients(self, group: Optional[str] = None):
     """deployment/model_deploy.py:473-503 (tf.add_n over clones) -> NCCL all-reduce(sum) of the flat bucket ('G' / 'D' set
