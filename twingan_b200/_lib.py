@@ -1,5 +1,6 @@
 """ctypes binding of libtwg.so (the C-ABI declared in include/twg.h, the JPEG decoder's in include/twgjpeg.h, the
-JPEG encoder's in include/twgjenc.h and the PNG decoder's in include/twgpng.h).
+progressive JPEG decoder's in include/twgjpegp.h, the JPEG encoder's in include/twgjenc.h and the PNG decoder's in
+include/twgpng.h).
 
 The prototypes are parsed from the header itself so the Python side can never drift from the ABI.
 There is no CPU fallback: if the library is missing, or a kernel entry point is called without a CUDA
@@ -16,6 +17,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'twg.h')
 JPEG_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'twgjpeg.h')
 JPEG_PREFIX = 'twgjpeg_'
+JPEGP_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'twgjpegp.h')
+JPEGP_PREFIX = 'twgjpegp_'
 JENC_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'twgjenc.h')
 JENC_PREFIX = 'twgjenc_'
 PNG_HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'twgpng.h')
@@ -62,9 +65,11 @@ class _Lib:
     self.cdll = ctypes.CDLL(LIB_PATH)
     self.protos = parse_header()
     self.jpeg_protos = parse_header(JPEG_HEADER, JPEG_PREFIX)
+    self.jpegp_protos = parse_header(JPEGP_HEADER, JPEGP_PREFIX)
     self.jenc_protos = parse_header(JENC_HEADER, JENC_PREFIX)
     self.png_protos = parse_header(PNG_HEADER, PNG_PREFIX)
-    for name, (ret, args) in (list(self.protos.items()) + list(self.jpeg_protos.items()) + list(self.jenc_protos.items())
+    for name, (ret, args) in (list(self.protos.items()) + list(self.jpeg_protos.items())
+                              + list(self.jpegp_protos.items()) + list(self.jenc_protos.items())
                               + list(self.png_protos.items())):
       fn = getattr(self.cdll, name)  # raises AttributeError if the symbol is not exported
       fn.restype = _CTYPES[ret]

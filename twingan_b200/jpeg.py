@@ -98,6 +98,69 @@ def _huff_ok(bits: bytes, vals: bytes, is_dc: bool) -> bool:
   return not (is_dc and any(v > 15 for v in vals))
 
 
+def read_dht(seg: bytes, huff: dict, check: bool) -> None:
+  """The tables of one DHT segment into huff[(class, id)] = (BITS, HUFFVAL); with `check`, each is held to `_huff_ok`
+  as it is defined (a progressive file checks only the tables its scans use, when they use them)."""
+  i = 0
+  while i < len(seg):
+    if i + 17 > len(seg):
+      raise Unsupported('bad DHT')
+    tc, th = seg[i] >> 4, seg[i] & 15
+    bits = bytes(seg[i + 1:i + 17])
+    cnt = sum(bits)
+    if tc > 1 or th > 3 or cnt > 256 or i + 17 + cnt > len(seg):
+      raise Unsupported('bad DHT')
+    vals = bytes(seg[i + 17:i + 17 + cnt])
+    if check and not _huff_ok(bits, vals, tc == 0):
+      raise Unsupported('invalid Huffman table')
+    huff[(tc, th)] = (bits, vals)
+    i += 17 + cnt
+
+
+def read_dqt(seg: bytes, qt: dict) -> None:
+  """The tables of one DQT segment (8- or 16-bit) into qt[id] = int32 [64], zig-zag order."""
+  i = 0
+  while i < len(seg):
+    pq, tq = seg[i] >> 4, seg[i] & 15
+    size = 64 * (pq + 1)
+    if pq > 1 or tq > 3 or i + 1 + size > len(seg):
+      raise Unsupported('bad DQT')
+    raw = np.frombuffer(seg[i + 1:i + 1 + size], dtype='>u2' if pq else np.uint8)
+    qt[tq] = raw.astype(np.int32)
+    i += 1 + size
+
+
+def read_dri(seg: bytes) -> int:
+  if len(seg) != 2:
+    raise Unsupported('bad DRI')
+  return _u16(seg, 0)
+
+
+def is_jfif(seg: bytes) -> bool:
+  return len(seg) >= 14 and seg[:5] == b'JFIF\0'
+
+
+def is_adobe(seg: bytes) -> bool:
+  return len(seg) >= 12 and seg[:5] == b'Adobe'
+
+
+def colour_and_sampling(comps: Tuple[Component, ...], jfif: bool, adobe: bool, transform) -> Tuple[Component, ...]:
+  """The frame's components as decoded, or `Unsupported`: 3 components only when libjpeg reads them as YCbCr (a JFIF
+  APP0, an Adobe APP14 with transform 1, or neither marker and ids 1, 2, 3) at 4:4:4, 4:2:2 or 4:2:0; a lone
+  component is coded one block per MCU whatever its factors."""
+  if len(comps) == 3:
+    if not jfif:
+      if adobe and transform != 1:
+        raise Unsupported('Adobe transform %d' % transform)
+      if not adobe and [c.id for c in comps] != [1, 2, 3]:
+        raise Unsupported('component ids %s without JFIF or Adobe marker' % [c.id for c in comps])
+    y, cb, cr = comps
+    if (cb.h, cb.v, cr.h, cr.v) != (1, 1, 1, 1) or (y.h, y.v) not in ((1, 1), (2, 1), (2, 2)):
+      raise Unsupported('sampling %s' % ['%dx%d' % (c.h, c.v) for c in comps])
+    return comps
+  return (comps[0]._replace(h=1, v=1),)
+
+
 def parse(data: bytes) -> JpegInfo:
   """The header and segment layout of a JPEG file the device decodes; `Unsupported` otherwise."""
   b = memoryview(data).cast('B') if not isinstance(data, (bytes, bytearray)) else data
@@ -146,39 +209,15 @@ def parse(data: bytes) -> JpegInfo:
     elif m == 0xCC:
       raise Unsupported('arithmetic coding (DAC)')
     elif m == 0xC4:
-      i = 0
-      while i < len(seg):
-        if i + 17 > len(seg):
-          raise Unsupported('bad DHT')
-        tc, th = seg[i] >> 4, seg[i] & 15
-        bits = bytes(seg[i + 1:i + 17])
-        cnt = sum(bits)
-        if tc > 1 or th > 3 or cnt > 256 or i + 17 + cnt > len(seg):
-          raise Unsupported('bad DHT')
-        vals = bytes(seg[i + 17:i + 17 + cnt])
-        if not _huff_ok(bits, vals, tc == 0):
-          raise Unsupported('invalid Huffman table')
-        huff[(tc, th)] = (bits, vals)
-        i += 17 + cnt
+      read_dht(seg, huff, check=True)
     elif m == 0xDB:
-      i = 0
-      while i < len(seg):
-        pq, tq = seg[i] >> 4, seg[i] & 15
-        size = 64 * (pq + 1)
-        if pq > 1 or tq > 3 or i + 1 + size > len(seg):
-          raise Unsupported('bad DQT')
-        raw = np.frombuffer(seg[i + 1:i + 1 + size], dtype='>u2' if pq else np.uint8)
-        qt[tq] = raw.astype(np.int32)
-        i += 1 + size
+      read_dqt(seg, qt)
     elif m == 0xDD:
-      if len(seg) != 2:
-        raise Unsupported('bad DRI')
-      ri = _u16(seg, 0)
+      ri = read_dri(seg)
     elif m == 0xE0:
-      if len(seg) >= 14 and seg[:5] == b'JFIF\0':
-        jfif = True
+      jfif = jfif or is_jfif(seg)
     elif m == 0xEE:
-      if len(seg) >= 12 and seg[:5] == b'Adobe':
+      if is_adobe(seg):
         adobe, transform = True, seg[11]
     elif 0xE1 <= m <= 0xEF or m == 0xFE:
       pass
@@ -201,18 +240,7 @@ def parse(data: bytes) -> JpegInfo:
   if ss != 0 or se != 63 or ahal != 0:
     raise Unsupported('not a sequential scan (Ss %d, Se %d, AhAl %02X)' % (ss, se, ahal))
   tables = [(seg[2 + 2 * i] >> 4, seg[2 + 2 * i] & 15) for i in range(ns)]
-  # colour space and sampling
-  if len(comps) == 3:
-    if not jfif:
-      if adobe and transform != 1:
-        raise Unsupported('Adobe transform %d' % transform)
-      if not adobe and [c.id for c in comps] != [1, 2, 3]:
-        raise Unsupported('component ids %s without JFIF or Adobe marker' % [c.id for c in comps])
-    y, cb, cr = comps
-    if (cb.h, cb.v, cr.h, cr.v) != (1, 1, 1, 1) or (y.h, y.v) not in ((1, 1), (2, 1), (2, 2)):
-      raise Unsupported('sampling %s' % ['%dx%d' % (c.h, c.v) for c in comps])
-  else:
-    comps = (comps[0]._replace(h=1, v=1),)      # a lone component is coded one block per MCU whatever its factors
+  comps = colour_and_sampling(comps, jfif, adobe, transform)
   for c in comps:
     if c.tq not in qt:
       raise Unsupported('quantisation table %d undefined' % c.tq)

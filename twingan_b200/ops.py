@@ -16,7 +16,7 @@ from __future__ import annotations
 import contextlib
 import math
 import weakref
-from typing import Optional, Tuple
+from typing import Optional, Sequence, Tuple
 
 import torch
 from torch.autograd import Function
@@ -1650,19 +1650,64 @@ def jpeg_decode(payload: torch.Tensor, data: torch.Tensor, segs: torch.Tensor, c
   n = int(images.shape[0])
   status = torch.empty(n, device=dev, dtype=torch.int32)
   coefs = torch.empty(blocks * 64, device=dev, dtype=torch.int16)
-  planes = torch.empty(plane_bytes, device=dev, dtype=torch.uint8)
   L = lib()
   L.call('twgjpeg_entropy', data.data_ptr(), segs.data_ptr(), int(segs.shape[0]), images.data_ptr(), n,
          comps.data_ptr(), huff.data_ptr(), coefs.data_ptr(), status.data_ptr(), _st())
   if stage_hook:
     stage_hook(JPEG_STAGES[0])
+  _jpeg_pixels(payload, coefs, comps, images, qt, blocks, plane_bytes, pixels, status, stage_hook)
+  return status
+
+
+def _jpeg_pixels(payload, coefs, comps, images, qt, blocks: int, plane_bytes: int, pixels: int, status, stage_hook):
+  """The stages after entropy decoding, shared by baseline and progressive files: dequantisation and inverse DCT into
+  sample planes (twgjpeg_idct), then upsampling and colour conversion into the payload (twgjpeg_color)."""
+  planes = torch.empty(plane_bytes, device=payload.device, dtype=torch.uint8)
+  L = lib()
   L.call('twgjpeg_idct', coefs.data_ptr(), comps.data_ptr(), int(comps.shape[0]), blocks, qt.data_ptr(),
          planes.data_ptr(), status.data_ptr(), _st())
   if stage_hook:
     stage_hook(JPEG_STAGES[1])
-  L.call('twgjpeg_color', planes.data_ptr(), images.data_ptr(), n, comps.data_ptr(), pixels, payload.data_ptr(), _st())
+  L.call('twgjpeg_color', planes.data_ptr(), images.data_ptr(), int(images.shape[0]), comps.data_ptr(), pixels,
+         payload.data_ptr(), _st())
   if stage_hook:
     stage_hook(JPEG_STAGES[2])
+
+
+JPEGP_STAGES = ('twgjpegp_reset', 'twgjpegp_entropy') + JPEG_STAGES[1:]
+
+
+def jpeg_progressive_decode(payload: torch.Tensor, data: torch.Tensor, segs: torch.Tensor, scans: torch.Tensor,
+                            comps: torch.Tensor, images: torch.Tensor, qt: torch.Tensor, huff: torch.Tensor,
+                            blocks: int, plane_bytes: int, pixels: int, levels: Sequence[int], stage_hook=None
+                            ) -> torch.Tensor:
+  """Decode the progressive JPEG files of one batch into their regions of a uint8 CUDA payload: zero the coefficients
+  (twgjpegp_reset), decode the scans one level at a time in stream order (twgjpegp_entropy: segment rows
+  [levels[l], levels[l + 1]) are level l's), then the baseline inverse DCT and colour conversion (twgjpeg_idct,
+  twgjpeg_color).  The descriptors are a jpeg_progressive.Batch on the device, `blocks`, `plane_bytes`, `pixels` and
+  `levels` its host sizes.  Returns the int32 [images] device status without waiting for it: 0 for an image decoded bit
+  for bit as libjpeg-turbo, else the TWG_JPEG_* / TWG_JPEGP_* bits of what made the device stop
+  (jpeg.STATUS_*, jpeg_progressive.STATUS_*); such an image's region is undefined.  The scratch comes from the caching
+  allocator on the current stream, so calls on several streams may run at once.  `stage_hook(name)`, when given, is
+  called after each stage is enqueued, with 'twgjpegp_entropy:<level>' for each level (timing)."""
+  if not payload.is_cuda or payload.dtype != torch.uint8:
+    raise TwgError('jpeg_progressive_decode: payload must be a uint8 CUDA tensor (no CPU fallback)')
+  dev = payload.device
+  n = int(images.shape[0])
+  status = torch.empty(n, device=dev, dtype=torch.int32)
+  coefs = torch.empty(blocks * 64, device=dev, dtype=torch.int16)
+  L = lib()
+  L.call('twgjpegp_reset', coefs.data_ptr(), blocks, status.data_ptr(), n, _st())
+  if stage_hook:
+    stage_hook(JPEGP_STAGES[0])
+  for l in range(len(levels) - 1):
+    a, e = int(levels[l]), int(levels[l + 1])
+    if e > a:
+      L.call('twgjpegp_entropy', data.data_ptr(), segs[a:].data_ptr(), e - a, scans.data_ptr(), comps.data_ptr(),
+             huff.data_ptr(), coefs.data_ptr(), status.data_ptr(), _st())
+    if stage_hook:
+      stage_hook('%s:%d' % (JPEGP_STAGES[1], l))
+  _jpeg_pixels(payload, coefs, comps, images, qt, blocks, plane_bytes, pixels, status, stage_hook)
   return status
 
 

@@ -4,18 +4,20 @@ inference/image_translation_infer.py (docs/infer_and_eval.md), with its flag nam
   python -m twingan_b200.translate --model_path=<train_dir>/256 --image_hw=256 \\
       --input_image_path=<file or directory> --output_image_path=<file or directory>
 
-JPEG and PNG files are decoded on the device, pixel for pixel as PIL decodes them, and JPEG outputs are encoded there,
+JPEG (baseline and progressive) and PNG files are decoded on the device, pixel for pixel as PIL decodes them, and JPEG outputs are encoded there,
 byte for byte as PIL does; PIL decodes every other input (as util_io.imread) and encodes every other output (as
 util_io.imsave); everything between runs on the device.  Per batch:
   * a background thread reads the files of batch k+1 on a pool of `--num_decode_threads` threads.  A JPEG that
-    twingan_b200/jpeg.py accepts (baseline Huffman, grey or YCbCr, 4:4:4 / 4:2:2 / 4:2:0) or a PNG that
+    twingan_b200/jpeg.py accepts (baseline Huffman, grey or YCbCr, 4:4:4 / 4:2:2 / 4:2:0), a progressive JPEG that
+    twingan_b200/jpeg_progressive.py accepts (the same frames, every coefficient refined to its last bit) or a PNG that
     twingan_b200/png.py accepts (not interlaced, not animated, no palette transparency, known chunks, every CRC right)
     travels compressed, with its descriptors; PIL decodes every other file into its region of one uint8 payload + a
     table of {offset, H, W} (HostPrefetcher, pinned memory; the headers give the device files' rows before any
     decoding) while batch k computes;
   * the payload, table and compressed data are copied to the device on a side stream (DevicePrefetcher);
-  * three kernels decode the JPEG scans (ops.jpeg_decode) and three the PNG streams (ops.png_decode) into their regions
-    of a copy of the payload, on a stream of the batch's own, up to Translator.DECODE_AHEAD batches ahead of the one
+  * three kernels decode the JPEG scans (ops.jpeg_decode), three the PNG streams (ops.png_decode), and the progressive
+    JPEG files are entropy-decoded one level of scans at a time before the same inverse DCT and colour kernels
+    (ops.jpeg_progressive_decode), into their regions of a copy of the payload, on a stream of the batch's own, up to Translator.DECODE_AHEAD batches ahead of the one
     translated (_DeviceDecoder: the decoders are serial within a file, so batches decode side by side); the batch's
     status is read once, when it is translated, and an image the device could not decode exactly is decoded by PIL and
     written into its region instead (a file PIL refuses fails as before);
@@ -140,13 +142,30 @@ def _device_png(data: Optional[bytes]):
   return info
 
 
+def _device_jpegp(data: Optional[bytes]):
+  """jpeg_progressive.ProgressiveInfo when the device decodes this file, else None; as _device_jpeg, above PIL's
+  decompression-bomb limit PIL decides."""
+  from PIL import Image
+  from . import jpeg_progressive
+  info = jpeg_progressive.probe(data) if data else None
+  if info is not None and Image.MAX_IMAGE_PIXELS and info.H * info.W > Image.MAX_IMAGE_PIXELS:
+    return None
+  return info
+
+
+DEVICE_KINDS = ('jpeg', 'png', 'jpegp')      # the device decoders, in the order a batch packs and decodes their files
+
+
 def _device_file(data: Optional[bytes]):
-  """('jpeg' or 'png', its info) when the device decodes this file, else None."""
+  """('jpeg', 'png' or 'jpegp', its info) when the device decodes this file, else None."""
   info = _device_jpeg(data)
   if info is not None:
     return 'jpeg', info
   info = _device_png(data)
-  return ('png', info) if info is not None else None
+  if info is not None:
+    return 'png', info
+  info = _device_jpegp(data)
+  return ('jpegp', info) if info is not None else None
 
 
 def _redecode(payload: torch.Tensor, status: torch.Tensor, files: '_DeviceFiles') -> None:
@@ -161,7 +180,7 @@ def _redecode(payload: torch.Tensor, status: torch.Tensor, files: '_DeviceFiles'
 
 
 class _DeviceDecoder(object):
-  """Decodes batches' JPEG and PNG files on the device with `ahead` batches in flight behind the one being translated.
+  """Decodes batches' JPEG, PNG and progressive JPEG files on the device with `ahead` batches in flight behind the one being translated.
 
   Entropy decoding and inflate are serial within a file (a thread or a warp each), so one batch keeps a few SMs busy
   for as long as its largest file takes.  Each batch therefore decodes on a stream of its own, concurrently with the
@@ -176,9 +195,10 @@ class _DeviceDecoder(object):
     self._n = 0
 
   def start(self, payload: torch.Tensor, table: torch.Tensor, descriptors, jpegs: Optional['_DeviceFiles'],
-            pngs: Optional['_DeviceFiles']):
-    """(payload, table, handle) of a batch (the six tensors of a jpeg.Batch, then the three of a png.Batch, each present
-    when its files are), the first two copies owned by the caller from now on."""
+            pngs: Optional['_DeviceFiles'], jpegps: Optional['_DeviceFiles'] = None):
+    """(payload, table, handle) of a batch (the six tensors of a jpeg.Batch, then the three of a png.Batch, then the
+    seven of a jpeg_progressive.Batch, each present when its files are), the first two copies owned by the caller from
+    now on."""
     from . import ops
     payload, table = payload.clone(), table.clone()
     descriptors = [d.clone() for d in descriptors]
@@ -186,7 +206,7 @@ class _DeviceDecoder(object):
     copied.record(torch.cuda.current_stream(self.device))
     stream = self.streams[self._n % len(self.streams)]   # its last batch was finished before this one started
     self._n += 1
-    if jpegs is None and pngs is None:
+    if jpegs is None and pngs is None and jpegps is None:
       return payload, table, None
     stream.wait_event(copied)
     for t in [payload] + descriptors:
@@ -198,30 +218,34 @@ class _DeviceDecoder(object):
         descriptors = descriptors[6:]
       if pngs is not None:
         status.append(ops.png_decode(payload, *descriptors[:3], *pngs.sizes))
+        descriptors = descriptors[3:]
+      if jpegps is not None:
+        status.append(ops.jpeg_progressive_decode(payload, *descriptors[:7], *jpegps.sizes))
       status = torch.cat(status) if len(status) > 1 else status[0]
       host = torch.empty(status.numel(), dtype=torch.int32).pin_memory()
       host.copy_(status, non_blocking=True)
       done = torch.cuda.Event()
       done.record(stream)
-    return payload, table, (host, done, jpegs, pngs)
+    return payload, table, (host, done, (jpegs, pngs, jpegps))
 
   def finish(self, payload: torch.Tensor, handle) -> None:
     if handle is None:
       return
-    host, done, jpegs, pngs = handle
+    host, done, groups = handle
     done.synchronize()
     torch.cuda.current_stream(self.device).wait_event(done)
     status = host.clone()
-    nj = len(jpegs.paths) if jpegs is not None else 0
-    if jpegs is not None:
-      _redecode(payload, status[:nj], jpegs)
-    if pngs is not None:
-      _redecode(payload, status[nj:], pngs)
+    at = 0
+    for files in groups:                       # the groups' statuses follow one another, as start decoded them
+      if files is not None:
+        _redecode(payload, status[at:at + len(files.paths)], files)
+        at += len(files.paths)
 
 
 def _produce_batch(paths: Sequence[str], batch_size: int, pool: ThreadPoolExecutor):
-  """(tensors, (count, jpegs, pngs)) of one batch for Translator.run: PIL decodes the files the device does not."""
-  from . import jpeg, ops, png
+  """(tensors, (count, jpegs, pngs, jpegps)) of one batch for Translator.run: PIL decodes the files the device does
+  not."""
+  from . import jpeg, jpeg_progressive, ops, png
   blobs = list(pool.map(_read, paths))
   kinds = list(pool.map(_device_file, blobs))
   host = [i for i, k in enumerate(kinds) if k is None]
@@ -239,7 +263,7 @@ def _produce_batch(paths: Sequence[str], batch_size: int, pool: ThreadPoolExecut
   payload, table_t = torch.from_numpy(payload), torch.from_numpy(table)
   ops.check_table(table_t, payload.numel())
   tensors, files = (payload, table_t), []
-  for kind in ('jpeg', 'png'):
+  for kind in DEVICE_KINDS:
     dev = [i for i, k in enumerate(kinds) if k is not None and k[0] == kind]
     if not dev:
       files.append(None)
@@ -249,10 +273,14 @@ def _produce_batch(paths: Sequence[str], batch_size: int, pool: ThreadPoolExecut
       b = jpeg.pack(*args)
       tensors += tuple(torch.from_numpy(a) for a in (b.data, b.segs, b.comps, b.images, b.qt, b.huff))
       sizes = (b.blocks, b.plane_bytes, b.pixels)
-    else:
+    elif kind == 'png':
       b = png.pack(*args)
       tensors += tuple(torch.from_numpy(a) for a in (b.data, b.images, b.palettes))
       sizes = (b.raw_bytes, b.pixels)
+    else:
+      b = jpeg_progressive.pack(*args)
+      tensors += tuple(torch.from_numpy(a) for a in (b.data, b.segs, b.scans, b.comps, b.images, b.qt, b.huff))
+      sizes = (b.blocks, b.plane_bytes, b.pixels, b.levels)
     files.append(_DeviceFiles([paths[i] for i in dev], [tuple(int(v) for v in table[i]) for i in dev], sizes))
   return tensors, (len(paths),) + tuple(files)
 
@@ -346,7 +374,7 @@ def _padded_batches(images: Sequence[np.ndarray], batch_size: int):
     payload, table = ops.pack_images(chunk)
     if len(chunk) < batch_size:
       table = torch.cat([table, table[-1:].expand(batch_size - len(chunk), 3)], 0)
-    yield (payload, table), (len(chunk), None, None)
+    yield (payload, table), (len(chunk), None, None, None)
 
 
 class Translator(object):
@@ -369,9 +397,10 @@ class Translator(object):
     self.decoder = _DeviceDecoder(model.device, self.DECODE_AHEAD) if self.back.cuda else None
 
   def run(self, host_batches, jpeg_rows=None):
-    """host_batches: iterable of (tensors, (count, jpegs, pngs)): tensors = (payload, table) host tensors, followed by
-    the six descriptor tensors of a jpeg.Batch when `jpegs` (a _DeviceFiles) names JPEG images the device decodes, then
-    the three of a png.Batch when `pngs` names PNG images.  Yields the first
+    """host_batches: iterable of (tensors, (count, jpegs, pngs, jpegps)): tensors = (payload, table) host tensors,
+    followed by the six descriptor tensors of a jpeg.Batch when `jpegs` (a _DeviceFiles) names JPEG images the device
+    decodes, then the three of a png.Batch when `pngs` names PNG images, then the seven of a jpeg_progressive.Batch when
+    `jpegps` names progressive JPEG images.  Yields the first
     `count` translated images of each batch.  With `jpeg_rows` (per batch, `count` booleans), yields (images or None,
     {row: JPEG scan bytes}) instead: the marked rows are encoded on the device, and the images come back only when
     some row is not marked.  From the first batch with files the device decodes, the batches go through the decoder
@@ -392,11 +421,11 @@ class Translator(object):
       """(k, n, payload, table, staged): the batches in order, each once its images are in its payload; `staged`: the
       payload is the prefetcher's slot, to be released once the batch has been enqueued."""
       for k, batch in enumerate(feed):
-        n, jpegs, pngs = counts.popleft()
-        if jpegs is None and pngs is None and not decoding:
+        n, jpegs, pngs, jpegps = counts.popleft()
+        if jpegs is None and pngs is None and jpegps is None and not decoding:
           yield k, n, batch[0], batch[1], True
           continue
-        decoding.append((k, n) + self.decoder.start(batch[0], batch[1], batch[2:], jpegs, pngs))
+        decoding.append((k, n) + self.decoder.start(batch[0], batch[1], batch[2:], jpegs, pngs, jpegps))
         feed.release()                           # start copied the batch out of its slot
         while len(decoding) > self.DECODE_AHEAD:
           k0, n0, payload, table, handle = decoding.popleft()
